@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the xrdslam render-and-optimise hot path on B200.
+"""Benchmark of the xrdslam render-and-optimise hot path on H100.
 
     python bench.py [--config coslam|nice|vox|point] --gpus N --steps K --warmup W
-                    [--impl reference] [--scaling weak|strong]
+                    [--impl reference] [--scaling weak|strong] [--dump-outputs DIR]
 
 --config selects the BASELINE.json configuration: coslam = cfg 2 (the default: the
 configuration the headline metric is quoted on), vox = cfg 3, nice = cfg 4 (cfg 1 is its
@@ -24,6 +24,12 @@ forward + loss + backward on the GPU (incl. the smoothness term), optimizer step
   N > 1   mapping rays are sharded: every rank owns a fixed 4096-ray batch
           (weak scaling), one NCCL all-reduce over the flat gradient bucket
           (hash table + MLP) per iteration, Adam replicated.
+
+--dump-outputs DIR writes what the last timed step computed (its loss, the optimised parameters
+and poses) as DIR/<name>.npy, float32 or float64, at most 64 MB in all; arrays above 2 M
+elements (or above what is left of the 64 MB) are replaced by a fixed, seeded sample of their
+elements (<name>.npy flat, with <name>.idx.npy holding the flat indices as float64).  The inputs are seeded, so two builds of the project
+run with the same arguments can be compared output for output.
 
 --impl reference times the CPU oracle port (torch, all host threads) of the same
 step on rank 0 -- the reference's own code cannot travel to the GPU box (python
@@ -68,7 +74,43 @@ def parse():
                     help='N > 1: weak = fixed rays per GPU, strong = the single-GPU batch split over N')
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-torch-gpu-baseline', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step as DIR/<name>.npy')
     return ap.parse_args()
+
+
+DUMP_BUDGET = 64 * 1024 * 1024
+DUMP_SAMPLE = 1 << 21  # elements kept of a larger array (seeded, the same on every run)
+
+
+def dump_outputs(out_dir, arrays):
+    """arrays: (name, tensor) pairs, written in order as float32 (float64 stays float64).  An
+    array above DUMP_SAMPLE elements, or above what is left of the budget, is replaced by a
+    seeded sample of its flat elements, with the flat indices beside it (<name>.idx.npy, as
+    float64: exact below 2^53)."""
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_BUDGET
+    for i, (name, t) in enumerate(arrays):
+        a = t.detach()
+        a = (a.double() if a.dtype == torch.float64 else a.float()).cpu()
+        share = left // (len(arrays) - i)  # what later arrays are guaranteed
+        keep = min(a.numel(), DUMP_SAMPLE, share // a.element_size())
+        if keep < a.numel():
+            keep = min(keep, share // (a.element_size() + 8))
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.numel(), generator=g)[:keep].sort().values
+            a = a.reshape(-1)[idx]
+            np.save(os.path.join(out_dir, name + '.idx.npy'), idx.double().numpy())
+            left -= idx.numel() * 8
+        np.save(os.path.join(out_dir, name + '.npy'), a.numpy())
+        left -= a.numel() * a.element_size()
+
+
+def frame_poses(frames):
+    """Every parameter of each frame's pose, whatever its representation (axis-angle or
+    quaternion, rotation and translation separate or joined), concatenated per frame."""
+    return [('poses', torch.stack([torch.cat([p.detach().reshape(-1) for p in f.pose.parameters()])
+                                   for f in frames]))]
 
 
 # ------------------------------------------------------------------ clocks ---
@@ -154,17 +196,6 @@ def build_algorithm(device, seed):
                 separate_LR=True, rot_rep='axis_angle')
     algo.set_initialized()
     return algo, kfs, cur
-
-
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of one 4096-ray k_fused launch from the
-    committed `ncu --set full` capture of this round (profiles/r02_coslam_kfused_traffic.json,
-    written by scripts/ncu_summary.py); None when no capture of the current kernel exists."""
-    try:
-        d = json.load(open(os.path.join(ROOT, 'profiles', 'r02_coslam_kfused_traffic.json')))
-        return int(d['dram_bytes_read'] + d['dram_bytes_write'])
-    except Exception:
-        return None
 
 
 def flat_params(model):
@@ -308,12 +339,18 @@ def run_ours(args):
     barrier()
     t0 = time.perf_counter()
     for i in range(K):
-        flush.zero_()  # L2 flush (256 MB > 126 MB L2), outside the timed events
+        flush.zero_()  # L2 flush (256 MB > 50 MB L2), outside the timed events
         ev[i][0].record()
-        run_step(W + i)
+        last = run_step(W + i)
         ev[i][1].record()
     barrier()
     wall = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        poses = ([('poses', torch.cat([sess.rot, sess.trans], 1))] if use_graph
+                 else frame_poses(frames))
+        dump_outputs(args.dump_outputs,
+                     [('loss', last.reshape(1)), ('embed_fn.params', model.embed_fn.params)] +
+                     [('decoder.' + n, p) for n, p in model.decoder.named_parameters()] + poses)
     ms = sum(a.elapsed_time(b) for a, b in ev)
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
@@ -349,18 +386,17 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak = float(peaks.get('hbm_gbs', 6650.0))
+    peak = float(peaks.get('hbm_gbs', 3350.0))
     achieved = R * BYTES_PER_RAY / (k_ms * 1e-3) / 1e9
     roofline = {'bound': 'hbm', 'kernel': 'xrd::coslam::k_fused_g<true> (grouped persistent fused kernel)',
                 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
                 'frac': achieved / peak,
-                'peak_source': 'measured (MEASURED_PEAKS.json)' if peaks else 'fallback 6650',
-                # dram__bytes_read.sum + dram__bytes_write.sum of one 4096-ray launch
-                # (ncu --set full, profiles/r02_coslam_fused_g_4096rays_ncu.txt)
-                'traffic': ncu_traffic(), 'kernel_ms': k_ms,
+                'peak_source': ('measured (MEASURED_PEAKS.json)' if peaks else
+                                'fallback 3350 (H100 SXM data sheet)'),
+                'kernel_ms': k_ms,
                 'algorithmic_bytes_per_launch': R * BYTES_PER_RAY,
                 'note': 'table (6.56 MB) is L2-resident: DRAM traffic is far below '
-                        'the algorithmic bytes, see profiles/'}
+                        'the algorithmic bytes'}
 
     # ---------------- e2e: through the plugin, host ray bank ---------------
     algo.config.min_sample_pixels = map_cur
@@ -491,7 +527,7 @@ def _finish(world):
 # ------------------------------------------------------------ CPU baseline ---
 def coslam_ref_step_factory(R_bank, R_cur, device='cpu'):
     """One Co-SLAM mapping iteration of the oracle port (fwd + bwd + Adam) on `device`, on the
-    SAME workload as the B200 arm: the keyframe ray bank and the per-iteration sampler are
+    SAME workload as the GPU arm: the keyframe ray bank and the per-iteration sampler are
     CoSLAM.get_model_input's own host path (random.sample rows of the bank + current-frame
     pixels, per-ray pose gather), R_bank + R_cur rays, smoothness term, Adam on table +
     decoder."""
@@ -560,14 +596,14 @@ def cpu_baseline(iters=2):
     return {'value': R * iters / dt, 'unit': 'rays/s', 'cores': cores,
             'kind': 'port',
             'sample': f'{iters} mapping iterations x {R} rays x 43 samples, same sampler and '
-                      'batch as the B200 arm (oracle/coslam.py torch-CPU port incl. smoothness '
+                      'batch as the GPU arm (oracle/coslam.py torch-CPU port incl. smoothness '
                       '+ Adam)',
             'ms_per_iter': dt / iters * 1e3}
 
 
 def torch_gpu_baseline(dev, iters=10):
     """The restated reference PyTorch path (oracle/coslam.py: restated-tcnn hash grid + OneBlob
-    in torch ops, autograd, torch Adam) run on the B200 itself -- BASELINE.md section 5's
+    in torch ops, autograd, torch Adam) run on the same GPU -- BASELINE.md section 5's
     'reference PyTorch path on the GPU', what north_star's >= 10x is quoted against."""
     try:
         step = coslam_ref_step_factory(MAP_KF, MAP_CUR, device=str(dev))
@@ -597,9 +633,8 @@ def run_reference(args):
     R = MAP_KF + MAP_CUR
     step = coslam_ref_step_factory(MAP_KF, MAP_CUR)
     cores = pick_threads(step)
-    K = min(args.steps, 10)
-    W = min(args.warmup, 2)
-    for _ in range(max(W, 1)):
+    K, W = args.steps, args.warmup
+    for _ in range(W):
         step()
     t0 = time.perf_counter()
     for _ in range(K):
@@ -612,12 +647,12 @@ def run_reference(args):
         'value': v, 'unit': 'rays/s', 'n_gpus': int(os.environ.get('WORLD_SIZE', '1')),
         'steps': K, 'warmup': W, 'ms_per_step': dt / K * 1e3, 'higher_is_better': True,
         'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
-        # same workload, same batch, same sampler as the B200 arm; fewer steps
+        # same workload, same batch, same sampler as the GPU arm
         'config': {'workload': WORKLOAD, 'rays_per_step_per_gpu': R,
                    'precision': 'fp32 (torch CPU)',
                    'sample': f'{K} full steps of {R} rays (same frames, ray bank, sampler, decoder, '
-                             'losses, smoothness, Adam); the reference\'s own python cannot run on '
-                             'the box (py3.12 + tinycudann absent): CPU oracle port, all host threads'},
+                             'losses, smoothness, Adam); the reference\'s own python does not run '
+                             'under py3.12 without tinycudann: CPU oracle port, all host threads'},
         'cpu_baseline': {'value': v, 'unit': 'rays/s', 'cores': cores, 'kind': 'port',
                          'sample': f'{K} steps x {R} rays'},
         'e2e': {'value': v, 'unit': 'rays/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
@@ -676,10 +711,15 @@ def run_workload(args):
     for i in range(K):
         flush.zero_()  # L2 flush between timed steps (outside the events)
         ev[i][0].record()
-        wl.step(sched[i])
+        last = wl.step(sched[i])
         ev[i][1].record()
     barrier()
     wall = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs,
+                     [('loss', last.reshape(1))] +
+                     [(n, p) for n, p in wl.algo.model.named_parameters()] +
+                     frame_poses(wl.frames))
     ms = sum(a.elapsed_time(b) for a, b in ev)
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
@@ -704,10 +744,10 @@ def run_workload(args):
     k_ms = float(np.median(kms))
     if args.config == 'vox':
         n_pts = int(wl.algo.model.last_march.get('n_points', 0)) or None
-        roofline = wl.kernel_roofline(k_ms, float(peaks.get('bf16_tflops_sustained', 1400.0)),
+        roofline = wl.kernel_roofline(k_ms, float(peaks.get('bf16_tflops_sustained', 989.0)),
                                       n_pts or 1)
     else:
-        roofline = wl.kernel_roofline(k_ms, float(peaks.get('hbm_gbs', 6650.0)))
+        roofline = wl.kernel_roofline(k_ms, float(peaks.get('hbm_gbs', 3350.0)))
     roofline['peak_source'] = 'measured (MEASURED_PEAKS.json)' if peaks else 'fallback'
 
     # ---- e2e through the plugin call
@@ -775,7 +815,7 @@ def cpu_baseline_workload(wl, budget_s=20.0):
     dt = time.perf_counter() - t0
     return {'value': R * n / dt, 'unit': 'rays/s', 'cores': cores, 'kind': 'port',
             'sample': f'{n} mapping iterations x {R} rays, same frames / window / batch as the '
-                      f'B200 arm: {what}', 'ms_per_iter': dt / n * 1e3}
+                      f'GPU arm: {what}', 'ms_per_iter': dt / n * 1e3}
 
 
 def run_reference_workload(args):
@@ -786,7 +826,9 @@ def run_reference_workload(args):
         wl.build()  # the map (octree / point cloud) is built by the product's own maintenance code
     step, R, what = wl.cpu_step_factory()
     cores = pick_threads(step)
-    K = max(1, min(args.steps, 5))
+    K = args.steps
+    for _ in range(args.warmup):
+        step()
     t0 = time.perf_counter()
     for _ in range(K):
         step()
@@ -794,7 +836,7 @@ def run_reference_workload(args):
     v = R * K / dt
     print(json.dumps({
         'impl': 'reference', 'metric': wl.metric, 'value': v, 'unit': 'rays/s',
-        'n_gpus': int(os.environ.get('WORLD_SIZE', '1')), 'steps': K, 'warmup': 2,
+        'n_gpus': int(os.environ.get('WORLD_SIZE', '1')), 'steps': K, 'warmup': args.warmup,
         'ms_per_step': dt / K * 1e3, 'higher_is_better': True, 'scaling': 'weak',
         'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
         'config': {'workload': wl.workload, 'rays_per_step_per_gpu': R,

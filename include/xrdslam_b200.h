@@ -1,15 +1,15 @@
 /*
- * xrdslam_b200 -- C-ABI of the B200-native render-and-optimise hot path.
+ * xrdslam_b200 -- C-ABI of the H100-native render-and-optimise hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Every entry point is
  * `extern "C"`, takes plain pointers / sizes / POD structs, never allocates,
  * never frees, never synchronises the stream: one call = an asynchronous enqueue
- * of sm_100a kernels on `stream` (a cudaStream_t passed as void*).  All buffers,
+ * of sm_90a kernels on `stream` (a cudaStream_t passed as void*).  All buffers,
  * including the workspace, are owned by the caller (torch on the Python side).
  * Return value: XRD_OK (0) or a negative XrdStatus.  No exceptions, no exit().
  *
- * What each entry point replaces in the reference (paths relative to
- * /root/reference, commit f0366f20):
+ * What each entry point replaces in the reference (paths relative to the
+ * xrdslam repository, commit f0366f20):
  *
  *   xrd_coslam_step        slam/models/joint_encoding.py:158-163  get_outputs
  *                          -> render_rays :250-344, run_network :483-507,
@@ -44,7 +44,7 @@ extern "C" {
 typedef enum {
   XRD_OK = 0,
   XRD_E_SHAPE = -1,     /* inconsistent sizes / unsupported configuration   */
-  XRD_E_ARCH = -2,      /* device is not sm_100                              */
+  XRD_E_ARCH = -2,      /* device is not sm_90                               */
   XRD_E_WORKSPACE = -3, /* workspace too small                               */
   XRD_E_NOHIT = -4,     /* Vox-Fusion: no ray hit any voxel (reference: None) */
   XRD_E_CUDA = -5,      /* a CUDA runtime call failed (see xrd_last_cuda_error) */
@@ -654,11 +654,11 @@ typedef struct {
 
 /* Measurement / parity hook: arithmetic of the wide-MLP GEMMs (Point-SLAM colour stage and
  * the Vox-Fusion decoder):
- * 0 = fp32 SIMT, 1 = 3xTF32 tensor cores (default, fp32-level accuracy): tcgen05 / TMEM / TMA
+ * 0 = fp32 SIMT, 1 = 3xTF32 tensor cores (default, fp32-level accuracy): wgmma / TMA
  * kernel where the shape qualifies, mma.sync otherwise, 2 = plain TF32 (mma.sync),
  * 3 = 3xTF32 on mma.sync only.  Thread-local, like the error state. */
 int xrd_debug_gemm_mode(int mode);
-/* bring-up hook of the tcgen05 GEMM (descriptor field variants); 0 = production */
+/* bring-up hook of the wgmma GEMM (bit 0 swaps the descriptor strides); 0 = production */
 int xrd_debug_gemm_variant(int variant);
 
 /* The wide-MLP GEMM itself (unit tests): C[m][n] = act(sum_k A(m,k) B[k][n] + bias[m]) with

@@ -2,7 +2,7 @@
 
   oracle/_ref/svo.so    third_party/sparse_octree (CPU C++, TorchScript class svo.Octree)
   oracle/_ref/grid.so   third_party/sparse_voxels (CUDA ext `grid`: svo_intersect,
-                        inverse_cdf_sampling, ...) cross-compiled for sm_100a
+                        inverse_cdf_sampling, ...) cross-compiled for sm_90a
 
 Sources are compiled where they lie under /root/reference (never copied); outputs go only to
 oracle/_ref/ (git-ignored, NOT gpurun-ignored: the .so files travel to the GPU box, where
@@ -28,7 +28,7 @@ def _build(name, sources, includes, cuda):
             os.path.getmtime(target) >= os.path.getmtime(s) for s in sources):
         return target
     from torch.utils.cpp_extension import load
-    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '10.0a')
+    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '9.0a')
     bdir = os.path.join(OUT, 'build_' + name)
     os.makedirs(bdir, exist_ok=True)
     load(name=name, sources=sources, extra_include_paths=includes,

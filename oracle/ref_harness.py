@@ -134,6 +134,34 @@ def copy_nice_ref_to_oracle(ref, ora):
             ora.grids['grid_coarse'].copy_(ref.grid_c['grid_coarse'])
 
 
+def copy_nice_oracle_to_ref(ora, ref):
+    """The reverse of copy_nice_ref_to_oracle: oracle.nice.NiceOracle parameters and grids
+    into a reference ConvOnet."""
+    import torch
+    with torch.no_grad():
+        for name in ('middle', 'fine', 'color'):
+            r = getattr(ref.decoder, name + '_decoder')
+            o = getattr(ora, name)
+            r.embedder._B.copy_(o.B)
+            for i in range(5):
+                r.fc_c[i].weight.copy_(o.fc_c[i].weight)
+                r.fc_c[i].bias.copy_(o.fc_c[i].bias)
+                r.pts_linears[i].weight.copy_(o.pts[i].weight)
+                r.pts_linears[i].bias.copy_(o.pts[i].bias)
+            r.output_linear.weight.copy_(o.out.weight)
+            r.output_linear.bias.copy_(o.out.bias)
+        for k in ('grid_middle', 'grid_fine', 'grid_color'):
+            ref.grid_c[k] = ora.grids[k].detach().clone()
+        if getattr(ora, 'coarse', None) is not None:
+            r, o = ref.decoder.coarse_decoder, ora.coarse
+            for i in range(5):
+                r.pts_linears[i].weight.copy_(o.pts[i].weight)
+                r.pts_linears[i].bias.copy_(o.pts[i].bias)
+            r.output_linear.weight.copy_(o.out.weight)
+            r.output_linear.bias.copy_(o.out.bias)
+            ref.grid_c['grid_coarse'] = ora.grids['grid_coarse'].detach().clone()
+
+
 # ---- Point-SLAM: the reference's ConvOnet2 with an exact-kNN stand-in for faiss -----------
 class _ExactIndex:
     """Minimal faiss.Index stand-in: exact L2 search (the real IndexIVFFlat(nlist 400,

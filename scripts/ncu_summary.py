@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (read here, no GPU) into a small text file for profiles/."""
+"""Summarise an .ncu-rep (read here, no GPU) into a small text file."""
 import csv, subprocess, sys, io
 rep, out = sys.argv[1], sys.argv[2]
 raw = subprocess.run(['ncu', '-i', rep, '--page', 'raw', '--csv'], capture_output=True, text=True).stdout

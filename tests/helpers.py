@@ -1,4 +1,6 @@
 """Shared builders for the parity tests (oracle <-> CUDA path)."""
+import os
+
 import numpy as np
 import torch
 
@@ -20,7 +22,7 @@ def make_rays(R, seed=0, zero_depth_every=7):
 
 
 def coslam_pair(device, table_amp=0.3, seed=1, **cfg):
-    """(oracle on CPU, B200 model on device) with identical parameters."""
+    """(oracle on CPU, CUDA model on device) with identical parameters."""
     from oracle.coslam import CoslamOracle
     from xrdslam_b200.camera import Camera
     from xrdslam_b200.joint_encoding import JointEncodingConfig
@@ -76,7 +78,7 @@ def load_golden_coslam():
 
 
 def set_coslam_params(obj, g, kind):
-    """Load golden parameters into an oracle (kind='oracle') or B200 model."""
+    """Load golden parameters into an oracle (kind='oracle') or CUDA model."""
     with torch.no_grad():
         t = lambda k: torch.from_numpy(g[k])
         if kind == 'oracle':
@@ -104,7 +106,7 @@ def load_golden_nice():
 
 
 def nice_from_golden(g, kind, device=None):
-    """Build an oracle (kind='oracle') or B200 model from the golden parameters."""
+    """Build an oracle (kind='oracle') or CUDA model from the golden parameters."""
     t = lambda k: torch.from_numpy(g[k])
     if kind == 'oracle':
         from oracle.nice import NiceOracle
@@ -149,7 +151,7 @@ def load_golden_pointslam():
 
 
 def pointslam_from_golden(g, kind, device=None):
-    """Oracle (kind='oracle') or B200 ConvOnet2 with the golden decoder + point cloud."""
+    """Oracle (kind='oracle') or CUDA ConvOnet2 with the golden decoder + point cloud."""
     t = lambda k: torch.from_numpy(g[k])
     pre = 'dec.'
     if kind == 'oracle':
@@ -209,4 +211,30 @@ def oracle_cdec_grads(ora):
         out[f'mlp_col_neighbor.{name}.weight'] = lin.weight.grad
         out[f'mlp_col_neighbor.{name}.bias'] = lin.bias.grad
     out['output_linear.weight'], out['output_linear.bias'] = c.out.weight.grad, c.out.bias.grad
+    return out
+
+
+# ---- outputs of the original project's own code, recorded by tests/golden/make_golden_live.py
+REFERENCE_LIVE = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden',
+                              'reference_live.npz')
+
+
+def digest(*ts):
+    """SHA-256 over dtype, shape and bytes of each tensor / array (exact-equality checks of
+    outputs too large to store)."""
+    import hashlib
+    h = hashlib.sha256()
+    for t in ts:
+        a = t.detach().cpu().contiguous().numpy() if torch.is_tensor(t) else np.ascontiguousarray(t)
+        h.update(f'{a.dtype}{a.shape}'.encode())
+        h.update(a.tobytes())
+    return h.hexdigest()
+
+
+def reference_live(case):
+    """{key: array} the original project returned for `case`."""
+    z = np.load(REFERENCE_LIVE)
+    pre = case + '/'
+    out = {k[len(pre):]: z[k] for k in z.files if k.startswith(pre)}
+    assert out, f'no recorded reference outputs for {case}'
     return out

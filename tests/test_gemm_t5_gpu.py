@@ -1,4 +1,4 @@
-"""The Blackwell-native GEMM (csrc/gemm_t5.cuh: tcgen05.mma kind::tf32 + TMEM + TMA, 3xTF32)
+"""The Hopper-native GEMM (csrc/gemm_t5.cuh: wgmma.mma_async tf32 + TMA + mbarrier, 3xTF32)
 against float64 matmul and against the mma.sync path, on the shapes of the Vox-Fusion decoder and
 the Point-SLAM colour trunk (forward and transposed-weight backward GEMMs, ragged N, masks)."""
 import pytest
@@ -46,7 +46,7 @@ def run(dev, M, N, K, transA, act, mode, mask=False, addend=False, seed=0):
     (128, 5000, 16, 0, 1),       # vox layer 0 (K = 16, ragged N)
     (128, 1111, 144, 0, 1),      # colour layer: K = 144 -> two-stage pipeline
     (128, 2048, 129, 1, 0),      # backward through sdf_out (transposed weights, K = 129)
-    (144, 3000, 128, 1, 0),      # 144 rows = 128 (tcgen05) + 16 (mma.sync)
+    (144, 3000, 128, 1, 0),      # 144 rows = 128 (wgmma) + 16 (mma.sync)
     (64, 1024, 128, 0, 3),       # M < 128 (zero-padded rows)
     (32, 3000, 128, 0, 0),       # Point-SLAM 128 -> 32 neighbour layer
     (128, 150000, 128, 0, 1),    # benchmark-sized point count
@@ -65,8 +65,8 @@ def test_gemm_t5_mask_and_addend(cuda_dev):
     assert (got - ref).abs().max().item() < 5e-6 * max(1.0, ref.abs().max().item())
 
 
-def test_gemm_t5_sass_is_blackwell_native():
-    """The shipped library contains tcgen05 MMAs, TMEM loads and TMA loads (SASS mnemonics)."""
+def test_gemm_t5_sass_is_hopper_native():
+    """The shipped library contains warpgroup MMAs, TMA loads and mbarrier waits (SASS mnemonics)."""
     import os
     import shutil
     import subprocess
@@ -75,12 +75,12 @@ def test_gemm_t5_sass_is_blackwell_native():
     if not os.path.exists(cuobjdump):
         pytest.skip('cuobjdump not available')
     sass = subprocess.run([cuobjdump, '-sass', LIB_PATH], capture_output=True, text=True).stdout
-    for mn in ('UTCHMMA', 'LDTM', 'UTMALDG'):
+    for mn in ('HGMMA.64x128x8.F32.TF32', 'UTMALDG', 'SYNCS.PHASECHK'):
         assert mn in sass, mn
 
 
 def test_gemm_t5_softplus_epilogue(cuda_dev):
-    """Point-SLAM trunk epilogue: nn.Softplus(beta=100) on the SFU in the tcgen05 kernel."""
+    """Point-SLAM trunk epilogue: nn.Softplus(beta=100) in the wgmma kernel."""
     from xrdslam_b200 import _cabi
     lib = _cabi.lib()
     g = torch.Generator().manual_seed(3)

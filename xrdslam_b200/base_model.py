@@ -5,7 +5,7 @@ py3.12-safe: the reference's dataclass-instance defaults do not import on python
 
 A Model owns the map parameters and launches the fused CUDA step; the Algorithm (algorithm.py)
 drives it through exactly four calls: ``forward(input)``, ``get_loss_dict(...)``,
-``get_param_groups()`` and -- B200 additions -- the two switches below."""
+``get_param_groups()`` and -- CUDA-path additions -- the two switches below."""
 from __future__ import annotations
 
 from dataclasses import dataclass, field

@@ -1,4 +1,4 @@
-"""Build libxrdslam_b200.so (the C-ABI shared library) in-tree with nvcc for sm_100a.
+"""Build libxrdslam_b200.so (the C-ABI shared library) in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m xrdslam_b200.build [--force] [--verbose]
 The library carries no torch dependency: plain CUDA runtime + the C-ABI in
@@ -18,7 +18,7 @@ LIB_DIR = os.path.join(HERE, 'lib')
 LIB_PATH = os.path.join(LIB_DIR, 'libxrdslam_b200.so')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
     '-std=c++17', '--expt-relaxed-constexpr', '-Xcompiler', '-fPIC', '-I',
     os.path.join(ROOT, 'include'), '-I', CSRC
 ]
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             raise RuntimeError(f'nvcc failed on {src}')
     cmd = [nvcc, '-shared', '-o', LIB_PATH] + objs + [
-        '-gencode', 'arch=compute_100a,code=sm_100a', '-lcudart'
+        '-gencode', 'arch=compute_90a,code=sm_90a', '-lcudart'
     ]
     subprocess.check_call(cmd)
     return LIB_PATH

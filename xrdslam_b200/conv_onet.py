@@ -1,4 +1,4 @@
-"""NICE-SLAM model behind the reference's ``Model`` plugin surface, B200-native.
+"""NICE-SLAM model behind the reference's ``Model`` plugin surface, H100-native.
 
 Host-side mirror of slam/models/conv_onet.py (reference @ f0366f20): same class / config
 field names, same ``forward / get_loss_dict / get_param_groups`` signatures, same
@@ -203,7 +203,7 @@ class ConvOnet(Model):
         cfg = self.config
         if cfg.rendering_n_importance or cfg.rendering_perturb or \
                 cfg.rendering_lindisp or not cfg.occupancy:
-            raise NotImplementedError('B200 path covers the reference nice-slam config: '
+            raise NotImplementedError('CUDA path covers the reference nice-slam config: '
                                       'occupancy, no importance sampling / perturbation')
         self.bounding_box = torch.as_tensor(np.asarray(self.bounding_box),
                                             dtype=torch.float64).clone()

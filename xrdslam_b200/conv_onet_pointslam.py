@@ -1,4 +1,4 @@
-"""Point-SLAM model behind the reference's ``Model`` plugin surface, B200-native.
+"""Point-SLAM model behind the reference's ``Model`` plugin surface, H100-native.
 
 Host-side mirror of slam/models/conv_onet_pointslam.py (class ConvOnet2, same config fields,
 ``forward / get_loss_dict / get_param_groups`` signatures, groups ``decoder``, ``geometry``,
@@ -182,7 +182,7 @@ class ConvOnet2(Model):
         cfg = self.config
         if not cfg.use_dynamic_radius or cfg.pointcloud_nn_weighting != 'distance' or \
                 cfg.rendering_sample_near_pcl or cfg.model_encode_exposure:
-            raise NotImplementedError('B200 path covers the reference point-slam config')
+            raise NotImplementedError('CUDA path covers the reference point-slam config')
         self.decoder = POINT(cfg.model_c_dim)
         self.load_pretrain()
         self.neural_point_cloud = None

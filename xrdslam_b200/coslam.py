@@ -1,6 +1,6 @@
 """Co-SLAM algorithm (host-side mirror of slam/algorithms/coslam.py): global
 keyframe ray bank, per-ray pose gather for bundle adjustment, persistent model
-optimizers -- driving the fused B200 step in joint_encoding.py."""
+optimizers -- driving the fused CUDA step in joint_encoding.py."""
 from __future__ import annotations
 
 import functools
@@ -60,7 +60,7 @@ class CoSLAMConfig(AlgorithmConfig):
     mapping_bound: List[List[float]] = field(
         default_factory=lambda: [[-3, 3], [-4, 2.5], [-2, 2.5]])
     optimizers: Dict[str, Any] = field(default_factory=_coslam_optimizers)
-    # B200: run the mapping iterations as one CUDA graph each (coslam_graph.py)
+    # run the mapping iterations as one CUDA graph each (coslam_graph.py)
     graph_mapping: bool = True
 
 

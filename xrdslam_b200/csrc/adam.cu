@@ -90,7 +90,7 @@ extern "C" int xrd_adam_step(const XrdAdamTensor* tensors, int n_tensors, int ze
     }
     long long bx = (nmax / 4 + 255) / 256;
     if (bx < 1) bx = 1;
-    if (bx > 148 * 8) bx = 148 * 8;
+    if (bx > num_sms() * 8) bx = num_sms() * 8;
     adam::k_adam<<<dim3((unsigned)bx, (unsigned)A.n), 256, 0, (cudaStream_t)stream>>>(A);
     XRD_LAUNCH_CHECK();
   }

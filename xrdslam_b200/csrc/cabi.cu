@@ -14,11 +14,11 @@ namespace t5 { thread_local int g_t5_variant = 0; }
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -50,7 +50,10 @@ extern "C" int xrd_check_device(int dev) {
   int major = 0;
   cudaError_t e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   if (e != cudaSuccess) return xrd::cuda_fail(e);
-  return major == 10 ? XRD_OK : XRD_E_ARCH;
+  int minor = 0;
+  e = cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (e != cudaSuccess) return xrd::cuda_fail(e);
+  return (major == 9 && minor == 0) ? XRD_OK : XRD_E_ARCH;
 }
 
 // ATen's CPU linspace (aten/src/ATen/native/cpu/RangeFactoriesKernel.cpp): float step,

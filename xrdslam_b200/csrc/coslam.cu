@@ -1,4 +1,4 @@
-// Co-SLAM render-and-optimise step, fused forward + backward (sm_100a).
+// Co-SLAM render-and-optimise step, fused forward + backward (sm_90a).
 //
 // Replaces (reference @ f0366f20): slam/models/joint_encoding.py:250-344
 // render_rays, :483-507 run_network, :463-481 query_color_sdf (tcnn HashGrid +
@@ -314,7 +314,7 @@ __device__ __forceinline__ void encode_point(const Params& P, const Lv* __restri
 }
 
 // NL (point, level) items of the hash backward per call (scatter (g0,g1), optional d/dx).
-// Deliberately not inlined: instruction-cache footprint matters for this kernel (profiles/).
+// Deliberately not inlined: instruction-cache footprint matters for this kernel.
 // NL (point, level) items per call: the 8 NL corner loads of all levels are issued before any
 // is consumed (the kernel runs at 7 warps/SM, so memory-level parallelism has to come from
 // within the thread), then the 8 NL scatters.  on[h]: item present (level exists and its
@@ -1889,8 +1889,7 @@ using namespace xrd::coslam;
 
 // Optional Jacobian cache of the grouped kernel (2 halves x 8 levels x 6 floats per sample point):
 // the forward gather stores d feat / d xn so that the backward needs no second gather for the ray
-// gradients.  Measured on B200 (profiles/r02_coslam_kernel_ab.txt) it LOSES 2-4 % against
-// re-gathering (the table is L2-resident, the cache is 384 B/point of extra traffic), so it is
+// gradients.  The table is L2-resident and the cache is 384 B/point of extra traffic, so it is
 // off unless XRD_COSLAM_JAC is set; kept for tables that outgrow L2.
 static constexpr size_t kJacBytesPerPoint = 2 * 48 * sizeof(float);
 static constexpr size_t kJacMaxBytes = (size_t)512 << 20;  // beyond this the backward re-gathers

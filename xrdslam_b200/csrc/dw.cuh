@@ -318,7 +318,7 @@ static inline cudaError_t launch_dw(DwParams& Q, cudaStream_t stream) {
     else k_dw_tc<true><<<grid, 256, DW_SMEM, stream>>>(G);
     return cudaGetLastError();
   }
-  const long long want = 4LL * 148;
+  const long long want = 4LL * num_sms();
   long long chunks = (want + Q.n_jobs - 1) / Q.n_jobs;
   if (chunks < 1) chunks = 1;
   long long chunk = ((long long)Q.P + chunks - 1) / chunks;

@@ -256,10 +256,10 @@ static __global__ void __launch_bounds__(256, 2) k_gemm_tc(const GemmArgs G) {
 
 // Arithmetic of the wide-MLP GEMMs (xrd_debug_gemm_mode, cabi.cu):
 //   0 = fp32 SIMT (k_gemm)
-//   1 = 3xTF32 tensor cores (default): tcgen05 / TMEM / TMA kernel (gemm_t5.cuh) for the shapes
-//       it takes, mma.sync k_gemm_tc<true> for the rest
+//   1 = 3xTF32 tensor cores (default): wgmma / TMA kernel (gemm_t5.cuh) for the shapes it
+//       takes, mma.sync k_gemm_tc<true> for the rest
 //   2 = plain TF32 mma.sync (k_gemm_tc<false>)
-//   3 = 3xTF32 mma.sync only (k_gemm_tc<true>; the pre-Blackwell path, kept for A/B runs)
+//   3 = 3xTF32 mma.sync only (k_gemm_tc<true>; kept for A/B runs)
 extern thread_local int g_gemm_mode;
 
 static inline cudaError_t launch_gemm_legacy(const GemmArgs& G, cudaStream_t stream) {

@@ -1,38 +1,27 @@
-// Blackwell-native GEMM for the wide per-point MLP layers (Vox-Fusion decoder 16-128-128-129 /
-// 144-128-3, Point-SLAM colour trunk 5 x 128): tcgen05.mma kind::tf32 with the accumulators in
-// TMEM, activation tiles fetched by TMA (cp.async.bulk.tensor), warp-specialised roles, 3xTF32
-// error compensation for fp32-level parity.
+// Hopper-native GEMM for the wide per-point MLP layers (Vox-Fusion decoder 16-128-128-129 /
+// 144-128-3, Point-SLAM colour trunk 5 x 128): wgmma.mma_async m64n128k8 tf32 with fp32
+// accumulators in registers, activation tiles fetched by TMA (cp.async.bulk.tensor) into a
+// multi-stage mbarrier pipeline, 3xTF32 error compensation for fp32-level parity.
 //
 //   C[m][n] = epi( sum_k A(m,k) * B[k][n] )      (same contract as gemm.cuh: k_gemm / k_gemm_tc)
-//   MMA M = 128 output features (weights, zero padded), MMA N = BN points per tile (256, or 128
-//   when K > 128 so that the resident weights still fit), K = 8 per instruction.
 //
-// Both operands sit in shared memory in the canonical "no swizzle" K-major UMMA layout (core
-// matrix = 8 rows x 16 bytes; cute/atom/mma_traits_sm100.hpp make_umma_desc<Major::K>):
-//      off(row, k) = (k/4) * (ROWS*16) + row*16 + (k%4)*4      LBO = ROWS*16 B, SBO = 128 B
-//   A (weights, ROWS = 128): staged ONCE per CTA by all threads (handles transA / lda /
-//      padding) as  big = x with the 13 low mantissa bits cleared,  small = x - big.
-//   B (activations [K][N], points contiguous in HBM, ROWS = BN): one TMA box (BN points x BK
-//      rows, row-major) per stage lands in a raw staging tile; the splitter warp-group
-//      transposes it into the K-major layout while splitting big / small (each thread reads
-//      4 k-values of a point from 4 rows and writes one 16-byte chunk: conflict-free).
-//   D: 128 lanes x BN fp32 columns of TMEM, two accumulators, so the epilogue of tile i overlaps
-//      the MMAs of tile i+1.
-// Revision 2 (V2 = true, the default) came out of the ncu capture of revision 1
-// (profiles/r02_gemm_t5_ncu.txt): the kernel was EPILOGUE-bound -- the MMA warp spent 40 % of its
-// time waiting for a drained accumulator, the epilogue warps stalled on instruction fetch
-// (4 056 SASS instructions: a `switch (act)` with an inlined expf per element, scalar tail-guarded
-// mask / addend loops) and on the tcgen05.ld round trip -- and the weight staging cost 17 of
-// 96 us (32 rows x 4 bytes per load instruction, each load waited for before the next).  Now:
-// the steady-state epilogue is a compact vector path (bias + relu as one FADD + FMNMX, the
-// mask / addend / act_out rows as 16-byte accesses, the next 32 columns' tcgen05.ld in flight
-// while the current ones are processed); tails, unaligned rows and sigmoid take the old path.
-// The weights are staged 8 loads at a time, 8 rows x 16 bytes per instruction.  Revision 1 stays
-// selectable (xrd_debug_gemm_variant bit 1) for A/B timing.
-// Roles (384 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer (one elected
-// lane), warps 4-7 = epilogue (tcgen05.ld 32x32b, bias / activation / mask / addend, 128-byte
-// row stores), warps 8-11 = splitter.  All hand-offs are mbarriers; every wait is bounded (a
-// broken pipeline traps instead of hanging the GPU).
+// wgmma takes tf32 operands from shared memory only K-major, and the activations lie in HBM
+// points-contiguous ([K][N]), so the roles are swapped against the math:
+//   MMA M = points (64 per consumer warpgroup, 128 per tile), the A operand from REGISTERS:
+//      every thread reads its fragment straight out of the raw TMA tile (BK rows x BP points,
+//      row-major) and splits it into big = x with the 13 low mantissa bits cleared and
+//      small = x - big;
+//   MMA N = 128 output features (the weights, zero padded), the B operand from SHARED memory,
+//      staged ONCE per CTA by all threads (handles transA / lda / padding) as big / small in the
+//      canonical no-swizzle K-major layout (core matrix = 8 rows x 16 bytes):
+//      off(row, k) = (k/4) * (NF*16) + row*16 + (k%4)*4      LBO = NF*16 B (K), SBO = 128 B (rows)
+//   D: 64 fp32 registers per thread (m64n128), so the epilogue writes C[feature][point] with
+//      the 8 lanes of a quad group covering 8 consecutive points (full 32-byte sectors).
+// Roles (288 threads): warps 0-7 = two consumer warpgroups (fragment loads, 3 wgmma per k8
+// step, epilogue), warp 8 = TMA producer (one elected lane).  The producer runs up to STAGES
+// k-blocks ahead, across tile boundaries, so the next tile's loads overlap this tile's epilogue.
+// All hand-offs are mbarriers; every wait is bounded (a broken pipeline traps instead of
+// hanging the GPU).
 #pragma once
 #include <cuda.h>
 
@@ -41,14 +30,18 @@
 namespace xrd {
 namespace t5 {
 
-constexpr int BM = 128, BK = 16;
-constexpr int NTHREADS = 384;
+constexpr int NF = 128;  // output features per launch (the wgmma N)
+constexpr int BM = NF;   // rows of C one launch covers (launch_gemm splits taller GEMMs)
+constexpr int BP = 128;  // points per tile: 2 consumer warpgroups x 64
+constexpr int BK = 16;   // k rows per pipeline stage (2 wgmma k-steps)
+constexpr int STAGES = 4;
+constexpr int NTHREADS = 288;
 constexpr uint32_t SPIN_LIMIT = 1u << 27;
 
 struct Params {
   GemmArgs G;
   int Kpad;      // K rounded up to BK
-  int n_tiles;   // ceil(N / BN)
+  int n_tiles;   // ceil(N / BP)
   int variant;   // debug (xrd_debug_gemm_variant): bit 0 swaps LBO / SBO in the descriptors
 };
 
@@ -86,12 +79,6 @@ __device__ __forceinline__ void fence_proxy_async() {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0,
                                             int c1) {
   asm volatile(
@@ -100,198 +87,77 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* holder, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(holder)),
-               "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 points][128 features] (+)= A[64 points][8 k] (registers) * B[8 k][128 features] (smem)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b,
+                                           uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes (this warp's TMEM quadrant) x 32 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
 
-// the same load split into issue and wait, so that a second load can be in flight while the
-// first one's registers are consumed; the wait names the registers as in/out operands so that no
-// use of them can be scheduled above it
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]),
-                 "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]),
-                 "+r"(r[14]), "+r"(r[15]), "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]),
-                 "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]), "+r"(r[25]),
-                 "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :
-               : "memory");
-}
-
-// steady-state epilogue of one 32-column chunk of row m (all row pointers 16-byte aligned, the
-// chunk entirely inside N): C = [mask](max(acc + bias, floor)) [+ addend], act_out before addend
-__device__ __forceinline__ void epi_fast(const GemmArgs& G, const uint32_t (&r)[32], int m, int nb,
-                                         float bias, float floorv) {
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = fmaxf(__uint_as_float(r[j]) + bias, floorv);
-  if (G.act == ACT_SOFTPLUS100) {
-    // nn.Softplus(beta = 100) on the SFU (ex2 / lg2): log(1 + e^{100 v}) / 100 with an absolute
-    // error below 3e-8 (the accurate expf / log1pf pair is ~40 instructions per element and
-    // thrashes the instruction cache when unrolled 32 times)
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const float t = v[j] * 100.f;
-      v[j] = (t > 20.f) ? v[j] : __logf(1.f + __expf(t)) * 0.01f;
-    }
-  }
-  if (G.relu_mask) {
-    const float4* mk = reinterpret_cast<const float4*>(G.relu_mask + (size_t)m * G.ldmask + nb);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 k4 = mk[j];
-      if (!(k4.x > 0.f)) v[4 * j] = 0.f;
-      if (!(k4.y > 0.f)) v[4 * j + 1] = 0.f;
-      if (!(k4.z > 0.f)) v[4 * j + 2] = 0.f;
-      if (!(k4.w > 0.f)) v[4 * j + 3] = 0.f;
-    }
-  }
-  if (G.act_out) {
-    float4* ao = reinterpret_cast<float4*>(G.act_out + (size_t)m * G.ldact + nb);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) ao[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-  }
-  if (G.addend) {
-    const float4* ad = reinterpret_cast<const float4*>(G.addend + (size_t)m * G.ldadd + nb);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 a4 = ad[j];
-      v[4 * j] += a4.x; v[4 * j + 1] += a4.y; v[4 * j + 2] += a4.z; v[4 * j + 3] += a4.w;
-    }
-  }
-  float4* cp = reinterpret_cast<float4*>(G.C + (size_t)m * G.ldc + nb);
-  if (G.accumulate) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 c4 = cp[j];
-      cp[j] = make_float4(c4.x + v[4 * j], c4.y + v[4 * j + 1], c4.z + v[4 * j + 2], c4.w + v[4 * j + 3]);
-    }
-  } else {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) cp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-  }
-}
-
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address, leading / stride
-// byte offsets (16-byte units), Blackwell version field = 1, layout type (0 = no swizzle,
-// 2 = 128-byte swizzle) in bits [61,64)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                              uint32_t layout_type) {
+// shared-memory matrix descriptor (sm_90 GMMA): start address, leading / stride byte offsets
+// (16-byte units), base offset 0, layout type 0 (no swizzle) in bits [62,64)
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(layout_type & 7) << 61;
   return d;
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major,
-// M = 128, N = BN
-template <int BN>
-__host__ __device__ constexpr uint32_t make_idesc() {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(BN >> 3) << 17) |
-         ((uint32_t)(BM >> 4) << 24);
 }
 
 __device__ __forceinline__ float tf32_big(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
-template <int BN, int STAGES, bool V2>
 static __global__ void __launch_bounds__(NTHREADS, 1)
 k_gemm_t5(const __grid_constant__ CUtensorMap tmap_b, const Params P) {
-  constexpr int RAW_STAGES = STAGES, OP_STAGES = STAGES;
-  constexpr int RAW_BYTES = BK * BN * 4;  // one TMA box: BK rows x BN points, row-major
-  constexpr int OP_BYTES = BK * BN * 4;   // the same tile in the K-major operand layout
+  constexpr int RAW_BYTES = BK * BP * 4;  // one TMA box: BK rows x BP points, row-major
   extern __shared__ __align__(1024) uint8_t smem[];
   const GemmArgs& G = P.G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int Kpad = P.Kpad;
-  const int a_bytes = BM * Kpad * 4;
-  float* a_big = reinterpret_cast<float*>(smem);
-  float* a_small = reinterpret_cast<float*>(smem + a_bytes);
-  uint8_t* raw_base = smem + 2 * a_bytes;                       // [RAW_STAGES][RAW_BYTES]
-  uint8_t* op_base = raw_base + RAW_STAGES * RAW_BYTES;         // [OP_STAGES][big | small]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(op_base + OP_STAGES * 2 * OP_BYTES);
-  uint64_t* full = bars;                    // [STAGES] TMA bytes landed
-  uint64_t* rawfree = bars + STAGES;        // [STAGES] raw tile consumed by the splitter (128 arrivals)
-  uint64_t* split = bars + 2 * STAGES;      // [STAGES] big / small operand tiles ready (128 arrivals)
-  uint64_t* empty = bars + 3 * STAGES;      // [STAGES] MMAs that read the operand tiles are complete
-  uint64_t* tfull = bars + 4 * STAGES;      // [2]  accumulator complete
-  uint64_t* tempty = bars + 4 * STAGES + 2; // [2]  accumulator drained (128 epilogue arrivals)
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 4 * STAGES + 4);
+  const int w_bytes = NF * Kpad * 4;
+  float* w_big = reinterpret_cast<float*>(smem);
+  float* w_small = reinterpret_cast<float*>(smem + w_bytes);
+  uint8_t* raw_base = smem + 2 * w_bytes;  // [STAGES][RAW_BYTES]
+  uint64_t* full = reinterpret_cast<uint64_t*>(raw_base + STAGES * RAW_BYTES);  // [STAGES] TMA bytes landed
+  uint64_t* empty = full + STAGES;  // [STAGES] fragments read by all 256 consumer threads
 
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full + s, 1); mbar_init(rawfree + s, 128); mbar_init(split + s, 128);
-      mbar_init(empty + s, 1);
-    }
-    for (int s = 0; s < 2; ++s) { mbar_init(tfull + s, 1); mbar_init(tempty + s, 128); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 256); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_holder, 2 * BN);
-  // ---- stage the weights once: A(m,k) -> canonical K-major core-matrix layout, big / small
-  if (V2) {
-    // lane = (m & 7) | (k & 3) << 3: conflict-free shared-memory writes (32 consecutive floats),
-    // 8 rows x 16 bytes (row-major A) or 4 rows x 32 bytes (transposed A) per global request;
-    // 8 independent loads in flight per thread
-    const int n_e = BM * Kpad;
+  // ---- stage the weights once: A(m,k) -> canonical K-major core-matrix layout, big / small.
+  // lane = (m & 7) | (k & 3) << 3: conflict-free shared-memory writes (32 consecutive floats),
+  // 8 rows x 16 bytes (row-major A) or 4 rows x 32 bytes (transposed A) per global request;
+  // 8 independent loads in flight per thread
+  {
+    const int n_e = NF * Kpad;
     for (int e0 = tid; e0 < n_e; e0 += NTHREADS * 8) {
       float v[8];
 #pragma unroll
       for (int u = 0; u < 8; ++u) {
         const int e = e0 + u * NTHREADS;
         const int hi = e >> 5, lo = e & 31;
-        const int m = ((hi % (BM / 8)) << 3) | (lo & 7);
-        const int k = ((hi / (BM / 8)) << 2) | (lo >> 3);
+        const int m = ((hi % (NF / 8)) << 3) | (lo & 7);
+        const int k = ((hi / (NF / 8)) << 2) | (lo >> 3);
         v[u] = 0.f;
         if (e < n_e && m < G.M && k < G.K)
           v[u] = G.transA ? G.A[(size_t)k * G.lda + m] : G.A[(size_t)m * G.lda + k];
@@ -301,198 +167,101 @@ k_gemm_t5(const __grid_constant__ CUtensorMap tmap_b, const Params P) {
         const int e = e0 + u * NTHREADS;
         if (e < n_e) {
           const int hi = e >> 5, lo = e & 31;
-          const int m = ((hi % (BM / 8)) << 3) | (lo & 7);
-          const int k = ((hi / (BM / 8)) << 2) | (lo >> 3);
+          const int m = ((hi % (NF / 8)) << 3) | (lo & 7);
+          const int k = ((hi / (NF / 8)) << 2) | (lo >> 3);
           const float big = tf32_big(v[u]);
-          const int off = (k >> 2) * (BM * 4) + m * 4 + (k & 3);
-          a_big[off] = big;
-          a_small[off] = v[u] - big;
+          const int off = (k >> 2) * (NF * 4) + m * 4 + (k & 3);
+          w_big[off] = big;
+          w_small[off] = v[u] - big;
         }
       }
     }
-  } else {
-    for (int e = tid; e < BM * Kpad; e += NTHREADS) {
-      const int m = e % BM, k = e / BM;
-      float v = 0.f;
-      if (m < G.M && k < G.K) v = G.transA ? G.A[(size_t)k * G.lda + m] : G.A[(size_t)m * G.lda + k];
-      const float big = tf32_big(v);
-      const int off = (k >> 2) * (BM * 4) + m * 4 + (k & 3);
-      a_big[off] = big;
-      a_small[off] = v - big;
-    }
   }
   fence_proxy_async();  // generic-proxy writes -> visible to the tensor core (async proxy)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
   const int n_kb = Kpad / BK;
-  const bool swap = (P.variant & 1) != 0;
-  // K-major, no swizzle: LBO = distance between the two 16-byte K chunks of one MMA,
-  // SBO = distance between 8-row groups
-  const uint32_t a_lbo = swap ? 128u : BM * 16u, a_sbo = swap ? BM * 16u : 128u;
-  const uint32_t b_lbo = swap ? 128u : BN * 16u, b_sbo = swap ? BN * 16u : 128u;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int it = 0;
       for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
         for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const int s = it % RAW_STAGES;
-          mbar_wait(rawfree + s, ((it / RAW_STAGES) & 1) ^ 1);
+          const int s = it % STAGES;
+          mbar_wait(empty + s, ((it / STAGES) & 1) ^ 1);
           mbar_expect_tx(full + s, RAW_BYTES);
-          tma_load_2d(raw_base + (size_t)s * RAW_BYTES, &tmap_b, full + s, tile * BN, kb * BK);
+          tma_load_2d(raw_base + (size_t)s * RAW_BYTES, &tmap_b, full + s, tile * BP, kb * BK);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc<BN>();
-    int it = 0, lt = 0;
-    for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      mbar_wait(tempty + acc, ((lt >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)acc * BN;
-      for (int kb = 0; kb < n_kb; ++kb, ++it) {
-        const int s = it % OP_STAGES;
-        mbar_wait(split + s, (it / OP_STAGES) & 1);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t bb = smem_u32(op_base + (size_t)s * 2 * OP_BYTES);
-          const uint32_t bs = bb + OP_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < BK / 8; ++ks) {
-            const int kca = (kb * (BK / 8) + ks) * 2;  // 16-byte K chunk index in the resident A
-            const int kcb = ks * 2;                    // ... and in this stage's B tile
-            const uint64_t da_b = make_desc(smem_u32(a_big) + kca * (BM * 16), a_lbo, a_sbo, 0);
-            const uint64_t da_s = make_desc(smem_u32(a_small) + kca * (BM * 16), a_lbo, a_sbo, 0);
-            const uint64_t db_b = make_desc(bb + kcb * (BN * 16), b_lbo, b_sbo, 0);
-            const uint64_t db_s = make_desc(bs + kcb * (BN * 16), b_lbo, b_sbo, 0);
-            const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
-            umma_tf32(d_tmem, da_s, db_b, idesc, first);  // small terms first (3xTF32)
-            umma_tf32(d_tmem, da_b, db_s, idesc, 1u);
-            umma_tf32(d_tmem, da_b, db_b, idesc, 1u);
-          }
-          umma_commit(empty + s);                      // operand stage reusable once these retire
-          if (kb == n_kb - 1) umma_commit(tfull + acc);  // accumulator complete
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp >= 8) {
-    // ============ splitter: raw [BK][BN] fp32 tile -> K-major big / small operand tiles ============
-    const int st = tid - 256;  // 0..127
-    int it = 0;
-    for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
-      for (int kb = 0; kb < n_kb; ++kb, ++it) {
-        const int rs = it % RAW_STAGES, os = it % OP_STAGES;
-        mbar_wait(full + rs, (it / RAW_STAGES) & 1);          // TMA landed
-        mbar_wait(empty + os, ((it / OP_STAGES) & 1) ^ 1);    // operand slot no longer read by MMAs
-        const float* raw = reinterpret_cast<const float*>(raw_base + (size_t)rs * RAW_BYTES);
-        float4* big = reinterpret_cast<float4*>(op_base + (size_t)os * 2 * OP_BYTES);
-        float4* sml = reinterpret_cast<float4*>(op_base + (size_t)os * 2 * OP_BYTES + OP_BYTES);
-#pragma unroll
-        for (int q = 0; q < (BK / 4) * BN / 128; ++q) {
-          const int c = st + q * 128;      // chunk = (k quad, point)
-          const int kq = c / BN, n = c - kq * BN;
-          const float v0 = raw[(kq * 4 + 0) * BN + n], v1 = raw[(kq * 4 + 1) * BN + n];
-          const float v2 = raw[(kq * 4 + 2) * BN + n], v3 = raw[(kq * 4 + 3) * BN + n];
-          const float4 b = make_float4(tf32_big(v0), tf32_big(v1), tf32_big(v2), tf32_big(v3));
-          big[kq * BN + n] = b;
-          sml[kq * BN + n] = make_float4(v0 - b.x, v1 - b.y, v2 - b.z, v3 - b.w);
-        }
-        fence_proxy_async();
-        mbar_arrive(split + os);
-        mbar_arrive(rawfree + rs);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int q = warp & 3;              // TMEM lane quadrant of this warp
-    const int m = q * 32 + lane;         // output feature row
-    const bool row_ok = m < G.M;
-    const float bias = (row_ok && G.bias) ? G.bias[m] : 0.f;
-    const bool vec = ((G.ldc & 3) == 0) && ((((uintptr_t)G.C) & 15) == 0);
-    auto row16 = [](const float* p, int ld) { return !p || (((ld & 3) == 0) && ((((uintptr_t)p) & 15) == 0)); };
-    const bool fast = vec && G.act != ACT_SIGMOID && row16(G.relu_mask, G.ldmask) &&  // NONE / RELU / SOFTPLUS100
-                      row16(G.addend, G.ldadd) && row16(G.act_out, G.ldact);
-    const float floorv = (G.act == ACT_RELU) ? 0.f : -INFINITY;  // relu as max(v, 0), none as max(v, -inf)
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x, ++lt) {
-      const int acc = lt & 1;
-      mbar_wait(tfull + acc, (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * BN;
-      const int n0 = tile * BN;
-      if (V2 && fast && n0 + BN <= G.N) {
-        // steady state: full tile, 16-byte aligned rows, no sigmoid.  Two register buffers: the
-        // tcgen05.ld of the next 32 columns is in flight while this chunk is processed.
-        uint32_t ra[32], rb[32];
-        tmem_ld32_issue(t0, ra);
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; c += 2) {
-          tmem_ld32_wait(ra);
-          tmem_ld32_issue(t0 + (c + 1) * 32, rb);
-          if (row_ok) epi_fast(G, ra, m, n0 + c * 32, bias, floorv);
-          tmem_ld32_wait(rb);
-          if (c + 2 < BN / 32) tmem_ld32_issue(t0 + (c + 2) * 32, ra);
-          if (row_ok) epi_fast(G, rb, m, n0 + (c + 1) * 32, bias, floorv);
-        }
-        tc_fence_before();
-        mbar_arrive(tempty + acc);
-        continue;
-      }
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        float v[32];
-        tmem_ld32(t0 + c * 32, v);
-        const int nb = n0 + c * 32;
-        if (row_ok && nb < G.N) {
-          const int nv = min(32, G.N - nb);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = act_apply(v[j] + bias, G.act);
-          if (G.relu_mask) {
-            const float* mk = G.relu_mask + (size_t)m * G.ldmask + nb;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nv && !(mk[j] > 0.f)) v[j] = 0.f;
-          }
-          if (G.act_out) {
-            float* ao = G.act_out + (size_t)m * G.ldact + nb;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nv) ao[j] = v[j];
-          }
-          if (G.addend) {
-            const float* ad = G.addend + (size_t)m * G.ldadd + nb;
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nv) v[j] += ad[j];
-          }
-          float* cp = G.C + (size_t)m * G.ldc + nb;
-          if (vec && nv == 32 && !G.accumulate) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<float4*>(cp + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (j < nv) cp[j] = G.accumulate ? (cp[j] + v[j]) : v[j];
-          }
-        }
-        __syncwarp();  // tcgen05.ld is warp-collective: reconverge before the next chunk
-      }
-      tc_fence_before();
-      mbar_arrive(tempty + acc);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * BN);
+
+  // ===================== consumers: warpgroup c owns points [c*64, c*64 + 64) of a tile ======
+  const int c = warp >> 2, wq = warp & 3, g = lane >> 2, t = lane & 3;
+  const int pl = c * 64 + wq * 16 + g;  // this thread's first point in the tile (second: + 8)
+  const bool swap = (P.variant & 1) != 0;
+  const uint32_t lbo = swap ? 128u : NF * 16u, sbo = swap ? NF * 16u : 128u;
+  const uint32_t wb = smem_u32(w_big), ws = smem_u32(w_small);
+  int it = 0;
+  for (int tile = blockIdx.x; tile < P.n_tiles; tile += gridDim.x) {
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < n_kb; ++kb, ++it) {
+      const int s = it % STAGES;
+      mbar_wait(full + s, (it / STAGES) & 1);
+      const float* raw = reinterpret_cast<const float*>(raw_base + (size_t)s * RAW_BYTES);
+      // A fragment of m64n128k8 (per warp: 16 points x 8 k): a0 = (g, t), a1 = (g + 8, t),
+      // a2 = (g, t + 4), a3 = (g + 8, t + 4) as (point, k)
+      uint32_t ab[BK / 8][4], as[BK / 8][4];
+#pragma unroll
+      for (int ks = 0; ks < BK / 8; ++ks) {
+        const float* r0 = raw + (ks * 8 + t) * BP + pl;
+        const float* r4 = r0 + 4 * BP;
+        const float v[4] = {r0[0], r0[8], r4[0], r4[8]};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float big = tf32_big(v[i]);
+          ab[ks][i] = __float_as_uint(big);
+          as[ks][i] = __float_as_uint(v[i] - big);
+        }
+      }
+      mbar_arrive(empty + s);  // the raw slot may be refilled
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < BK / 8; ++ks) {
+        const uint32_t koff = (uint32_t)(kb * (BK / 4) + ks * 2) * (NF * 16);  // 16-byte K chunks
+        const uint64_t db = make_desc(wb + koff, lbo, sbo), dsm = make_desc(ws + koff, lbo, sbo);
+        wgmma_tf32(acc, as[ks], db, (kb | ks) != 0 ? 1u : 0u);  // small terms first (3xTF32)
+        wgmma_tf32(acc, ab[ks], dsm, 1u);
+        wgmma_tf32(acc, ab[ks], db, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();  // the A fragments live in registers that the next k-block reuses
+    }
+    // ---- epilogue: acc[4i + 2h + j] = (point pl + 8h, feature 8i + 2t + j)
+    const int n0 = tile * BP + pl;
+#pragma unroll
+    for (int i = 0; i < NF / 8; ++i) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int m = 8 * i + 2 * t + j;
+        if (m >= G.M) continue;
+        const float bias = G.bias ? G.bias[m] : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int n = n0 + 8 * h;
+          if (n >= G.N) continue;
+          float v = act_apply(acc[4 * i + 2 * h + j] + bias, G.act);
+          if (G.relu_mask && !(G.relu_mask[(size_t)m * G.ldmask + n] > 0.f)) v = 0.f;
+          if (G.act_out) G.act_out[(size_t)m * G.ldact + n] = v;
+          if (G.addend) v += G.addend[(size_t)m * G.ldadd + n];
+          float* cp = G.C + (size_t)m * G.ldc + n;
+          *cp = G.accumulate ? (*cp + v) : v;
+        }
+      }
+    }
   }
 }
 
@@ -524,45 +293,36 @@ static inline bool eligible(const GemmArgs& G) {
 
 extern thread_local int g_t5_variant;
 
-template <int BN, int STAGES, bool V2>
-static inline cudaError_t launch_bn(const GemmArgs& G, cudaStream_t stream) {
+static inline cudaError_t launch(const GemmArgs& G, cudaStream_t stream) {
   Params P;
   P.G = G;
   P.Kpad = (G.K + BK - 1) / BK * BK;
-  P.n_tiles = (G.N + BN - 1) / BN;
+  P.n_tiles = (G.N + BP - 1) / BP;
   P.variant = g_t5_variant;
-  // B [K][ldb] fp32 as a 2-D tensor (points innermost); box = (BN points, BK rows), no swizzle;
+  // B [K][ldb] fp32 as a 2-D tensor (points innermost); box = (BP points, BK rows), no swizzle;
   // rows >= K and columns >= ldb read as zero (out-of-bounds fill)
   CUtensorMap tm;
   const cuuint64_t dims[2] = {(cuuint64_t)G.ldb, (cuuint64_t)G.K};
   const cuuint64_t strides[1] = {(cuuint64_t)G.ldb * 4};  // bytes, dim 1
-  const cuuint32_t box[2] = {BN, BK};
+  const cuuint32_t box[2] = {BP, BK};
   const cuuint32_t estr[2] = {1, 1};
   CUresult r = encode_fn()(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(G.B), dims, strides,
                            box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return cudaErrorInvalidValue;
-  const size_t smem = 2 * (size_t)BM * P.Kpad * 4 + (size_t)STAGES * 3 * BK * BN * 4 +
-                      256;
+  // resident weights (big + small, 2 x 128 x Kpad x 4 B: 144 KB at K = 144) + STAGES raw
+  // activation tiles (8 KB each) + barriers must fit the 227 KB an H100 block may use
+  const size_t smem = 2 * (size_t)NF * P.Kpad * 4 + (size_t)STAGES * BK * BP * 4 + 2 * STAGES * 8;
   if (smem > 232448) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_gemm_t5<BN, STAGES, V2>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
+    cudaError_t e = cudaFuncSetAttribute(k_gemm_t5, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   int grid = P.n_tiles < num_sms() ? P.n_tiles : num_sms();
-  k_gemm_t5<BN, STAGES, V2><<<grid, NTHREADS, smem, stream>>>(tm, P);
+  k_gemm_t5<<<grid, NTHREADS, smem, stream>>>(tm, P);
   return cudaGetLastError();
-}
-
-static inline cudaError_t launch(const GemmArgs& G, cudaStream_t stream) {
-  // resident weights (big + small, 2 x 128 x Kpad x 4 B) + STAGES x (raw + big + small operand
-  // tiles) (+ the epilogue transposition tiles) must fit 227 KB
-  if (g_t5_variant & 2)  // revision 1 (A/B timing only)
-    return G.K > 128 ? launch_bn<128, 2, false>(G, stream) : launch_bn<256, 2, false>(G, stream);
-  return G.K > 128 ? launch_bn<128, 2, true>(G, stream) : launch_bn<256, 2, true>(G, stream);
 }
 
 }  // namespace t5

@@ -1,4 +1,4 @@
-// NICE-SLAM render-and-optimise step (sm_100a).
+// NICE-SLAM render-and-optimise step (sm_90a).
 //
 // Replaces (reference @ f0366f20): slam/models/conv_onet.py:377-524 render_batch_ray,
 // :339-375 eval_points, slam/model_components/decoder_nice.py:386-414 NICE.forward with the

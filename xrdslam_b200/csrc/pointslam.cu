@@ -1,4 +1,4 @@
-// Point-SLAM render-and-optimise step, stages 'geometry' and 'color' (sm_100a): exact hash-grid kNN, inverse-
+// Point-SLAM render-and-optimise step, stages 'geometry' and 'color' (sm_90a): exact hash-grid kNN, inverse-
 // distance feature interpolation over the neural point cloud, Fourier MLP, normalised occupancy
 // compositing, losses and backward.
 //

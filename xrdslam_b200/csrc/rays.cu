@@ -3,8 +3,8 @@
 //     rays_d = sum_j dir_cam[j] * c2w[id][:3, j],   rays_o = c2w[id][:3, 3]
 //   (slam/common/common.py:39-53 get_rays_from_uv; slam/algorithms/coslam.py:208-216 per-ray
 //   pose gather `poses_all[ids_all]`), and the reduction of d loss / d rays into d loss / d c2w
-//   that torch does with an index_put(accumulate) sort + scatter (0.5 ms per iteration at
-//   4096 rays, profiles/r01_launches_*.csv) -- here one launch with shared-memory accumulators.
+//   that torch does with an index_put(accumulate) sort + scatter -- here one launch with
+//   shared-memory accumulators.
 #include "common.cuh"
 #include "../../include/xrdslam_b200.h"
 
@@ -194,7 +194,7 @@ extern "C" int xrd_rays_pose_grads(int n_rays, const float* dirs_cam, const int6
   p.R = n_rays; p.n_poses = n_poses; p.dirs = dirs_cam; p.ids = pose_ids;
   p.d_rays_o = d_rays_o; p.d_rays_d = d_rays_d; p.d_poses = d_poses;
   int blocks = (n_rays + 255) / 256;
-  if (blocks > 148) blocks = 148;
+  if (blocks > num_sms()) blocks = num_sms();
   rays::k_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(p);
   XRD_LAUNCH_CHECK();
   return XRD_OK;

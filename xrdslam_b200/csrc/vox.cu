@@ -1,4 +1,4 @@
-// Vox-Fusion render-and-optimise step (sm_100a): in-kernel octree traversal, inverse-CDF
+// Vox-Fusion render-and-optimise step (sm_90a): in-kernel octree traversal, inverse-CDF
 // sampling, embedding trilerp, width-128 decoder, SDF compositing, losses and backward.
 //
 // Replaces (reference @ f0366f20):

@@ -1,4 +1,4 @@
-"""Co-SLAM model behind the reference's ``Model`` plugin surface, B200-native.
+"""Co-SLAM model behind the reference's ``Model`` plugin surface, H100-native.
 
 Host-side mirror of slam/models/joint_encoding.py (reference @ f0366f20): same
 class name, same config fields, same ``forward / get_outputs / get_loss_dict /
@@ -7,7 +7,7 @@ signatures, same parameter-group names (``decoder``, ``embed_fn``) and the same
 state_dict keys (``embed_fn.params``, ``decoder.sdf_net.model.{0,2}.weight``,
 ``decoder.color_net.model.{0,2}.weight``).
 
-Nothing is computed in PyTorch: ``forward`` enqueues the fused sm_100a kernels of
+Nothing is computed in PyTorch: ``forward`` enqueues the fused sm_90a kernels of
 ``xrd_coslam_step`` through the C-ABI (forward + loss + full backward in one
 launch when targets are present and grad is enabled) and ``get_loss_dict``
 hands the already-computed loss terms back, wired into autograd so that
@@ -73,7 +73,7 @@ class JointEncodingConfig(ModelConfig):
     cam_far: float = 5.0
     cam_depth_trunc: float = 100.0
     mesh_render_color: bool = False
-    # --- B200 path knobs (not in the reference) ---
+    # --- CUDA path knobs (not in the reference) ---
     seed: int = 0  # Philox seed for in-kernel jitter when no noise is passed
     strict_loss_grad: bool = False  # verify upstream d(total)/d(term) == 1
     rays_per_tile: int = 0   # 0 automatic, -1 tile kernel (k_fused), -2 grouped kernel (k_fused_g)
@@ -192,7 +192,7 @@ class JointEncoding(Model):
         cfg = self.config
         if not cfg.oneGrid or cfg.tcnn_network or cfg.training_n_importance:
             raise NotImplementedError(
-                'B200 path covers the reference defaults: oneGrid=True, '
+                'CUDA path covers the reference defaults: oneGrid=True, '
                 'tcnn_network=False, n_importance=0 (input_config.py:253-254)')
         if not cfg.tcnn_encoding:
             raise NotImplementedError('tcnn_encoding=True is the co-slam '
@@ -276,7 +276,7 @@ class JointEncoding(Model):
         dev = table.device
         if dev.type != 'cuda':
             raise RuntimeError('xrdslam_b200 has no CPU path: model must be on '
-                               'a CUDA (sm_100) device')
+                               'a CUDA (sm_90) device')
         lib = _cabi.lib()
         f32 = dict(dtype=torch.float32, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()

@@ -1,4 +1,4 @@
-"""Neural point cloud of Point-SLAM, B200-native (host-side mirror of
+"""Neural point cloud of Point-SLAM, H100-native (host-side mirror of
 slam/model_components/neural_point_cloud.py): positions and features are device tensors (the
 reference keeps positions in Python lists and re-tensorises them every call,
 decoder_pointslam.py:172,417), and neighbour search is an EXACT radius-limited 8-NN over a

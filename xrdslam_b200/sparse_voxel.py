@@ -1,4 +1,4 @@
-"""Vox-Fusion model behind the reference's ``Model`` plugin surface, B200-native.
+"""Vox-Fusion model behind the reference's ``Model`` plugin surface, H100-native.
 
 Host-side mirror of slam/models/sparse_voxel.py (reference @ f0366f20): same class / config
 names, ``forward / get_loss_dict / get_param_groups / insert_points / update_map_states``
@@ -54,7 +54,7 @@ class SparseVoxelConfig(ModelConfig):
     keyframe_th: int = 30
     keyframe_selection: str = 'random'
     data_sc_factor: int = 1
-    # --- B200 path knobs ---
+    # --- CUDA path knobs ---
     max_samples_per_ray: int = 256  # capacity of the per-ray sample arrays
     seed: int = 0
     device_octree: bool = True  # grow the octree on the device (octree_device.py)
