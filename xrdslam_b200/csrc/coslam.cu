@@ -314,17 +314,29 @@ __device__ __forceinline__ void encode_point(const Params& P, const Lv* __restri
 }
 
 // NL (point, level) items of the hash backward per call (scatter (g0,g1), optional d/dx).
-// Deliberately not inlined: instruction-cache footprint matters for this kernel.
+// Deliberately not inlined: instruction-cache footprint matters for this kernel.  It takes the
+// two table pointers by value: a `const Params&` argument of a non-inlined function forces the
+// caller to copy the whole ~730-byte kernel-parameter block to local memory.
 // NL (point, level) items per call: the 8 NL corner loads of all levels are issued before any
 // is consumed (the kernel runs at 7 warps/SM, so memory-level parallelism has to come from
 // within the thread), then the 8 NL scatters.  on[h]: item present (level exists and its
-// gradient is non-zero).  Levels are l0 + 4 h (fragment layout: lane t owns levels 4 nt + t).
+// gradient is non-zero).  Levels are l0 + lstride h (tile kernel: lane t owns levels 4 nt + t).
+// The items travel by value as well: an array passed by reference would live in local memory.
 template <int NL>
-__device__ __noinline__ float3 hash_backward_multi(const Params& P, const Lv* __restrict__ lv,
-                                                   int l0, const bool (&on)[NL], float x0,
-                                                   float x1, float x2, const float (&g)[NL][2],
-                                                   bool need_dx, bool scatter, int lstride = 4) {
-  const float2* __restrict__ tab = reinterpret_cast<const float2*>(P.table);
+struct LevelItems {
+  float g[NL][2];  // d loss / d (f0, f1) of level l0 + lstride h
+  bool on[NL];
+};
+template <int NL>
+__device__ __noinline__ float3 hash_backward_multi(const float* __restrict__ table,
+                                                   float* __restrict__ d_table,
+                                                   const Lv* __restrict__ lv, int l0,
+                                                   const LevelItems<NL> it, float x0, float x1,
+                                                   float x2, bool need_dx, bool scatter,
+                                                   int lstride = 4) {
+  const float2* __restrict__ tab = reinterpret_cast<const float2*>(table);
+  const auto& on = it.on;
+  const auto& g = it.g;
   const float x[3] = {x0, x1, x2};
   float w[NL][3], sc[NL];
   uint32_t idx[NL][8];
@@ -374,7 +386,7 @@ __device__ __noinline__ float3 hash_backward_multi(const Params& P, const Lv* __
       for (int k = 0; k < 8; ++k) {
         const float wk = ((k & 1) ? w[h][0] : 1.f - w[h][0]) * ((k & 2) ? w[h][1] : 1.f - w[h][1]) *
                          ((k & 4) ? w[h][2] : 1.f - w[h][2]);
-        red_add_v2(P.d_table + 2 * (size_t)idx[h][k], wk * g[h][0], wk * g[h][1]);
+        red_add_v2(d_table + 2 * (size_t)idx[h][k], wk * g[h][0], wk * g[h][1]);
       }
     }
   }
@@ -503,16 +515,47 @@ constexpr int SW_TOTAL = SWC1 + 32 * LDC1; // 6784 floats
 //   [0,2) d w_col1   [2,18) d w_col0   [18,22) d w_sdf1   [22,42) d w_sdf0
 constexpr int DW_TILES = 42;
 
-template <bool PREC3>
+// record of the grouped kernel (k_fused_g), stride 132 == 4 (mod 32): the 48 OneBlob bins are
+// kept in compact form (blob_compact_dim), so that the decoder-input columns outside the OneBlob
+// block sit at their own index: [feat 0..31 | blob] for the SDF decoder, [blob | geo 48..62 |
+// sdf 63] for the colour decoder.
+constexpr int G_FEAT = 0, G_BLOB = 32, G_GEO = 48, G_SDF = 63, G_H1 = 64, G_C1 = 96, G_RAW = 128,
+              GREC = 132;
+
+// A fragment values of the dense OneBlob bins (g, g + 8) of dimension bd for points p0 (k-slot t)
+// and p1 (k-slot t + 4), expanded from the compact form: both bins live in slot g & 3, with
+// quarters g >> 2 and (g >> 2) + 2.
+__device__ __forceinline__ void blob_dw_frag(const float* __restrict__ p0,
+                                             const float* __restrict__ p1, int bd, int g,
+                                             float (&va)[4]) {
+  const int e = g & 3;
+  const uint32_t m = (uint32_t)(g >> 2);
+  const float a0 = p0[G_BLOB + 4 * bd + e], a1 = p1[G_BLOB + 4 * bd + e];
+  const uint32_t q0 = reinterpret_cast<const uint8_t*>(p0 + G_BLOB + 12 + bd)[e];
+  const uint32_t q1 = reinterpret_cast<const uint8_t*>(p1 + G_BLOB + 12 + bd)[e];
+  va[0] = (q0 == m) ? a0 : 0.f;
+  va[1] = (q0 == m + 2) ? a0 : 0.f;
+  va[2] = (q1 == m) ? a1 : 0.f;
+  va[3] = (q1 == m + 2) ? a1 : 0.f;
+}
+
+// STRIDE: record stride; BLOB && bd >= 0: the 16 A rows are the OneBlob bins of dimension bd of a
+// compact grouped-kernel record (aoff unused).
+template <bool PREC3, int STRIDE = REC, bool BLOB = false>
 __device__ __forceinline__ void dw_tile(const float* __restrict__ recs, int npts, int aoff,
-                                        int boff, float (&acc)[4]) {
+                                        int boff, float (&acc)[4], int bd = -1) {
   // acc[16 x 8] += sum_p A[p][aoff + m] * B[p][boff + n]; k-slot t <-> point 2t, t+4 <-> 2t+1
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll 2
   for (int k0 = 0; k0 < npts; k0 += 8) {
-    const float* p0 = recs + (k0 + 2 * t) * REC;
-    const float* p1 = p0 + REC;
-    const float va[4] = {p0[aoff + g], p0[aoff + g + 8], p1[aoff + g], p1[aoff + g + 8]};
+    const float* p0 = recs + (k0 + 2 * t) * STRIDE;
+    const float* p1 = p0 + STRIDE;
+    float va[4];
+    if (BLOB && bd >= 0) {
+      blob_dw_frag(p0, p1, bd, g, va);
+    } else {
+      va[0] = p0[aoff + g]; va[1] = p0[aoff + g + 8]; va[2] = p1[aoff + g]; va[3] = p1[aoff + g + 8];
+    }
     FragA<PREC3> a;
     a.set(va);
     FragB<PREC3> b;
@@ -880,18 +923,17 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
             if (row < npts) {
               const float x3[3] = {xnb[row * 3], xnb[row * 3 + 1], xnb[row * 3 + 2]};
               {  // the 4 levels of this lane (t, 4 + t, 8 + t, 12 + t) in one call
-                bool on[4];
-                float gg[4][2];
+                LevelItems<4> it;
                 bool any = false;
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt) {
-                  gg[nt][0] = c[mt][nt][2 * h]; gg[nt][1] = c[mt][nt][2 * h + 1];
-                  on[nt] = (4 * nt + t) < P.g.n_levels && (gg[nt][0] != 0.f || gg[nt][1] != 0.f);
-                  any |= on[nt];
+                  it.g[nt][0] = c[mt][nt][2 * h]; it.g[nt][1] = c[mt][nt][2 * h + 1];
+                  it.on[nt] = (4 * nt + t) < P.g.n_levels && (it.g[nt][0] != 0.f || it.g[nt][1] != 0.f);
+                  any |= it.on[nt];
                 }
                 if (any) {
-                  const float3 d3 = hash_backward_multi<4>(P, s_lv, t, on, x3[0], x3[1], x3[2], gg,
-                                                           need_dx, map_grads);
+                  const float3 d3 = hash_backward_multi<4>(P.table, P.d_table, s_lv, t, it, x3[0],
+                                                           x3[1], x3[2], need_dx, map_grads);
                   hdx[mt][h][0] += d3.x; hdx[mt][h][1] += d3.y; hdx[mt][h][2] += d3.z;
                 }
               }
@@ -993,14 +1035,61 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
 // phases that were serialised behind __syncthreads() in k_fused now overlap on the SM.
 // Two threads share one sample point in the gather phases (8 levels each), one warp owns one
 // 16-row MMA tile; all intra-group synchronisation is a named barrier (bar.sync grp+1, 192).
+// Shared memory per slot: the 132-float compact record (GREC) and its z value; sigma(sdf/tr)
+// and the composite weights live in registers (a lane owns <= G_KPL samples of a ray), xn is
+// recomputed from the ray and z where the backward needs it.
 constexpr int GT = 192;      // threads per group
 constexpr int GW = 6;        // warps per group = m-tiles of 16 points per unit
 constexpr int GP = 96;       // record slots per group
 constexpr int NGROUPS = 3;
 constexpr int G_SLOTS = 7;   // 42 weight-gradient tiles / 6 warps
+constexpr int G_KPL = (GP + 31) / 32;  // samples per lane in the per-ray composite (S <= GP)
 
 __device__ __forceinline__ void group_sync(int grp) {
   asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(GT) : "memory");
+}
+
+// OneBlob of one coordinate in compact form.  The three images s = -1, 0, 1 of blob_forward fill
+// windows of 3 bins that lie 15..17 bins apart (16 up to the rounding of x - s), so no bin gets
+// two contributions, at most 4 of the 16 bins are non-zero (for any x, inside the bounding box or
+// not) and two non-zero bins never agree mod 4.  Bin b is kept in slot b & 3: v[b & 3] holds
+// exactly the float of the dense form (0 + contribution) and byte b & 3 of q holds b >> 2.
+// Dense bin b = (q[b & 3] == b >> 2) ? v[b & 3] : 0; empty slots hold value 0.
+// Per point: [v dim0 (4) | v dim1 (4) | v dim2 (4) | q dim0 | q dim1 | q dim2 | unused].
+__device__ __forceinline__ void blob_compact_dim(float x, float* __restrict__ v,
+                                                 uint8_t* __restrict__ q) {
+  *reinterpret_cast<float4*>(v) = make_float4(0.f, 0.f, 0.f, 0.f);
+  *reinterpret_cast<uint32_t*>(q) = 0u;
+#pragma unroll
+  for (int s = -1; s <= 1; ++s) {
+    const float u = (x - (float)s) * (float)kBins;
+    const float fl = floorf(u);
+    if (fl < -1.f || fl > (float)kBins) continue;
+    const int b0 = (int)fl;
+    const float f = u - fl;
+    const float c0 = qcdf(-f), c1 = qcdf(1.f - f);
+    if (b0 - 1 >= 0 && b0 - 1 < kBins) { v[(b0 - 1) & 3] = 0.f + c0; q[(b0 - 1) & 3] = (uint8_t)((b0 - 1) >> 2); }
+    if (b0 >= 0 && b0 < kBins) { v[b0 & 3] = 0.f + (c1 - c0); q[b0 & 3] = (uint8_t)(b0 >> 2); }
+    if (b0 + 1 >= 0 && b0 + 1 < kBins) { v[(b0 + 1) & 3] = 0.f + (1.f - c1); q[(b0 + 1) & 3] = (uint8_t)((b0 + 1) >> 2); }
+  }
+}
+
+// A fragment of k-step kb of the dense 48-column OneBlob block for rows g, g + 8 of a warp's
+// compact records: lane t needs bins t, t + 4 of dimension kb >> 1, half kb & 1, i.e. slot t with
+// quarters 2 (kb & 1) and 2 (kb & 1) + 1.
+__device__ __forceinline__ void blob_frag(const float* __restrict__ wrec, int kb, int g, int t,
+                                          float (&v)[4]) {
+  const int d = kb >> 1;
+  const uint32_t m = 2u * (uint32_t)(kb & 1);
+  const float* r0 = wrec + g * GREC + G_BLOB;
+  const float* r8 = r0 + 8 * GREC;
+  const float a0 = r0[4 * d + t], a8 = r8[4 * d + t];
+  const uint32_t q0 = reinterpret_cast<const uint8_t*>(r0 + 12 + d)[t];
+  const uint32_t q8 = reinterpret_cast<const uint8_t*>(r8 + 12 + d)[t];
+  v[0] = (q0 == m) ? a0 : 0.f;
+  v[1] = (q8 == m) ? a8 : 0.f;
+  v[2] = (q0 == m + 1) ? a0 : 0.f;
+  v[3] = (q8 == m + 1) ? a8 : 0.f;
 }
 
 // hash levels half, half+2, ... and the OneBlob dims of this half (0: x,y  1: z)
@@ -1012,7 +1101,7 @@ __device__ __forceinline__ void encode_half(const Params& P, const Lv* __restric
   for (int i = 0; i < kL / 2; ++i) {
     const int l = half + 2 * i;
     if (l >= P.g.n_levels) {
-      *reinterpret_cast<float2*>(rec + R_FEAT + 2 * l) = make_float2(0.f, 0.f);
+      *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) = make_float2(0.f, 0.f);
       if (jac) {
         *reinterpret_cast<float2*>(jac + 6 * i) = make_float2(0.f, 0.f);
         *reinterpret_cast<float2*>(jac + 6 * i + 2) = make_float2(0.f, 0.f);
@@ -1040,7 +1129,7 @@ __device__ __forceinline__ void encode_half(const Params& P, const Lv* __restric
       f0 = fmaf(wk, v[k].x, f0);
       f1 = fmaf(wk, v[k].y, f1);
     }
-    *reinterpret_cast<float2*>(rec + R_FEAT + 2 * l) = make_float2(f0, f1);
+    *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) = make_float2(f0, f1);
     if (jac) {
       // d feat / d xn while the 8 corners are in registers: [f0: dx dy dz | f1: dx dy dz] * scale
       const float w0 = w[0], w1 = w[1], w2 = w[2], sc = L.scale;
@@ -1058,28 +1147,17 @@ __device__ __forceinline__ void encode_half(const Params& P, const Lv* __restric
       *reinterpret_cast<float2*>(jac + 6 * i + 4) = make_float2(sc * jy1, sc * jz1);
     }
   }
-  const int d_lo = half ? 2 : 0, d_hi = half ? 3 : 2;
-  for (int d = d_lo; d < d_hi; ++d) {
-    float* o = rec + R_BLOB + d * kBins;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) *reinterpret_cast<float4*>(o + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int s = -1; s <= 1; ++s) {
-      const float u = (xn[d] - (float)s) * (float)kBins;
-      const float fl = floorf(u);
-      if (fl < -1.f || fl > (float)kBins) continue;
-      const int b0 = (int)fl;
-      const float f = u - fl;
-      const float c0 = qcdf(-f), c1 = qcdf(1.f - f);
-      if (b0 - 1 >= 0 && b0 - 1 < kBins) o[b0 - 1] += c0;
-      if (b0 >= 0 && b0 < kBins) o[b0] += c1 - c0;
-      if (b0 + 1 >= 0 && b0 + 1 < kBins) o[b0 + 1] += 1.f - c1;
-    }
-  }
+  // (constant indices into xn: a run-time index would put it in local memory)
+  const int d0 = half ? 2 : 0;
+  blob_compact_dim(half ? xn[2] : xn[0], rec + G_BLOB + 4 * d0,
+                   reinterpret_cast<uint8_t*>(rec + G_BLOB + 12 + d0));
+  if (!half)
+    blob_compact_dim(xn[1], rec + G_BLOB + 4, reinterpret_cast<uint8_t*>(rec + G_BLOB + 13));
 }
 
-// one 16-row m-tile: C[nt] += A * B   (A rows = wrec[row*REC + aoff + k])
-template <int KS, int NT, bool TRANS, bool PREC3>
+// one 16-row m-tile: C[nt] += A * B   (A rows = wrec[row*GREC + aoff + k]; k-steps
+// [BK0, BK0 + 6) are the 48-column OneBlob block instead, expanded from the compact records)
+template <int KS, int NT, bool TRANS, bool PREC3, int BK0 = -1>
 __device__ __forceinline__ void warp_gemm1(const float* __restrict__ wrec, int aoff,
                                            const float* __restrict__ w, int ld, int koff,
                                            int noff, float (&c)[NT][4]) {
@@ -1088,8 +1166,13 @@ __device__ __forceinline__ void warp_gemm1(const float* __restrict__ wrec, int a
   for (int ks = 0; ks < KS; ++ks) {
     FragA<PREC3> a;
     {
-      const float* r0 = wrec + g * REC + aoff + ks * 8 + t;
-      const float v[4] = {r0[0], r0[8 * REC], r0[4], r0[8 * REC + 4]};
+      float v[4];
+      if (BK0 >= 0 && ks >= BK0 && ks < BK0 + 6) {
+        blob_frag(wrec, ks - BK0, g, t, v);
+      } else {
+        const float* r0 = wrec + g * GREC + aoff + ks * 8 + t;
+        v[0] = r0[0]; v[1] = r0[8 * GREC]; v[2] = r0[4]; v[3] = r0[8 * GREC + 4];
+      }
       a.set(v);
     }
 #pragma unroll
@@ -1116,9 +1199,9 @@ __device__ __forceinline__ void store_c1(float* __restrict__ wrec, int coff, con
   for (int nt = 0; nt < NT; ++nt) {
     float v0 = c[nt][0], v1 = c[nt][1], v2 = c[nt][2], v3 = c[nt][3];
     if (RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
-    float* r0 = wrec + g * REC + coff + nt * 8 + 2 * t;
+    float* r0 = wrec + g * GREC + coff + nt * 8 + 2 * t;
     *reinterpret_cast<float2*>(r0) = make_float2(v0, v1);
-    *reinterpret_cast<float2*>(r0 + 8 * REC) = make_float2(v2, v3);
+    *reinterpret_cast<float2*>(r0 + 8 * GREC) = make_float2(v2, v3);
   }
 }
 
@@ -1130,19 +1213,17 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   const int grp = tid / GT, gt = tid - grp * GT;
   const int gw = gt >> 5, lane = gt & 31;
   const int g = lane >> 2, t = lane & 3;
-  float* recs = sw + SW_TOTAL + grp * (GP * REC);
-  float* misc = sw + SW_TOTAL + NGROUPS * (GP * REC) + grp * (GP * 6);
-  float* zbuf = misc;          // GP z values
-  float* sgb = misc + GP;      // GP sigma(sdf/trunc)
-  float* ub = misc + 2 * GP;   // GP unnormalised weights
-  float* xnb = misc + 3 * GP;  // GP*3 normalised coordinates
+  float* recs = sw + SW_TOTAL + grp * (GP * GREC);
+  float* zbuf = sw + SW_TOTAL + NGROUPS * (GP * GREC) + grp * GP;  // GP z values
   const int S = P.S;
 
   __shared__ Lv s_lv[kL];
   __shared__ int s_unit[NGROUPS];
+  __shared__ double s_loss[4];  // loss sums of the CTA (registers are the scarce resource here)
   load_levels(s_lv, P.g);
+  if (tid < 4) s_loss[tid] = 0.0;
   for (int q = tid; q < SW_TOTAL; q += blockDim.x) sw[q] = 0.f;
-  for (int q = gt; q < GP * REC; q += GT) recs[q] = 0.f;
+  for (int q = gt; q < GP * GREC; q += GT) recs[q] = 0.f;
   __syncthreads();
   for (int q = tid; q < 80 * 32; q += blockDim.x) {
     int i = q / 32, j = q % 32;
@@ -1170,7 +1251,6 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     sdf_w = 1.0f - n_sdf / n;
     inv_nvalid = 1.0f / (float)P.counts[2];
   }
-  double l_rgb = 0.0, l_depth = 0.0, l_sdf = 0.0, l_fs = 0.0;
   float dwacc[G_SLOTS][4];
 #pragma unroll
   for (int j = 0; j < G_SLOTS; ++j)
@@ -1179,8 +1259,8 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   __syncthreads();
 
   const int p = gt >> 1, half = gt & 1;       // gather phases: two threads per point
-  float* rec = recs + p * REC;
-  float* wrec = recs + (gw * 16) * REC;       // MMA phases: this warp's 16 records
+  float* rec = recs + p * GREC;
+  float* wrec = recs + (gw * 16) * GREC;      // MMA phases: this warp's 16 records
   const bool need_dx = BWD && ((P.d_rays_o != nullptr) || (P.d_rays_d != nullptr));
   const bool map_grads = BWD && (P.d_table != nullptr);
   int prev_npts = 0;
@@ -1208,114 +1288,130 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         float pt = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], zv));
         xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
       }
-      if (half == 0) {
-        zbuf[p] = zv;
-        xnb[p * 3] = xn[0]; xnb[p * 3 + 1] = xn[1]; xnb[p * 3 + 2] = xn[2];
-      }
+      if (half == 0) zbuf[p] = zv;
       encode_half(P, s_lv, xn, rec, half,
                   (need_dx && P.jac) ? P.jac + ((size_t)((size_t)r * S + k) * 2 + half) * 48 : nullptr);
     } else if (p < prev_npts) {
       // rows left dirty by a larger unit must read as zero in every GEMM
-      float* z0 = rec + half * (REC / 2);
+      float* z0 = rec + half * (GREC / 2);
 #pragma unroll 1
-      for (int q = 0; q < REC / 2; q += 2) *reinterpret_cast<float2*>(z0 + q) = make_float2(0.f, 0.f);
+      for (int q = 0; q < GREC / 2; q += 2) *reinterpret_cast<float2*>(z0 + q) = make_float2(0.f, 0.f);
     }
     prev_npts = npts;
     __syncwarp();
     if (warp_active) {
-      {  // h1 = relu(x W0^T)
+      {  // h1 = relu([feat, blob] W0^T)
         float c[4][4];
         zero_c1<4>(c);
-        warp_gemm1<10, 4, false, PREC3>(wrec, R_FEAT, sw + SW0, LD0, 0, 0, c);
-        store_c1<4, true>(wrec, R_H1, c);
+        warp_gemm1<10, 4, false, PREC3, 4>(wrec, G_FEAT, sw + SW0, LD0, 0, 0, c);
+        store_c1<4, true>(wrec, G_H1, c);
       }
       __syncwarp();
       {  // [geo, sdf] = h1 W1^T
         float c[2][4];
         zero_c1<2>(c);
-        warp_gemm1<4, 2, false, PREC3>(wrec, R_H1, sw + SW1, LD1, 0, 0, c);
-        store_c1<2, false>(wrec, R_GEO, c);
+        warp_gemm1<4, 2, false, PREC3>(wrec, G_H1, sw + SW1, LD1, 0, 0, c);
+        store_c1<2, false>(wrec, G_GEO, c);
       }
       __syncwarp();
       {  // c1 = relu([blob, geo, (sdf: zero weight row)] Wc0^T)
         float c[4][4];
         zero_c1<4>(c);
-        warp_gemm1<8, 4, false, PREC3>(wrec, R_BLOB, sw + SWC0, LDC0, 0, 0, c);
-        store_c1<4, true>(wrec, R_C1, c);
+        warp_gemm1<8, 4, false, PREC3, 0>(wrec, 0, sw + SWC0, LDC0, 0, 0, c);
+        store_c1<4, true>(wrec, G_C1, c);
       }
       __syncwarp();
       {  // rgb logits = c1 Wc1^T (cols 0..2 of an 8-wide tile)
         float c[1][4];
         zero_c1<1>(c);
-        warp_gemm1<4, 1, false, PREC3>(wrec, R_C1, sw + SWC1, LDC1, 0, 0, c);
-        float* q0 = wrec + g * REC + R_RAW;
+        warp_gemm1<4, 1, false, PREC3>(wrec, G_C1, sw + SWC1, LDC1, 0, 0, c);
+        float* q0 = wrec + g * GREC + G_RAW;
         if (t == 0) {
           q0[0] = c[0][0]; q0[1] = c[0][1];
-          q0[8 * REC] = c[0][2]; q0[8 * REC + 1] = c[0][3];
+          q0[8 * GREC] = c[0][2]; q0[8 * GREC + 1] = c[0][3];
         } else if (t == 1) {
           q0[2] = c[0][0];
-          q0[8 * REC + 2] = c[0][2];
+          q0[8 * GREC + 2] = c[0][2];
         }
       }
       __syncwarp();
     }
     if (active && half == 0) {
-      rec[R_RAW + 3] = rec[R_SDF];
+      rec[G_RAW + 3] = rec[G_SDF];
       if (P.raw) {
-        float4 rw = *reinterpret_cast<const float4*>(rec + R_RAW);
+        float4 rw = *reinterpret_cast<const float4*>(rec + G_RAW);
         *reinterpret_cast<float4*>(P.raw + ((size_t)r * S + k) * 4) = rw;
       }
     }
     group_sync(grp);
     // ---------------- phase 2: per-ray composite, loss, d loss / d raw ----
+    // lane owns samples lane + 32 i (i < G_KPL): sigma(s/tr) and the unnormalised weight u stay
+    // in registers
     for (int q = gw; q < nr; q += GW) {
       const int rr = r0 + q;
       const float* zr = zbuf + q * S;
-      float* sg_r = sgb + q * S;
-      float* u_r = ub + q * S;
-      float* rq = recs + (size_t)(q * S) * REC;
+      float* rq = recs + (size_t)(q * S) * GREC;
       const float tr = P.trunc;
+      float sg_r[G_KPL], u_r[G_KPL];
       int first = 0x7fffffff;
-      for (int kk = lane; kk < S; kk += 32) {
-        float* rp = rq + kk * REC + R_RAW;
-        const float s = rp[3];
-        const float sg = sigmoidf_acc(s / tr);
-        sg_r[kk] = sg;
-        u_r[kk] = sg * sigmoidf_acc((-s) / tr);
-        rp[0] = sigmoidf_acc(rp[0]);
-        rp[1] = sigmoidf_acc(rp[1]);
-        rp[2] = sigmoidf_acc(rp[2]);
-        if (kk < S - 1 && rq[(kk + 1) * REC + R_RAW + 3] * s < 0.f) first = min(first, kk);
+#pragma unroll
+      for (int i = 0; i < G_KPL; ++i) {
+        const int kk = lane + 32 * i;
+        sg_r[i] = 0.f;
+        u_r[i] = 0.f;
+        if (kk < S) {
+          float* rp = rq + kk * GREC + G_RAW;
+          const float s = rp[3];
+          const float sg = sigmoidf_acc(s / tr);
+          sg_r[i] = sg;
+          u_r[i] = sg * sigmoidf_acc((-s) / tr);
+          rp[0] = sigmoidf_acc(rp[0]);
+          rp[1] = sigmoidf_acc(rp[1]);
+          rp[2] = sigmoidf_acc(rp[2]);
+          if (kk < S - 1 && rq[(kk + 1) * GREC + G_RAW + 3] * s < 0.f) first = min(first, kk);
+        }
       }
       first = warp_min_i(first);
       if (first == 0x7fffffff) first = 0;
       __syncwarp();
       const float zlim = zr[first] + P.trunc;
       float usum = 0.f;
-      for (int kk = lane; kk < S; kk += 32) {
-        const float u = (zr[kk] < zlim) ? u_r[kk] : 0.f;
-        u_r[kk] = u;
-        usum += u;
+#pragma unroll
+      for (int i = 0; i < G_KPL; ++i) {
+        const int kk = lane + 32 * i;
+        if (kk < S) {
+          const float u = (zr[kk] < zlim) ? u_r[i] : 0.f;
+          u_r[i] = u;
+          usum += u;
+        }
       }
       usum = warp_sum(usum);
       const float W = usum + 1e-8f;
       float o_r = 0.f, o_g = 0.f, o_b = 0.f, o_d = 0.f, o_acc = 0.f;
-      for (int kk = lane; kk < S; kk += 32) {
-        const float* rp = rq + kk * REC + R_RAW;
-        const float w = u_r[kk] / W;
-        o_r = fmaf(w, rp[0], o_r);
-        o_g = fmaf(w, rp[1], o_g);
-        o_b = fmaf(w, rp[2], o_b);
-        o_d = fmaf(w, zr[kk], o_d);
-        o_acc += w;
+#pragma unroll
+      for (int i = 0; i < G_KPL; ++i) {
+        const int kk = lane + 32 * i;
+        if (kk < S) {
+          const float* rp = rq + kk * GREC + G_RAW;
+          const float w = u_r[i] / W;
+          o_r = fmaf(w, rp[0], o_r);
+          o_g = fmaf(w, rp[1], o_g);
+          o_b = fmaf(w, rp[2], o_b);
+          o_d = fmaf(w, zr[kk], o_d);
+          o_acc += w;
+        }
       }
       o_r = warp_sum(o_r); o_g = warp_sum(o_g); o_b = warp_sum(o_b);
       o_d = warp_sum(o_d); o_acc = warp_sum(o_acc);
       if (P.depth_var) {
         float v = 0.f;
-        for (int kk = lane; kk < S; kk += 32) {
-          const float dz = zr[kk] - o_d;
-          v = fmaf(u_r[kk] / W, dz * dz, v);
+#pragma unroll
+        for (int i = 0; i < G_KPL; ++i) {
+          const int kk = lane + 32 * i;
+          if (kk < S) {
+            const float dz = zr[kk] - o_d;
+            v = fmaf(u_r[i] / W, dz * dz, v);
+          }
         }
         v = warp_sum(v);
         if (lane == 0) P.depth_var[rr] = v;
@@ -1336,26 +1432,33 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
         const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * inv_nvalid : 0.f;
         if (lane == 0) {
-          l_rgb += (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
-                            (o_b - tb_) * (o_b - tb_));
-          if (valid) l_depth += (double)((o_d - td) * (o_d - td));
+          atomicAdd(&s_loss[0], (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
+                                         (o_b - tb_) * (o_b - tb_)));
+          if (valid) atomicAdd(&s_loss[1], (double)((o_d - td) * (o_d - td)));
         }
         float qw = 0.f;
-        for (int kk = lane; kk < S; kk += 32) {
-          const float* rp = rq + kk * REC + R_RAW;
-          const float q_ = g_r * rp[0] + g_g * rp[1] + g_b * rp[2] + g_d * zr[kk];
-          qw = fmaf(q_, u_r[kk] / W, qw);
+#pragma unroll
+        for (int i = 0; i < G_KPL; ++i) {
+          const int kk = lane + 32 * i;
+          if (kk < S) {
+            const float* rp = rq + kk * GREC + G_RAW;
+            const float q_ = g_r * rp[0] + g_g * rp[1] + g_b * rp[2] + g_d * zr[kk];
+            qw = fmaf(q_, u_r[i] / W, qw);
+          }
         }
         qw = warp_sum(qw);
         float a_fs = 0.f, a_sdf = 0.f;
         const float c_fs = P.ls[3] * P.w_fs * fs_w * 2.0f / RS;
         const float c_sdf = P.ls[2] * P.w_sdf * sdf_w * 2.0f / RS;
-        for (int kk = lane; kk < S; kk += 32) {
-          float* rp = rq + kk * REC + R_RAW;
+#pragma unroll
+        for (int i = 0; i < G_KPL; ++i) {
+          const int kk = lane + 32 * i;
+          if (kk >= S) continue;
+          float* rp = rq + kk * GREC + G_RAW;
           const float z = zr[kk];
           const float s = rp[3];
-          const float sg = sg_r[kk];
-          const float u = u_r[kk];  // a * mask
+          const float sg = sg_r[i];
+          const float u = u_r[i];  // a * mask
           const float w = u / W;
           const float c0 = rp[0], c1 = rp[1], c2 = rp[2];
           const float q_ = g_r * c0 + g_g * c1 + g_b * c2 + g_d * z;
@@ -1378,100 +1481,107 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         }
         a_fs = warp_sum(a_fs);
         a_sdf = warp_sum(a_sdf);
-        if (lane == 0) { l_fs += (double)a_fs; l_sdf += (double)a_sdf; }
+        if (lane == 0) { atomicAdd(&s_loss[3], (double)a_fs); atomicAdd(&s_loss[2], (double)a_sdf); }
       }
     }
     if (!BWD) continue;  // the barrier at the top of the loop orders the next unit
     group_sync(grp);
     // ---------------- phase 3: backward ----------------------------------
     const int npts8 = (npts + 7) & ~7;
-    auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n) {
+    // m-tile mt of a layer input covers its columns 16 mt .. 16 mt + 15 at record offset aoff;
+    // m-tiles [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form
+    auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
       if (!map_grads) return;
 #pragma unroll
       for (int j = 0; j < G_SLOTS; ++j) {
         const int id = gw + j * GW;
         if (id >= lo && id < hi) {
           const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
-          dw_tile<BPREC3>(recs, npts8, aoff + 16 * mt, boff + 8 * nt, dwacc[j]);
+          const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
+          dw_tile<BPREC3, GREC, true>(recs, npts8, aoff + 16 * mt, boff + 8 * nt, dwacc[j], bd);
         }
       }
     };
     // d w_col1 += c1^T draw   (8-wide n tile over raw[4] + 4 floats of the next record: columns
-    dw_phase(0, 2, R_C1, R_RAW, 1);  //  3..7 are never written out; the last record's overrun
-    group_sync(grp);                 //  stays inside the group's misc block)
+    dw_phase(0, 2, G_C1, G_RAW, 1, -1);  //  3..7 are never written out; the last record's
+    group_sync(grp);                     //  overrun stays inside the kernel's shared memory)
     float draw3 = 0.f;
     if (active) {
-      const float4 dr = *reinterpret_cast<const float4*>(rec + R_RAW);
+      const float4 dr = *reinterpret_cast<const float4*>(rec + G_RAW);
       draw3 = dr.w;
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj) {
         const int j = half * 16 + jj;
         const float* w = sw + SWC1 + j * LDC1;
-        const float c1 = rec[R_C1 + j];
-        rec[R_C1 + j] = (c1 > 0.f) ? (dr.x * w[0] + dr.y * w[1] + dr.z * w[2]) : 0.f;
+        const float c1 = rec[G_C1 + j];
+        rec[G_C1 + j] = (c1 > 0.f) ? (dr.x * w[0] + dr.y * w[1] + dr.z * w[2]) : 0.f;
       }
     }
     group_sync(grp);
     // d w_col0 += [blob, geo, sdf]^T dc1pre   (row 63 is discarded at write-out)
-    dw_phase(2, 18, R_BLOB, R_C1, 4);
+    dw_phase(2, 18, 0, G_C1, 4, 0);
     group_sync(grp);
     if (warp_active) {
       // dgeo = dc1pre Wc0[:, 48:64]  -> dH = [dgeo(15), dsdf]
       float c[2][4];
       zero_c1<2>(c);
-      warp_gemm1<4, 2, true, BPREC3>(wrec, R_C1, sw + SWC0, LDC0, 0, 48, c);
-      store_c1<2, false>(wrec, R_GEO, c);
+      warp_gemm1<4, 2, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 48, c);
+      store_c1<2, false>(wrec, G_GEO, c);
     }
     __syncwarp();
-    if (active && half == 0) rec[R_SDF] = draw3;
+    if (active && half == 0) rec[G_SDF] = draw3;
     group_sync(grp);
     // d w_sdf1 += h1^T dH
-    dw_phase(18, 22, R_H1, R_GEO, 2);
+    dw_phase(18, 22, G_H1, G_GEO, 2, -1);
     group_sync(grp);
     if (warp_active) {
       // dh1pre = (h1 > 0) * (dH W1)
       float c[4][4];
       zero_c1<4>(c);
-      warp_gemm1<2, 4, true, BPREC3>(wrec, R_GEO, sw + SW1, LD1, 0, 0, c);
+      warp_gemm1<2, 4, true, BPREC3>(wrec, G_GEO, sw + SW1, LD1, 0, 0, c);
 #pragma unroll
       for (int nt = 0; nt < 4; ++nt) {
-        float* q0 = wrec + g * REC + R_H1 + nt * 8 + 2 * t;
+        float* q0 = wrec + g * GREC + G_H1 + nt * 8 + 2 * t;
         float2 h0 = *reinterpret_cast<float2*>(q0);
-        float2 h8 = *reinterpret_cast<float2*>(q0 + 8 * REC);
+        float2 h8 = *reinterpret_cast<float2*>(q0 + 8 * GREC);
         *reinterpret_cast<float2*>(q0) =
             make_float2(h0.x > 0.f ? c[nt][0] : 0.f, h0.y > 0.f ? c[nt][1] : 0.f);
-        *reinterpret_cast<float2*>(q0 + 8 * REC) =
+        *reinterpret_cast<float2*>(q0 + 8 * GREC) =
             make_float2(h8.x > 0.f ? c[nt][2] : 0.f, h8.y > 0.f ? c[nt][3] : 0.f);
       }
     }
     group_sync(grp);
     // d w_sdf0 += x^T dh1pre
-    dw_phase(22, 42, R_FEAT, R_H1, 4);
+    dw_phase(22, 42, G_FEAT, G_H1, 4, 2);
     // (readers of C1 / GEO slots are done: dW phases 2 and 3 finished before the last barrier)
     float cfeat[4][4];
     zero_c1<4>(cfeat);
     if (warp_active) {
       if (need_dx) {
         // dblob = dc1pre Wc0[:, 0:48] + dh1pre W0[:, 32:80]  -> scratch (C1 slots 0..31, GEO 32..47)
-        float c[6][4];
-        zero_c1<6>(c);
-        warp_gemm1<4, 6, true, BPREC3>(wrec, R_C1, sw + SWC0, LDC0, 0, 0, c);
-        warp_gemm1<4, 6, true, BPREC3>(wrec, R_H1, sw + SW0, LD0, 0, 32, c);
-        __syncwarp();
-#pragma unroll
-        for (int nt = 0; nt < 6; ++nt) {
-          const int col = nt * 8 + 2 * t;
-          const int off = (col < 32) ? (R_C1 + col) : (R_GEO + col - 32);
-          float* q0 = wrec + g * REC + off;
-          *reinterpret_cast<float2*>(q0) = make_float2(c[nt][0], c[nt][1]);
-          *reinterpret_cast<float2*>(q0 + 8 * REC) = make_float2(c[nt][2], c[nt][3]);
+        // in two passes (register budget): columns 32..47 go to the dead GEO slots at once,
+        // columns 0..31 replace dc1pre after the last read of it
+        {
+          float c[2][4];
+          zero_c1<2>(c);
+          warp_gemm1<4, 2, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 32, c);
+          warp_gemm1<4, 2, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 64, c);
+          store_c1<2, false>(wrec, G_GEO, c);
+        }
+        {
+          float c[4][4];
+          zero_c1<4>(c);
+          warp_gemm1<4, 4, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 0, c);
+          warp_gemm1<4, 4, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 32, c);
+          __syncwarp();
+          store_c1<4, false>(wrec, G_C1, c);
         }
       }
       // dfeat = dh1pre W0[:, 0:32]
-      if (map_grads || need_dx) warp_gemm1<4, 4, true, BPREC3>(wrec, R_H1, sw + SW0, LD0, 0, 0, cfeat);
+      if (map_grads || need_dx) warp_gemm1<4, 4, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 0, cfeat);
     }
     group_sync(grp);  // every warp is past the x^T dh1pre tiles: the FEAT slots are free
-    if (warp_active && (map_grads || need_dx)) store_c1<4, false>(wrec, R_FEAT, cfeat);
+    if (warp_active && (map_grads || need_dx)) store_c1<4, false>(wrec, G_FEAT, cfeat);
     group_sync(grp);
     // ---- hash backward, point-parallel and BALANCED: thread (pp, half) owns levels half, half+2, ..
     // of point pp = every 6th point of the unit per warp (a ray's samples behind the surface carry
@@ -1482,23 +1592,31 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
       const int qd = gt >> 1;
       const int pp = (qd & 15) * GW + (qd >> 4);
       const bool act2 = pp < npts;
-      float* rec2 = recs + pp * REC;
+      float* rec2 = recs + pp * GREC;
       float dxh[3] = {0.f, 0.f, 0.f};
       float xq[3] = {0.f, 0.f, 0.f};
-      if (act2) { xq[0] = xnb[pp * 3]; xq[1] = xnb[pp * 3 + 1]; xq[2] = xnb[pp * 3 + 2]; }
+      const float zq = act2 ? zbuf[pp] : 0.f;
+      if (act2) {
+        // xn of point pp, recomputed exactly as in the forward
+        const int rq = r0 + pp / S;
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+          const float pt = __fadd_rn(P.rays_o[rq * 3 + d], __fmul_rn(P.rays_d[rq * 3 + d], zq));
+          xq[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
+        }
+      }
       if (act2 && (map_grads || need_dx)) {
         const float* jp = (need_dx && P.jac) ? P.jac + ((size_t)((size_t)r0 * S + pp) * 2 + half) * 48 : nullptr;
 #pragma unroll 1
         for (int i2 = 0; i2 < kL / 2; i2 += 2) {  // two levels per call: half + 2 i2, half + 2 i2 + 2
-          bool on[2];
-          float gg[2][2];
+          LevelItems<2> it;
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int l = half + 2 * (i2 + e);
-            const float2 gv = *reinterpret_cast<const float2*>(rec2 + R_FEAT + 2 * l);
-            gg[e][0] = gv.x; gg[e][1] = gv.y;
-            on[e] = l < P.g.n_levels && (gv.x != 0.f || gv.y != 0.f);
-            if (jp && on[e]) {
+            const float2 gv = *reinterpret_cast<const float2*>(rec2 + G_FEAT + 2 * l);
+            it.g[e][0] = gv.x; it.g[e][1] = gv.y;
+            it.on[e] = l < P.g.n_levels && (gv.x != 0.f || gv.y != 0.f);
+            if (jp && it.on[e]) {
               const float2 j0 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e));
               const float2 j1 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e) + 2);
               const float2 j2 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e) + 4);
@@ -1507,9 +1625,10 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
               dxh[2] = fmaf(gv.x, j1.x, fmaf(gv.y, j2.y, dxh[2]));
             }
           }
-          if ((map_grads || (need_dx && !jp)) && (on[0] || on[1])) {
-            const float3 d3 = hash_backward_multi<2>(P, s_lv, half + 2 * i2, on, xq[0], xq[1], xq[2],
-                                                     gg, need_dx && !jp, map_grads, 2);
+          if ((map_grads || (need_dx && !jp)) && (it.on[0] || it.on[1])) {
+            const float3 d3 = hash_backward_multi<2>(P.table, P.d_table, s_lv, half + 2 * i2, it,
+                                                     xq[0], xq[1], xq[2], need_dx && !jp,
+                                                     map_grads, 2);
             dxh[0] += d3.x; dxh[1] += d3.y; dxh[2] += d3.z;
           }
         }
@@ -1520,7 +1639,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         for (int d = 0; d < 3; ++d) dxh[d] += __shfl_xor_sync(0xffffffffu, dxh[d], 1);
         float dp0 = 0.f, dp1 = 0.f;
         if (act2) {
-          auto dblob = [&](int i) { return (i < 32) ? rec2[R_C1 + i] : rec2[R_GEO + i - 32]; };
+          auto dblob = [&](int i) { return (i < 32) ? rec2[G_C1 + i] : rec2[G_GEO + i - 32]; };
           if (half == 0) {
             dp0 = (float)((double)(blob_backward_dim(xq[0], 0, dblob) + dxh[0]) * P.g.binv[0]);
             dp1 = (float)((double)(blob_backward_dim(xq[1], 1, dblob) + dxh[1]) * P.g.binv[1]);
@@ -1530,13 +1649,12 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         }
         __syncwarp();  // both halves have read the dblob scratch before C1[0..5] is reused
         if (act2) {
-          const float zq = zbuf[pp];
           // park d loss / d pts and z * d loss / d pts in the (dead) C1 slots 0..5
           if (half == 0) {
-            rec2[R_C1 + 0] = dp0; rec2[R_C1 + 3] = dp0 * zq;
-            rec2[R_C1 + 1] = dp1; rec2[R_C1 + 4] = dp1 * zq;
+            rec2[G_C1 + 0] = dp0; rec2[G_C1 + 3] = dp0 * zq;
+            rec2[G_C1 + 1] = dp1; rec2[G_C1 + 4] = dp1 * zq;
           } else {
-            rec2[R_C1 + 2] = dp0; rec2[R_C1 + 5] = dp0 * zq;
+            rec2[G_C1 + 2] = dp0; rec2[G_C1 + 5] = dp0 * zq;
           }
         }
       }
@@ -1546,7 +1664,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
       for (int q = gw; q < nr; q += GW) {
         float a[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         for (int kk = lane; kk < S; kk += 32) {
-          const float* rp = recs + (size_t)(q * S + kk) * REC + R_C1;
+          const float* rp = recs + (size_t)(q * S + kk) * GREC + G_C1;
 #pragma unroll
           for (int d = 0; d < 6; ++d) a[d] += rp[d];
         }
@@ -1564,17 +1682,12 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   }
 
   if (BWD) {
-    if (lane == 0) {
-      if (l_rgb != 0.0) atomicAdd(&P.loss_acc[0], l_rgb);
-      if (l_depth != 0.0) atomicAdd(&P.loss_acc[1], l_depth);
-      if (l_sdf != 0.0) atomicAdd(&P.loss_acc[2], l_sdf);
-      if (l_fs != 0.0) atomicAdd(&P.loss_acc[3], l_fs);
-    }
+    __syncthreads();
+    if (tid < 4 && s_loss[tid] != 0.0) atomicAdd(&P.loss_acc[tid], s_loss[tid]);
     if (map_grads) {
       // sum the weight-gradient tiles of the NGROUPS groups in shared memory (the record area is
       // dead now), then one red.global per element and CTA
       float* red = sw + SW_TOTAL;  // [42 tiles][4][32 lanes]
-      __syncthreads();
       for (int gsel = 0; gsel < NGROUPS; ++gsel) {
         if (grp == gsel) {
 #pragma unroll
@@ -1992,10 +2105,12 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   P.jac = nullptr;
   const int sms = num_sms();
   // Kernel choice (rays_per_tile: 0 = automatic, -1 = tile kernel, -2 = grouped kernel, > 0 = tile
-  // kernel with that many rays per tile).  Automatic: the grouped kernel wins the gradient pass
-  // once every group has >= 1 unit in flight after the first wave (R = 4096: 436 vs 459 us,
-  // 16384: 1461 vs 1607, 65536: 5629 vs 6230); the tile kernel wins small batches (tracking,
-  // R = 1024: 182 vs 204 us) and forward-only rendering (160 vs 182 us at 4096 rays).
+  // kernel with that many rays per tile).  Automatic: the grouped kernel runs the gradient pass
+  // once every group has >= 1 unit in flight after the first wave; the tile kernel runs small
+  // batches (tracking) and forward-only rendering.  On H100 (400 W) the grouped kernel takes
+  // 0.514 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
+  // random rays (mode 1) the two are close: tile / grouped fwd+bwd R = 1024: 214 / 195 us,
+  // 4096: 462 / 468, 16384: 1470 / 1520, 65536: 5463 / 5818 us; the rule is unchanged.
   bool grouped = false;
   if (S <= GP) {
     const int units = (R + GP / S - 1) / (GP / S);
@@ -2010,11 +2125,20 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
                                            align_up((size_t)R * S * sizeof(float), 256))
                 : nullptr;
     int* queue = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 128);  // zeroed above
-    const size_t smem_g = sizeof(float) * ((size_t)SW_TOTAL + (size_t)NGROUPS * GP * (REC + 6));
+    // weights + NGROUPS x GP records + one z value per slot: 180 352 B.  Four groups would fit
+    // (231 424 B) but need <= 80 registers per thread and spill more; with three, the ~48 KB
+    // of shared memory left over serve as L1 for the gathers (1.25x the step rate on H100).
+    const size_t smem_g = sizeof(float) * ((size_t)SW_TOTAL + (size_t)NGROUPS * GP * (GREC + 1));
+    int dev = 0, smem_optin = 0;
+    XRD_CUDA_TRY(cudaGetDevice(&dev));
+    XRD_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     int gridx = (P.n_tiles + NGROUPS - 1) / NGROUPS;
     if (gridx > sms) gridx = sms;
 #define XRD_LAUNCH_G(KERNEL)                                                                      \
   do {                                                                                            \
+    cudaFuncAttributes fa;                                                                        \
+    XRD_CUDA_TRY(cudaFuncGetAttributes(&fa, KERNEL));                                             \
+    if (smem_g + fa.sharedSizeBytes > (size_t)smem_optin) return XRD_E_SHAPE;                     \
     XRD_CUDA_TRY(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
                                       (int)smem_g));                                              \
     KernelTimer kt(stream);                                                                       \
