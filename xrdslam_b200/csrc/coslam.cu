@@ -11,7 +11,7 @@
 //   k_sample   one warp per ray: merge the 32 uniform + 11 depth-guided samples,
 //              stratified jitter, batch-global counts n_fs / n_sdf / n_valid.
 //   k_fused    persistent CTAs over tiles of NR rays (NR*S points, one thread per
-//              point for the gathers).  Per-point fp32 record in shared memory:
+//              point for the gathers).  Per-point fp32 record in shared memory, dense:
 //                [feat32 | blob48 | geo15 | sdf | h1_32 | c1_32 | raw4]   (stride 164)
 //              The decoder runs on the tensor cores: every warp pushes its own 32
 //              points through mma.sync m16n8k8 TF32 tiles whose A fragments are read
@@ -24,9 +24,12 @@
 //              points on the K axis, accumulated in registers for the whole launch;
 //              the hash backward runs in the MMA fragment layout (lane (g,t) owns
 //              level 4*nt+t of rows g, g+8) and scatters with red.global.add.v2.f32.
+//   k_fused_g  the same arithmetic through the same device functions, scheduled as
+//              independent groups of warps with named barriers, one m-tile per warp, a
+//              132-float record with OneBlob in compact form and a balanced
+//              point-parallel hash backward (see its comment).
 //   k_finalize loss accumulators -> the 4 weighted loss terms.
 #include <math.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -35,9 +38,24 @@ namespace coslam {
 
 constexpr int kL = XRD_MAX_LEVELS;
 constexpr int kBins = 16;
-// record layout (floats); stride == 4 (mod 32) keeps 128-bit LDS conflict-free
+// Per-point records (floats); stride == 4 (mod 32) keeps 128-bit LDS conflict-free.
+// Dense (tile kernel, k_query): [feat32 | blob48 | geo15 | sdf | h1 32 | c1 32 | raw4], stride 164.
 constexpr int R_FEAT = 0, R_BLOB = 32, R_GEO = 80, R_SDF = 95, R_H1 = 96, R_C1 = 128,
               R_RAW = 160, REC = 164;
+// Compact (grouped kernel), stride 132: the 48 OneBlob bins are kept in compact form
+// (blob_compact_dim), so that the decoder-input columns outside the OneBlob block sit at their
+// own index: [feat 0..31 | blob] for the SDF decoder, [blob | geo 48..62 | sdf 63] for the colour
+// decoder.  The tile kernel keeps the dense record: on the compact one its gradient pass is
+// slower (DESIGN.md section 4.1).
+constexpr int G_FEAT = 0, G_BLOB = 32, G_GEO = 48, G_SDF = 63, G_H1 = 64, G_C1 = 96, G_RAW = 128,
+              GREC = 132;
+// per-layout offsets for the code both kernels share
+template <bool COMPACT>
+struct Rec {
+  static constexpr int N = COMPACT ? GREC : REC, GEO = COMPACT ? G_GEO : R_GEO,
+                       H1 = COMPACT ? G_H1 : R_H1, C1 = COMPACT ? G_C1 : R_C1,
+                       RAW = COMPACT ? G_RAW : R_RAW;
+};
 struct GridDev {
   float scale[kL];
   uint32_t res[kL], size[kL], offset[kL], hashed[kL];
@@ -68,8 +86,6 @@ struct Params {
   double* loss_acc;   // 4 sums
   int NR;             // rays per tile
   int n_tiles;
-  float* jac;         // k_fused_g: [R*S][2 halves][8 levels][6] d feat / d xn, written by the forward
-                      // gather when position gradients are wanted (replaces the backward re-gather)
 };
 
 // ------------------------------------------------------------------ sample ---
@@ -247,6 +263,31 @@ __device__ __forceinline__ void blob_forward(const float xn[3], float* __restric
   }
 }
 
+// Compact form of one coordinate: the three images fill windows of 3 bins that lie 15..17 bins
+// apart (16 up to the rounding of x - s), so no bin gets two contributions, at most 4 of the 16
+// bins are non-zero (for any x, inside the bounding box or not) and two non-zero bins never agree
+// mod 4.  Bin b is kept in slot b & 3: v[b & 3] holds exactly the float of the dense sum
+// (0 + contribution) and byte b & 3 of q holds b >> 2.
+// Dense bin b = (q[b & 3] == b >> 2) ? v[b & 3] : 0; empty slots hold value 0.
+// Per point: [v dim0 (4) | v dim1 (4) | v dim2 (4) | q dim0 | q dim1 | q dim2 | unused].
+__device__ __forceinline__ void blob_compact_dim(float x, float* __restrict__ v,
+                                                 uint8_t* __restrict__ q) {
+  *reinterpret_cast<float4*>(v) = make_float4(0.f, 0.f, 0.f, 0.f);
+  *reinterpret_cast<uint32_t*>(q) = 0u;
+#pragma unroll
+  for (int s = -1; s <= 1; ++s) {
+    const float u = (x - (float)s) * (float)kBins;
+    const float fl = floorf(u);
+    if (fl < -1.f || fl > (float)kBins) continue;
+    const int b0 = (int)fl;
+    const float f = u - fl;
+    const float c0 = qcdf(-f), c1 = qcdf(1.f - f);
+    if (b0 - 1 >= 0 && b0 - 1 < kBins) { v[(b0 - 1) & 3] = 0.f + c0; q[(b0 - 1) & 3] = (uint8_t)((b0 - 1) >> 2); }
+    if (b0 >= 0 && b0 < kBins) { v[b0 & 3] = 0.f + (c1 - c0); q[b0 & 3] = (uint8_t)(b0 >> 2); }
+    if (b0 + 1 >= 0 && b0 + 1 < kBins) { v[(b0 + 1) & 3] = 0.f + (1.f - c1); q[(b0 + 1) & 3] = (uint8_t)((b0 + 1) >> 2); }
+  }
+}
+
 // d/dx of dimension d's 16 OneBlob outputs, contracted with dblob (read through the functor)
 template <typename F>
 __device__ __forceinline__ float blob_backward_dim(float x, int d, F dblob) {
@@ -277,40 +318,43 @@ __device__ __forceinline__ void blob_backward(const float xn[3], F dblob, float 
   }
 }
 
-__device__ __forceinline__ void encode_point(const Params& P, const Lv* __restrict__ lv,
-                                             const float xn[3], float* __restrict__ rec) {
-  const float2* __restrict__ tab = reinterpret_cast<const float2*>(P.table);
-#pragma unroll 4
-  for (int l = 0; l < kL; ++l) {
-    if (l >= P.g.n_levels) {
-      rec[R_FEAT + 2 * l] = 0.f;
-      rec[R_FEAT + 2 * l + 1] = 0.f;
-      continue;
-    }
-    float w[3];
-    uint32_t c[3];
-    const Lv L = lv[l];
-    pos_fract(xn[0], L.scale, w[0], c[0]);
-    pos_fract(xn[1], L.scale, w[1], c[1]);
-    pos_fract(xn[2], L.scale, w[2], c[2]);
-    float2 v[8];
+// the two features of level L at xn, trilinear over the 8 corners (all 8 loads issued first)
+__device__ __forceinline__ float2 level_feature(const float2* __restrict__ tab, const Lv& L,
+                                                const float xn[3]) {
+  float w[3];
+  uint32_t c[3];
+  pos_fract(xn[0], L.scale, w[0], c[0]);
+  pos_fract(xn[1], L.scale, w[1], c[1]);
+  pos_fract(xn[2], L.scale, w[2], c[2]);
+  float2 v[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      uint32_t idx = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1),
-                                c[2] + ((k >> 2) & 1));
-      v[k] = __ldg(&tab[idx]);
-    }
-    float f0 = 0.f, f1 = 0.f;
+  for (int k = 0; k < 8; ++k)
+    v[k] = __ldg(&tab[grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1))]);
+  float f0 = 0.f, f1 = 0.f;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
-                 ((k & 4) ? w[2] : 1.f - w[2]);
-      f0 = fmaf(wk, v[k].x, f0);
-      f1 = fmaf(wk, v[k].y, f1);
-    }
-    *reinterpret_cast<float2*>(rec + R_FEAT + 2 * l) = make_float2(f0, f1);
+  for (int k = 0; k < 8; ++k) {
+    const float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
+                     ((k & 4) ? w[2] : 1.f - w[2]);
+    f0 = fmaf(wk, v[k].x, f0);
+    f1 = fmaf(wk, v[k].y, f1);
   }
-  blob_forward(xn, rec);
+  return make_float2(f0, f1);
+}
+
+// Hash features of xn into a record (FEAT = 0 in both layouts): levels l0, l0 + LSTRIDE, ...
+// Tile kernel and k_query: one thread per point, (l0, LSTRIDE) = (0, 1); grouped kernel: two
+// threads per point, (half, 2).
+template <int LSTRIDE>
+__device__ __forceinline__ void encode(const float* __restrict__ table, int n_levels,
+                                       const Lv* __restrict__ lv, const float xn[3],
+                                       float* __restrict__ rec, int l0) {
+  const float2* __restrict__ tab = reinterpret_cast<const float2*>(table);
+#pragma unroll(4 / LSTRIDE)
+  for (int i = 0; i < kL / LSTRIDE; ++i) {
+    const int l = l0 + LSTRIDE * i;
+    *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) =
+        (l < n_levels) ? level_feature(tab, lv[l], xn) : make_float2(0.f, 0.f);
+  }
 }
 
 // NL (point, level) items of the hash backward per call (scatter (g0,g1), optional d/dx).
@@ -447,21 +491,46 @@ __device__ __forceinline__ void mma(float (&d)[4], const FragA<PREC3>& a, const 
   mma_tf32(d, a.big, b.big);
 }
 
-// C[mt][nt] += A * B for the 32 points of this warp (2 m-tiles of 16 rows).
-//   A[row][k]   = wrec[row*REC + aoff + k]              (activations / gradients, records)
-//   B[k][n]     = TRANS ? w[(noff+n)*ld + koff + k] : w[(koff+k)*ld + noff + n]
-template <int KS, int NT, bool TRANS, bool PREC3>
+// A fragment of k-step kb of the dense 48-column OneBlob block for rows g, g + 8 of 16 compact
+// records: lane t needs bins t, t + 4 of dimension kb >> 1, half kb & 1, i.e. slot t with
+// quarters 2 (kb & 1) and 2 (kb & 1) + 1.
+__device__ __forceinline__ void blob_frag(const float* __restrict__ mrec, int kb, int g, int t,
+                                          float (&v)[4]) {
+  const int d = kb >> 1;
+  const uint32_t m = 2u * (uint32_t)(kb & 1);
+  const float* r0 = mrec + g * GREC + G_BLOB;
+  const float* r8 = r0 + 8 * GREC;
+  const float a0 = r0[4 * d + t], a8 = r8[4 * d + t];
+  const uint32_t q0 = reinterpret_cast<const uint8_t*>(r0 + 12 + d)[t];
+  const uint32_t q8 = reinterpret_cast<const uint8_t*>(r8 + 12 + d)[t];
+  v[0] = (q0 == m) ? a0 : 0.f;
+  v[1] = (q8 == m) ? a8 : 0.f;
+  v[2] = (q0 == m + 1) ? a0 : 0.f;
+  v[3] = (q8 == m + 1) ? a8 : 0.f;
+}
+
+// C[mt][nt] += A * B for MT m-tiles of 16 records of stride STRIDE from wrec (tile kernel: 2 per
+// warp, every B fragment serves both; grouped kernel: 1).
+//   A[row][k] = wrec[row*STRIDE + aoff + k], except k-steps [BK0, BK0 + 6): the 48-column OneBlob
+//               block, expanded from compact records
+//   B[k][n]   = TRANS ? w[(noff+n)*ld + koff + k] : w[(koff+k)*ld + noff + n]
+template <int KS, int NT, bool TRANS, bool PREC3, int STRIDE, int BK0 = -1, int MT>
 __device__ __forceinline__ void warp_gemm(const float* __restrict__ wrec, int aoff,
                                           const float* __restrict__ w, int ld, int koff,
-                                          int noff, float (&c)[2][NT][4]) {
+                                          int noff, float (&c)[MT][NT][4]) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll 1
   for (int ks = 0; ks < KS; ++ks) {
-    FragA<PREC3> a[2];
+    FragA<PREC3> a[MT];
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
-      const float* r0 = wrec + (mt * 16 + g) * REC + aoff + ks * 8 + t;
-      const float v[4] = {r0[0], r0[8 * REC], r0[4], r0[8 * REC + 4]};
+    for (int mt = 0; mt < MT; ++mt) {
+      float v[4];
+      if (BK0 >= 0 && ks >= BK0 && ks < BK0 + 6) {
+        blob_frag(wrec + mt * 16 * GREC, ks - BK0, g, t, v);
+      } else {
+        const float* r0 = wrec + (mt * 16 + g) * STRIDE + aoff + ks * 8 + t;
+        v[0] = r0[0]; v[1] = r0[8 * STRIDE]; v[2] = r0[4]; v[3] = r0[8 * STRIDE + 4];
+      }
       a[mt].set(v);
     }
 #pragma unroll
@@ -470,36 +539,43 @@ __device__ __forceinline__ void warp_gemm(const float* __restrict__ wrec, int ao
       const int k0 = koff + ks * 8 + t, n0 = noff + nt * 8 + g;
       if (TRANS) b.set(w[n0 * ld + k0], w[n0 * ld + k0 + 4]);
       else b.set(w[k0 * ld + n0], w[(k0 + 4) * ld + n0]);
-      mma<PREC3>(c[0][nt], a[0], b);
-      mma<PREC3>(c[1][nt], a[1], b);
+#pragma unroll
+      for (int mt = 0; mt < MT; ++mt) mma<PREC3>(c[mt][nt], a[mt], b);
     }
   }
 }
 
-template <int NT>
-__device__ __forceinline__ void zero_c(float (&c)[2][NT][4]) {
+template <int MT, int NT>
+__device__ __forceinline__ void zero_c(float (&c)[MT][NT][4]) {
 #pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
+  for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
       for (int i = 0; i < 4; ++i) c[mt][nt][i] = 0.f;
 }
 
-// store C (32 rows x 8*NT cols) into the records at column offset coff (float2 per row pair)
-template <int NT, bool RELU>
+// store C (16 MT rows x 8 NT cols) into the records at column offset coff (float2 per row pair).
+// RELU: max(c, 0); MASK: c where the value it replaces is > 0, else 0 (ReLU backward in place)
+enum Store { PLAIN, RELU, MASK };
+template <Store OP, int STRIDE, int MT, int NT>
 __device__ __forceinline__ void store_c(float* __restrict__ wrec, int coff,
-                                        const float (&c)[2][NT][4]) {
+                                        const float (&c)[MT][NT][4]) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll
-  for (int mt = 0; mt < 2; ++mt)
+  for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
       float v0 = c[mt][nt][0], v1 = c[mt][nt][1], v2 = c[mt][nt][2], v3 = c[mt][nt][3];
-      if (RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
-      float* r0 = wrec + (mt * 16 + g) * REC + coff + nt * 8 + 2 * t;
+      float* r0 = wrec + (mt * 16 + g) * STRIDE + coff + nt * 8 + 2 * t;
+      if (OP == RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
+      if (OP == MASK) {
+        const float2 h0 = *reinterpret_cast<float2*>(r0), h8 = *reinterpret_cast<float2*>(r0 + 8 * STRIDE);
+        v0 = h0.x > 0.f ? v0 : 0.f; v1 = h0.y > 0.f ? v1 : 0.f;
+        v2 = h8.x > 0.f ? v2 : 0.f; v3 = h8.y > 0.f ? v3 : 0.f;
+      }
       *reinterpret_cast<float2*>(r0) = make_float2(v0, v1);
-      *reinterpret_cast<float2*>(r0 + 8 * REC) = make_float2(v2, v3);
+      *reinterpret_cast<float2*>(r0 + 8 * STRIDE) = make_float2(v2, v3);
     }
 }
 
@@ -514,13 +590,6 @@ constexpr int SW_TOTAL = SWC1 + 32 * LDC1; // 6784 floats
 // weight-gradient tiles (16 in-features x 8 out-units each), global order
 //   [0,2) d w_col1   [2,18) d w_col0   [18,22) d w_sdf1   [22,42) d w_sdf0
 constexpr int DW_TILES = 42;
-
-// record of the grouped kernel (k_fused_g), stride 132 == 4 (mod 32): the 48 OneBlob bins are
-// kept in compact form (blob_compact_dim), so that the decoder-input columns outside the OneBlob
-// block sit at their own index: [feat 0..31 | blob] for the SDF decoder, [blob | geo 48..62 |
-// sdf 63] for the colour decoder.
-constexpr int G_FEAT = 0, G_BLOB = 32, G_GEO = 48, G_SDF = 63, G_H1 = 64, G_C1 = 96, G_RAW = 128,
-              GREC = 132;
 
 // A fragment values of the dense OneBlob bins (g, g + 8) of dimension bd for points p0 (k-slot t)
 // and p1 (k-slot t + 4), expanded from the compact form: both bins live in slot g & 3, with
@@ -540,10 +609,10 @@ __device__ __forceinline__ void blob_dw_frag(const float* __restrict__ p0,
 }
 
 // STRIDE: record stride; BLOB && bd >= 0: the 16 A rows are the OneBlob bins of dimension bd of a
-// compact grouped-kernel record (aoff unused).
-template <bool PREC3, int STRIDE = REC, bool BLOB = false>
+// compact record (aoff unused).
+template <bool PREC3, int STRIDE, bool BLOB>
 __device__ __forceinline__ void dw_tile(const float* __restrict__ recs, int npts, int aoff,
-                                        int boff, float (&acc)[4], int bd = -1) {
+                                        int boff, float (&acc)[4], int bd) {
   // acc[16 x 8] += sum_p A[p][aoff + m] * B[p][boff + n]; k-slot t <-> point 2t, t+4 <-> 2t+1
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll 2
@@ -564,6 +633,175 @@ __device__ __forceinline__ void dw_tile(const float* __restrict__ recs, int npts
   }
 }
 
+// The decoders for MT m-tiles of 16 records at wrec: h1, [geo, sdf], c1 and the rgb logits
+// (RAW[0..2]; RAW[3] = sdf is the caller's).  Caller: one warp.
+// COMPACT: the OneBlob A fragments are expanded from compact records.
+template <bool PREC3, int MT, bool COMPACT>
+__device__ __forceinline__ void decoder_forward(float* __restrict__ wrec, const float* __restrict__ sw) {
+  using L = Rec<COMPACT>;
+  constexpr int N = L::N;
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  {  // h1 = relu([feat, blob] W0^T)
+    float c[MT][4][4];
+    zero_c(c);
+    warp_gemm<10, 4, false, PREC3, N, COMPACT ? 4 : -1>(wrec, R_FEAT, sw + SW0, LD0, 0, 0, c);
+    store_c<RELU, N>(wrec, L::H1, c);
+  }
+  __syncwarp();
+  {  // [geo, sdf] = h1 W1^T
+    float c[MT][2][4];
+    zero_c(c);
+    warp_gemm<4, 2, false, PREC3, N>(wrec, L::H1, sw + SW1, LD1, 0, 0, c);
+    store_c<PLAIN, N>(wrec, L::GEO, c);
+  }
+  __syncwarp();
+  {  // c1 = relu([blob, geo, (sdf: zero weight row)] Wc0^T)
+    float c[MT][4][4];
+    zero_c(c);
+    warp_gemm<8, 4, false, PREC3, N, COMPACT ? 0 : -1>(wrec, COMPACT ? 0 : R_BLOB, sw + SWC0, LDC0, 0, 0, c);
+    store_c<RELU, N>(wrec, L::C1, c);
+  }
+  __syncwarp();
+  {  // rgb logits = c1 Wc1^T (cols 0..2 of an 8-wide tile)
+    float c[MT][1][4];
+    zero_c(c);
+    warp_gemm<4, 1, false, PREC3, N>(wrec, L::C1, sw + SWC1, LDC1, 0, 0, c);
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) {
+      float* q0 = wrec + (mt * 16 + g) * N + L::RAW;
+      if (t == 0) {
+        q0[0] = c[mt][0][0]; q0[1] = c[mt][0][1];
+        q0[8 * N] = c[mt][0][2]; q0[8 * N + 1] = c[mt][0][3];
+      } else if (t == 1) {
+        q0[2] = c[mt][0][0];
+        q0[8 * N + 2] = c[mt][0][2];
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// Zeroes the weight area, then stages the transposed decoder weights (zero padding included).
+// Whole CTA; the caller synchronises before the first read.
+__device__ __forceinline__ void stage_weights(float* __restrict__ sw, const Params& P) {
+  for (int q = threadIdx.x; q < SW_TOTAL; q += blockDim.x) sw[q] = 0.f;
+  __syncthreads();
+  for (int q = threadIdx.x; q < 80 * 32; q += blockDim.x) {
+    int i = q / 32, j = q % 32;
+    sw[SW0 + i * LD0 + j] = P.w_sdf0[j * 80 + i];
+  }
+  for (int q = threadIdx.x; q < 32 * 16; q += blockDim.x) {
+    int i = q / 16, jp = q % 16;  // jp: geo0..14 -> torch out 1..15, jp 15 -> out 0 (sdf)
+    int jt = (jp + 1) & 15;
+    sw[SW1 + i * LD1 + jp] = P.w_sdf1[jt * 32 + i];
+  }
+  for (int q = threadIdx.x; q < 63 * 32; q += blockDim.x) {
+    int i = q / 32, j = q % 32;
+    sw[SWC0 + i * LDC0 + j] = P.w_col0[j * 63 + i];
+  }
+  for (int q = threadIdx.x; q < 32 * 3; q += blockDim.x) {
+    int i = q / 3, k = q % 3;
+    sw[SWC1 + i * LDC1 + k] = P.w_col1[k * 32 + i];
+  }
+}
+
+// loss normalisers of the gradient pass (batch-global counts n_fs, n_sdf, n_valid)
+struct LossNorm {
+  float fs_w = 0.f, sdf_w = 0.f, inv_nvalid = 0.f;
+};
+__device__ __forceinline__ LossNorm loss_norm(const int* __restrict__ counts) {
+  LossNorm ln;
+  const float n_fs = (float)counts[0], n_sdf = (float)counts[1];
+  const float n = (float)(counts[0] + counts[1]);
+  ln.fs_w = 1.0f - n_fs / n;
+  ln.sdf_w = 1.0f - n_sdf / n;
+  ln.inv_nvalid = 1.0f / (float)counts[2];
+  return ln;
+}
+
+// This warp's share of one weight-gradient layer: tiles [lo, hi) of the 42, slot j holds tile
+// w + j * nw.  m-tile mt of the layer input covers its columns 16 mt .. 16 mt + 15 at record
+// offset aoff; m-tiles [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form.
+template <bool PREC3, bool COMPACT, int SLOTS>
+__device__ __forceinline__ void dw_layer(const float* __restrict__ recs, int npts, int w, int nw,
+                                         float (&acc)[SLOTS][4], int lo, int hi, int aoff,
+                                         int boff, int n_tiles_n, int blob_mt) {
+#pragma unroll
+  for (int j = 0; j < SLOTS; ++j) {
+    const int id = w + j * nw;
+    if (id >= lo && id < hi) {
+      const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
+      const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
+      dw_tile<PREC3, Rec<COMPACT>::N, COMPACT>(recs, npts, aoff + 16 * mt, boff + 8 * nt, acc[j], bd);
+    }
+  }
+}
+
+// Adds weight-gradient tile id (this lane's C fragment v; rows = in-feature, cols = out-unit) to
+// the weight gradients in global memory.
+__device__ __forceinline__ void dw_store(const Params& P, int id, const float (&v)[4]) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int rloc = g + ((i & 2) ? 8 : 0), cloc = 2 * t + (i & 1);
+    if (id < 2) {  // d w_col1 [3][32]
+      const int in = 16 * id + rloc, out = cloc;
+      if (out < 3) red_add(P.d_w_col1 + out * 32 + in, v[i]);
+    } else if (id < 18) {  // d w_col0 [32][63]
+      const int loc = id - 2, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
+      if (in < 63) red_add(P.d_w_col0 + out * 63 + in, v[i]);
+    } else if (id < 22) {  // d w_sdf1 [16][32], stored column jp -> torch row (jp+1)&15
+      const int loc = id - 18, in = 16 * (loc / 2) + rloc, jp = 8 * (loc % 2) + cloc;
+      red_add(P.d_w_sdf1 + ((jp + 1) & 15) * 32 + in, v[i]);
+    } else {  // d w_sdf0 [32][80]
+      const int loc = id - 22, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
+      red_add(P.d_w_sdf0 + out * 80 + in, v[i]);
+    }
+  }
+}
+
+// d_rays_o / d_rays_d of ray rr (one warp): sums over its S records (rq) of d loss / d pts and
+// z * d loss / d pts, parked in C1 slots 0..5
+template <bool COMPACT>
+__device__ __forceinline__ void ray_grads(const Params& P, const float* __restrict__ rq, int rr,
+                                          int lane) {
+  float a[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int kk = lane; kk < P.S; kk += 32) {
+    const float* rp = rq + (size_t)kk * Rec<COMPACT>::N + Rec<COMPACT>::C1;
+#pragma unroll
+    for (int d = 0; d < 6; ++d) a[d] += rp[d];
+  }
+#pragma unroll
+  for (int d = 0; d < 6; ++d) a[d] = warp_sum(a[d]);
+  if (lane == 0) {
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      if (P.d_rays_o) P.d_rays_o[rr * 3 + d] = a[d];
+      if (P.d_rays_d) P.d_rays_d[rr * 3 + d] = a[3 + d];
+    }
+  }
+}
+
+// dgeo = dc1pre Wc0[:, 48:64] -> dH = [dgeo(15), dsdf] in the GEO slots (SDF is the caller's),
+// then dh1pre = (h1 > 0) * (dH W1) in place of h1; the caller's barrier and dW layer run between
+// the two.  One warp, MT m-tiles.
+template <bool PREC3, int MT, bool COMPACT>
+__device__ __forceinline__ void backward_geo(float* __restrict__ wrec, const float* __restrict__ sw) {
+  using L = Rec<COMPACT>;
+  float c[MT][2][4];
+  zero_c(c);
+  warp_gemm<4, 2, true, PREC3, L::N>(wrec, L::C1, sw + SWC0, LDC0, 0, 48, c);
+  store_c<PLAIN, L::N>(wrec, L::GEO, c);
+}
+template <bool PREC3, int MT, bool COMPACT>
+__device__ __forceinline__ void backward_h1(float* __restrict__ wrec, const float* __restrict__ sw) {
+  using L = Rec<COMPACT>;
+  float c[MT][4][4];
+  zero_c(c);
+  warp_gemm<2, 4, true, PREC3, L::N>(wrec, L::GEO, sw + SW1, LD1, 0, 0, c);
+  store_c<MASK, L::N>(wrec, L::H1, c);
+}
+
 // ----------------------------------------------------------------- fused ---
 template <bool BWD, bool PREC3, bool BPREC3, int SLOTS>
 __global__ void __launch_bounds__(256) k_fused(const Params P) {
@@ -581,37 +819,10 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
 
   __shared__ Lv s_lv[kL];
   load_levels(s_lv, P.g);
-  // stage transposed weights (zero padding included)
-  for (int q = tid; q < SW_TOTAL; q += blockDim.x) sw[q] = 0.f;
-  __syncthreads();
-  for (int q = tid; q < 80 * 32; q += blockDim.x) {
-    int i = q / 32, j = q % 32;
-    sw[SW0 + i * LD0 + j] = P.w_sdf0[j * 80 + i];
-  }
-  for (int q = tid; q < 32 * 16; q += blockDim.x) {
-    int i = q / 16, jp = q % 16;  // jp: geo0..14 -> torch out 1..15, jp 15 -> out 0 (sdf)
-    int jt = (jp + 1) & 15;
-    sw[SW1 + i * LD1 + jp] = P.w_sdf1[jt * 32 + i];
-  }
-  for (int q = tid; q < 63 * 32; q += blockDim.x) {
-    int i = q / 32, j = q % 32;
-    sw[SWC0 + i * LDC0 + j] = P.w_col0[j * 63 + i];
-  }
-  for (int q = tid; q < 32 * 3; q += blockDim.x) {
-    int i = q / 3, k = q % 3;
-    sw[SWC1 + i * LDC1 + k] = P.w_col1[k * 32 + i];
-  }
+  stage_weights(sw, P);
   // the 8 pad records after the tile stay zero for the whole kernel (k-step overrun of dw_tile)
   for (int q = tid; q < 8 * REC; q += blockDim.x) recs[blockDim.x * REC + q] = 0.f;
-
-  float fs_w = 0.f, sdf_w = 0.f, inv_nvalid = 0.f;
-  if (BWD) {
-    const float n_fs = (float)P.counts[0], n_sdf = (float)P.counts[1];
-    const float n = (float)(P.counts[0] + P.counts[1]);
-    fs_w = 1.0f - n_fs / n;
-    sdf_w = 1.0f - n_sdf / n;
-    inv_nvalid = 1.0f / (float)P.counts[2];
-  }
+  const LossNorm ln = BWD ? loss_norm(P.counts) : LossNorm{};
   double l_rgb = 0.0, l_depth = 0.0, l_sdf = 0.0, l_fs = 0.0;
   float dwacc[SLOTS][4];
 #pragma unroll
@@ -646,7 +857,8 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
         xnb[tid * 3 + d] = xn[d];
       }
-      encode_point(P, s_lv, xn, rec);
+      encode<1>(P.table, P.g.n_levels, s_lv, xn, rec, 0);
+      blob_forward(xn, rec);
     } else {
       // inactive rows must read as zero in every GEMM (k-dimension of the dW tiles)
 #pragma unroll 1
@@ -654,46 +866,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         *reinterpret_cast<float4*>(rec + q) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     __syncwarp();
-    if (warp_active) {
-      {  // h1 = relu(x W0^T)
-        float c[2][4][4];
-        zero_c<4>(c);
-        warp_gemm<10, 4, false, PREC3>(wrec, R_FEAT, sw + SW0, LD0, 0, 0, c);
-        store_c<4, true>(wrec, R_H1, c);
-      }
-      __syncwarp();
-      {  // [geo, sdf] = h1 W1^T
-        float c[2][2][4];
-        zero_c<2>(c);
-        warp_gemm<4, 2, false, PREC3>(wrec, R_H1, sw + SW1, LD1, 0, 0, c);
-        store_c<2, false>(wrec, R_GEO, c);
-      }
-      __syncwarp();
-      {  // c1 = relu([blob, geo, (sdf: zero weight row)] Wc0^T)
-        float c[2][4][4];
-        zero_c<4>(c);
-        warp_gemm<8, 4, false, PREC3>(wrec, R_BLOB, sw + SWC0, LDC0, 0, 0, c);
-        store_c<4, true>(wrec, R_C1, c);
-      }
-      __syncwarp();
-      {  // rgb logits = c1 Wc1^T (cols 0..2 of an 8-wide tile)
-        float c[2][1][4];
-        zero_c<1>(c);
-        warp_gemm<4, 1, false, PREC3>(wrec, R_C1, sw + SWC1, LDC1, 0, 0, c);
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt) {
-          float* q0 = wrec + (mt * 16 + g) * REC + R_RAW;
-          if (t == 0) {
-            q0[0] = c[mt][0][0]; q0[1] = c[mt][0][1];
-            q0[8 * REC] = c[mt][0][2]; q0[8 * REC + 1] = c[mt][0][3];
-          } else if (t == 1) {
-            q0[2] = c[mt][0][0];
-            q0[8 * REC + 2] = c[mt][0][2];
-          }
-        }
-      }
-      __syncwarp();
-    }
+    if (warp_active) decoder_forward<PREC3, 2, false>(wrec, sw);
     if (active) {
       rec[R_RAW + 3] = rec[R_SDF];
       if (P.raw) {
@@ -771,7 +944,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         const float RS = (float)P.Rg * (float)S;
         const float c_rgb = P.ls[0] * P.w_rgb * 2.0f / (3.0f * (float)P.Rg);
         const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
-        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * inv_nvalid : 0.f;
+        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * ln.inv_nvalid : 0.f;
         if (lane == 0) {
           l_rgb += (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
                             (o_b - tb_) * (o_b - tb_));
@@ -785,8 +958,8 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         }
         qw = warp_sum(qw);
         float a_fs = 0.f, a_sdf = 0.f;
-        const float c_fs = P.ls[3] * P.w_fs * fs_w * 2.0f / RS;
-        const float c_sdf = P.ls[2] * P.w_sdf * sdf_w * 2.0f / RS;
+        const float c_fs = P.ls[3] * P.w_fs * ln.fs_w * 2.0f / RS;
+        const float c_sdf = P.ls[2] * P.w_sdf * ln.sdf_w * 2.0f / RS;
         for (int kk = lane; kk < S; kk += 32) {
           float* rp = rq + kk * REC + R_RAW;
           const float z = zr[kk];
@@ -822,19 +995,12 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     if (!BWD) continue;
     // ---------------- phase 3: backward ----------------------------------
     // weight-gradient tiles owned by this warp: tile id = warp + j * nwarps
-    auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n) {
-      if (!map_grads) return;
-#pragma unroll
-      for (int j = 0; j < SLOTS; ++j) {
-        const int id = warp + j * nwarps;
-        if (id >= lo && id < hi) {
-          const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
-          dw_tile<BPREC3>(recs, npts, aoff + 16 * mt, boff + 8 * nt, dwacc[j]);
-        }
-      }
+    auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
+      if (map_grads)
+        dw_layer<BPREC3, false>(recs, npts, warp, nwarps, dwacc, lo, hi, aoff, boff, n_tiles_n, blob_mt);
     };
     // d w_col1 += c1^T draw        (8-wide n tile over raw[4] + 4 floats of the next record:
-    dw_phase(0, 2, R_C1, R_RAW, 1);  //  columns 3..7 are never written out)
+    dw_phase(0, 2, R_C1, R_RAW, 1, -1);  //  columns 3..7 are never written out)
     __syncthreads();
     float draw3 = 0.f;
     if (active) {
@@ -849,42 +1015,19 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     }
     __syncthreads();
     // d w_col0 += [blob, geo, sdf]^T dc1pre   (row 63 is discarded at write-out)
-    dw_phase(2, 18, R_BLOB, R_C1, 4);
+    dw_phase(2, 18, R_BLOB, R_C1, 4, -1);
     __syncthreads();
-    if (warp_active) {
-      // dgeo = dc1pre Wc0[:, 48:64]  -> dH = [dgeo(15), dsdf]
-      float c[2][2][4];
-      zero_c<2>(c);
-      warp_gemm<4, 2, true, BPREC3>(wrec, R_C1, sw + SWC0, LDC0, 0, 48, c);
-      store_c<2, false>(wrec, R_GEO, c);
-    }
+    if (warp_active) backward_geo<BPREC3, 2, false>(wrec, sw);
     __syncwarp();
     if (active) rec[R_SDF] = draw3;
     __syncthreads();
     // d w_sdf1 += h1^T dH
-    dw_phase(18, 22, R_H1, R_GEO, 2);
+    dw_phase(18, 22, R_H1, R_GEO, 2, -1);
     __syncthreads();
-    if (warp_active) {
-      // dh1pre = (h1 > 0) * (dH W1)
-      float c[2][4][4];
-      zero_c<4>(c);
-      warp_gemm<2, 4, true, BPREC3>(wrec, R_GEO, sw + SW1, LD1, 0, 0, c);
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          float* q0 = wrec + (mt * 16 + g) * REC + R_H1 + nt * 8 + 2 * t;
-          float2 h0 = *reinterpret_cast<float2*>(q0);
-          float2 h8 = *reinterpret_cast<float2*>(q0 + 8 * REC);
-          *reinterpret_cast<float2*>(q0) =
-              make_float2(h0.x > 0.f ? c[mt][nt][0] : 0.f, h0.y > 0.f ? c[mt][nt][1] : 0.f);
-          *reinterpret_cast<float2*>(q0 + 8 * REC) =
-              make_float2(h8.x > 0.f ? c[mt][nt][2] : 0.f, h8.y > 0.f ? c[mt][nt][3] : 0.f);
-        }
-    }
+    if (warp_active) backward_h1<BPREC3, 2, false>(wrec, sw);
     __syncthreads();
     // d w_sdf0 += x^T dh1pre
-    dw_phase(22, 42, R_FEAT, R_H1, 4);
+    dw_phase(22, 42, R_FEAT, R_H1, 4, -1);
     // (readers of C1 / GEO slots are done: dW phases 2 and 3 finished before the last barrier)
     float hdx[2][2][3];  // hash-path d loss / d x for rows (mt, g / g+8), fragment layout
 #pragma unroll
@@ -895,9 +1038,9 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
       if (need_dx) {
         // dblob = dc1pre Wc0[:, 0:48] + dh1pre W0[:, 32:80]  -> scratch (C1 slots 0..31, GEO 32..47)
         float c[2][6][4];
-        zero_c<6>(c);
-        warp_gemm<4, 6, true, BPREC3>(wrec, R_C1, sw + SWC0, LDC0, 0, 0, c);
-        warp_gemm<4, 6, true, BPREC3>(wrec, R_H1, sw + SW0, LD0, 0, 32, c);
+        zero_c(c);
+        warp_gemm<4, 6, true, BPREC3, REC>(wrec, R_C1, sw + SWC0, LDC0, 0, 0, c);
+        warp_gemm<4, 6, true, BPREC3, REC>(wrec, R_H1, sw + SW0, LD0, 0, 32, c);
         __syncwarp();
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
@@ -913,8 +1056,8 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
       if (map_grads || need_dx) {
         // dfeat = dh1pre W0[:, 0:32]; lane (g,t) holds (f0,f1) of level 4*nt+t for rows g, g+8
         float c[2][4][4];
-        zero_c<4>(c);
-        warp_gemm<4, 4, true, BPREC3>(wrec, R_H1, sw + SW0, LD0, 0, 0, c);
+        zero_c(c);
+        warp_gemm<4, 4, true, BPREC3, REC>(wrec, R_H1, sw + SW0, LD0, 0, 0, c);
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -969,23 +1112,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     }
     __syncthreads();
     if (need_dx) {
-      for (int q = warp; q < nr; q += nwarps) {
-        float a[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int kk = lane; kk < S; kk += 32) {
-          const float* rp = recs + (size_t)(q * S + kk) * REC + R_C1;
-#pragma unroll
-          for (int d = 0; d < 6; ++d) a[d] += rp[d];
-        }
-#pragma unroll
-        for (int d = 0; d < 6; ++d) a[d] = warp_sum(a[d]);
-        if (lane == 0) {
-#pragma unroll
-          for (int d = 0; d < 3; ++d) {
-            if (P.d_rays_o) P.d_rays_o[(r0 + q) * 3 + d] = a[d];
-            if (P.d_rays_d) P.d_rays_d[(r0 + q) * 3 + d] = a[3 + d];
-          }
-        }
-      }
+      for (int q = warp; q < nr; q += nwarps) ray_grads<false>(P, recs + (size_t)(q * S) * REC, r0 + q, lane);
       __syncthreads();
     }
   }
@@ -998,34 +1125,14 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
       if (l_fs != 0.0) atomicAdd(&P.loss_acc[3], l_fs);
     }
     if (map_grads) {
-      // write out the weight-gradient tiles: C(16 x 8): rows = in-feature, cols = out-unit
 #pragma unroll
       for (int j = 0; j < SLOTS; ++j) {
         const int id = warp + j * nwarps;
-        if (id >= DW_TILES) continue;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float v = dwacc[j][i];
-          const int rloc = g + ((i & 2) ? 8 : 0), cloc = 2 * t + (i & 1);
-          if (id < 2) {  // d w_col1 [3][32]
-            const int in = 16 * id + rloc, out = cloc;
-            if (out < 3) red_add(P.d_w_col1 + out * 32 + in, v);
-          } else if (id < 18) {  // d w_col0 [32][63]
-            const int loc = id - 2, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
-            if (in < 63) red_add(P.d_w_col0 + out * 63 + in, v);
-          } else if (id < 22) {  // d w_sdf1 [16][32], stored column jp -> torch row (jp+1)&15
-            const int loc = id - 18, in = 16 * (loc / 2) + rloc, jp = 8 * (loc % 2) + cloc;
-            red_add(P.d_w_sdf1 + ((jp + 1) & 15) * 32 + in, v);
-          } else {  // d w_sdf0 [32][80]
-            const int loc = id - 22, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
-            red_add(P.d_w_sdf0 + out * 80 + in, v);
-          }
-        }
+        if (id < DW_TILES) dw_store(P, id, dwacc[j]);
       }
     }
   }
 }
-
 
 // ----------------------------------------------------------- fused, grouped ---
 // v5: the same record-based algorithm, re-organised for latency hiding.  One persistent CTA
@@ -1049,162 +1156,6 @@ __device__ __forceinline__ void group_sync(int grp) {
   asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(GT) : "memory");
 }
 
-// OneBlob of one coordinate in compact form.  The three images s = -1, 0, 1 of blob_forward fill
-// windows of 3 bins that lie 15..17 bins apart (16 up to the rounding of x - s), so no bin gets
-// two contributions, at most 4 of the 16 bins are non-zero (for any x, inside the bounding box or
-// not) and two non-zero bins never agree mod 4.  Bin b is kept in slot b & 3: v[b & 3] holds
-// exactly the float of the dense form (0 + contribution) and byte b & 3 of q holds b >> 2.
-// Dense bin b = (q[b & 3] == b >> 2) ? v[b & 3] : 0; empty slots hold value 0.
-// Per point: [v dim0 (4) | v dim1 (4) | v dim2 (4) | q dim0 | q dim1 | q dim2 | unused].
-__device__ __forceinline__ void blob_compact_dim(float x, float* __restrict__ v,
-                                                 uint8_t* __restrict__ q) {
-  *reinterpret_cast<float4*>(v) = make_float4(0.f, 0.f, 0.f, 0.f);
-  *reinterpret_cast<uint32_t*>(q) = 0u;
-#pragma unroll
-  for (int s = -1; s <= 1; ++s) {
-    const float u = (x - (float)s) * (float)kBins;
-    const float fl = floorf(u);
-    if (fl < -1.f || fl > (float)kBins) continue;
-    const int b0 = (int)fl;
-    const float f = u - fl;
-    const float c0 = qcdf(-f), c1 = qcdf(1.f - f);
-    if (b0 - 1 >= 0 && b0 - 1 < kBins) { v[(b0 - 1) & 3] = 0.f + c0; q[(b0 - 1) & 3] = (uint8_t)((b0 - 1) >> 2); }
-    if (b0 >= 0 && b0 < kBins) { v[b0 & 3] = 0.f + (c1 - c0); q[b0 & 3] = (uint8_t)(b0 >> 2); }
-    if (b0 + 1 >= 0 && b0 + 1 < kBins) { v[(b0 + 1) & 3] = 0.f + (1.f - c1); q[(b0 + 1) & 3] = (uint8_t)((b0 + 1) >> 2); }
-  }
-}
-
-// A fragment of k-step kb of the dense 48-column OneBlob block for rows g, g + 8 of a warp's
-// compact records: lane t needs bins t, t + 4 of dimension kb >> 1, half kb & 1, i.e. slot t with
-// quarters 2 (kb & 1) and 2 (kb & 1) + 1.
-__device__ __forceinline__ void blob_frag(const float* __restrict__ wrec, int kb, int g, int t,
-                                          float (&v)[4]) {
-  const int d = kb >> 1;
-  const uint32_t m = 2u * (uint32_t)(kb & 1);
-  const float* r0 = wrec + g * GREC + G_BLOB;
-  const float* r8 = r0 + 8 * GREC;
-  const float a0 = r0[4 * d + t], a8 = r8[4 * d + t];
-  const uint32_t q0 = reinterpret_cast<const uint8_t*>(r0 + 12 + d)[t];
-  const uint32_t q8 = reinterpret_cast<const uint8_t*>(r8 + 12 + d)[t];
-  v[0] = (q0 == m) ? a0 : 0.f;
-  v[1] = (q8 == m) ? a8 : 0.f;
-  v[2] = (q0 == m + 1) ? a0 : 0.f;
-  v[3] = (q8 == m + 1) ? a8 : 0.f;
-}
-
-// hash levels half, half+2, ... and the OneBlob dims of this half (0: x,y  1: z)
-__device__ __forceinline__ void encode_half(const Params& P, const Lv* __restrict__ lv,
-                                            const float xn[3], float* __restrict__ rec, int half,
-                                            float* __restrict__ jac) {
-  const float2* __restrict__ tab = reinterpret_cast<const float2*>(P.table);
-#pragma unroll 2
-  for (int i = 0; i < kL / 2; ++i) {
-    const int l = half + 2 * i;
-    if (l >= P.g.n_levels) {
-      *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) = make_float2(0.f, 0.f);
-      if (jac) {
-        *reinterpret_cast<float2*>(jac + 6 * i) = make_float2(0.f, 0.f);
-        *reinterpret_cast<float2*>(jac + 6 * i + 2) = make_float2(0.f, 0.f);
-        *reinterpret_cast<float2*>(jac + 6 * i + 4) = make_float2(0.f, 0.f);
-      }
-      continue;
-    }
-    float w[3];
-    uint32_t c[3];
-    const Lv L = lv[l];
-    pos_fract(xn[0], L.scale, w[0], c[0]);
-    pos_fract(xn[1], L.scale, w[1], c[1]);
-    pos_fract(xn[2], L.scale, w[2], c[2]);
-    float2 v[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      uint32_t idx = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
-      v[k] = __ldg(&tab[idx]);
-    }
-    float f0 = 0.f, f1 = 0.f;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
-                 ((k & 4) ? w[2] : 1.f - w[2]);
-      f0 = fmaf(wk, v[k].x, f0);
-      f1 = fmaf(wk, v[k].y, f1);
-    }
-    *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) = make_float2(f0, f1);
-    if (jac) {
-      // d feat / d xn while the 8 corners are in registers: [f0: dx dy dz | f1: dx dy dz] * scale
-      const float w0 = w[0], w1 = w[1], w2 = w[2], sc = L.scale;
-      const float a00 = (1 - w1) * (1 - w2), a10 = w1 * (1 - w2), a01 = (1 - w1) * w2, a11 = w1 * w2;
-      const float b00 = (1 - w0) * (1 - w2), b10 = w0 * (1 - w2), b01 = (1 - w0) * w2, b11 = w0 * w2;
-      const float c00 = (1 - w0) * (1 - w1), c10 = w0 * (1 - w1), c01 = (1 - w0) * w1, c11 = w0 * w1;
-      const float jx0 = a00 * (v[1].x - v[0].x) + a10 * (v[3].x - v[2].x) + a01 * (v[5].x - v[4].x) + a11 * (v[7].x - v[6].x);
-      const float jy0 = b00 * (v[2].x - v[0].x) + b10 * (v[3].x - v[1].x) + b01 * (v[6].x - v[4].x) + b11 * (v[7].x - v[5].x);
-      const float jz0 = c00 * (v[4].x - v[0].x) + c10 * (v[5].x - v[1].x) + c01 * (v[6].x - v[2].x) + c11 * (v[7].x - v[3].x);
-      const float jx1 = a00 * (v[1].y - v[0].y) + a10 * (v[3].y - v[2].y) + a01 * (v[5].y - v[4].y) + a11 * (v[7].y - v[6].y);
-      const float jy1 = b00 * (v[2].y - v[0].y) + b10 * (v[3].y - v[1].y) + b01 * (v[6].y - v[4].y) + b11 * (v[7].y - v[5].y);
-      const float jz1 = c00 * (v[4].y - v[0].y) + c10 * (v[5].y - v[1].y) + c01 * (v[6].y - v[2].y) + c11 * (v[7].y - v[3].y);
-      *reinterpret_cast<float2*>(jac + 6 * i) = make_float2(sc * jx0, sc * jy0);
-      *reinterpret_cast<float2*>(jac + 6 * i + 2) = make_float2(sc * jz0, sc * jx1);
-      *reinterpret_cast<float2*>(jac + 6 * i + 4) = make_float2(sc * jy1, sc * jz1);
-    }
-  }
-  // (constant indices into xn: a run-time index would put it in local memory)
-  const int d0 = half ? 2 : 0;
-  blob_compact_dim(half ? xn[2] : xn[0], rec + G_BLOB + 4 * d0,
-                   reinterpret_cast<uint8_t*>(rec + G_BLOB + 12 + d0));
-  if (!half)
-    blob_compact_dim(xn[1], rec + G_BLOB + 4, reinterpret_cast<uint8_t*>(rec + G_BLOB + 13));
-}
-
-// one 16-row m-tile: C[nt] += A * B   (A rows = wrec[row*GREC + aoff + k]; k-steps
-// [BK0, BK0 + 6) are the 48-column OneBlob block instead, expanded from the compact records)
-template <int KS, int NT, bool TRANS, bool PREC3, int BK0 = -1>
-__device__ __forceinline__ void warp_gemm1(const float* __restrict__ wrec, int aoff,
-                                           const float* __restrict__ w, int ld, int koff,
-                                           int noff, float (&c)[NT][4]) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-#pragma unroll 1
-  for (int ks = 0; ks < KS; ++ks) {
-    FragA<PREC3> a;
-    {
-      float v[4];
-      if (BK0 >= 0 && ks >= BK0 && ks < BK0 + 6) {
-        blob_frag(wrec, ks - BK0, g, t, v);
-      } else {
-        const float* r0 = wrec + g * GREC + aoff + ks * 8 + t;
-        v[0] = r0[0]; v[1] = r0[8 * GREC]; v[2] = r0[4]; v[3] = r0[8 * GREC + 4];
-      }
-      a.set(v);
-    }
-#pragma unroll
-    for (int nt = 0; nt < NT; ++nt) {
-      FragB<PREC3> b;
-      const int k0 = koff + ks * 8 + t, n0 = noff + nt * 8 + g;
-      if (TRANS) b.set(w[n0 * ld + k0], w[n0 * ld + k0 + 4]);
-      else b.set(w[k0 * ld + n0], w[(k0 + 4) * ld + n0]);
-      mma<PREC3>(c[nt], a, b);
-    }
-  }
-}
-template <int NT>
-__device__ __forceinline__ void zero_c1(float (&c)[NT][4]) {
-#pragma unroll
-  for (int nt = 0; nt < NT; ++nt)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) c[nt][i] = 0.f;
-}
-template <int NT, bool RELU>
-__device__ __forceinline__ void store_c1(float* __restrict__ wrec, int coff, const float (&c)[NT][4]) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int nt = 0; nt < NT; ++nt) {
-    float v0 = c[nt][0], v1 = c[nt][1], v2 = c[nt][2], v3 = c[nt][3];
-    if (RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
-    float* r0 = wrec + g * GREC + coff + nt * 8 + 2 * t;
-    *reinterpret_cast<float2*>(r0) = make_float2(v0, v1);
-    *reinterpret_cast<float2*>(r0 + 8 * GREC) = make_float2(v2, v3);
-  }
-}
-
 template <bool BWD, bool PREC3, bool BPREC3>
 __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int* __restrict__ queue) {
   extern __shared__ __align__(16) float smem[];
@@ -1212,7 +1163,6 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   const int tid = threadIdx.x;
   const int grp = tid / GT, gt = tid - grp * GT;
   const int gw = gt >> 5, lane = gt & 31;
-  const int g = lane >> 2, t = lane & 3;
   float* recs = sw + SW_TOTAL + grp * (GP * GREC);
   float* zbuf = sw + SW_TOTAL + NGROUPS * (GP * GREC) + grp * GP;  // GP z values
   const int S = P.S;
@@ -1222,35 +1172,9 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   __shared__ double s_loss[4];  // loss sums of the CTA (registers are the scarce resource here)
   load_levels(s_lv, P.g);
   if (tid < 4) s_loss[tid] = 0.0;
-  for (int q = tid; q < SW_TOTAL; q += blockDim.x) sw[q] = 0.f;
   for (int q = gt; q < GP * GREC; q += GT) recs[q] = 0.f;
-  __syncthreads();
-  for (int q = tid; q < 80 * 32; q += blockDim.x) {
-    int i = q / 32, j = q % 32;
-    sw[SW0 + i * LD0 + j] = P.w_sdf0[j * 80 + i];
-  }
-  for (int q = tid; q < 32 * 16; q += blockDim.x) {
-    int i = q / 16, jp = q % 16;  // jp: geo0..14 -> torch out 1..15, jp 15 -> out 0 (sdf)
-    int jt = (jp + 1) & 15;
-    sw[SW1 + i * LD1 + jp] = P.w_sdf1[jt * 32 + i];
-  }
-  for (int q = tid; q < 63 * 32; q += blockDim.x) {
-    int i = q / 32, j = q % 32;
-    sw[SWC0 + i * LDC0 + j] = P.w_col0[j * 63 + i];
-  }
-  for (int q = tid; q < 32 * 3; q += blockDim.x) {
-    int i = q / 3, k = q % 3;
-    sw[SWC1 + i * LDC1 + k] = P.w_col1[k * 32 + i];
-  }
-
-  float fs_w = 0.f, sdf_w = 0.f, inv_nvalid = 0.f;
-  if (BWD) {
-    const float n_fs = (float)P.counts[0], n_sdf = (float)P.counts[1];
-    const float n = (float)(P.counts[0] + P.counts[1]);
-    fs_w = 1.0f - n_fs / n;
-    sdf_w = 1.0f - n_sdf / n;
-    inv_nvalid = 1.0f / (float)P.counts[2];
-  }
+  stage_weights(sw, P);
+  const LossNorm ln = BWD ? loss_norm(P.counts) : LossNorm{};
   float dwacc[G_SLOTS][4];
 #pragma unroll
   for (int j = 0; j < G_SLOTS; ++j)
@@ -1289,8 +1213,14 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
       }
       if (half == 0) zbuf[p] = zv;
-      encode_half(P, s_lv, xn, rec, half,
-                  (need_dx && P.jac) ? P.jac + ((size_t)((size_t)r * S + k) * 2 + half) * 48 : nullptr);
+      encode<2>(P.table, P.g.n_levels, s_lv, xn, rec, half);
+      // OneBlob dims 0, 1 (half 0) and 2 (half 1); constant indices keep xn in registers
+      if (half) {
+        blob_compact_dim(xn[2], rec + G_BLOB + 8, reinterpret_cast<uint8_t*>(rec + G_BLOB + 14));
+      } else {
+        blob_compact_dim(xn[0], rec + G_BLOB, reinterpret_cast<uint8_t*>(rec + G_BLOB + 12));
+        blob_compact_dim(xn[1], rec + G_BLOB + 4, reinterpret_cast<uint8_t*>(rec + G_BLOB + 13));
+      }
     } else if (p < prev_npts) {
       // rows left dirty by a larger unit must read as zero in every GEMM
       float* z0 = rec + half * (GREC / 2);
@@ -1299,43 +1229,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     }
     prev_npts = npts;
     __syncwarp();
-    if (warp_active) {
-      {  // h1 = relu([feat, blob] W0^T)
-        float c[4][4];
-        zero_c1<4>(c);
-        warp_gemm1<10, 4, false, PREC3, 4>(wrec, G_FEAT, sw + SW0, LD0, 0, 0, c);
-        store_c1<4, true>(wrec, G_H1, c);
-      }
-      __syncwarp();
-      {  // [geo, sdf] = h1 W1^T
-        float c[2][4];
-        zero_c1<2>(c);
-        warp_gemm1<4, 2, false, PREC3>(wrec, G_H1, sw + SW1, LD1, 0, 0, c);
-        store_c1<2, false>(wrec, G_GEO, c);
-      }
-      __syncwarp();
-      {  // c1 = relu([blob, geo, (sdf: zero weight row)] Wc0^T)
-        float c[4][4];
-        zero_c1<4>(c);
-        warp_gemm1<8, 4, false, PREC3, 0>(wrec, 0, sw + SWC0, LDC0, 0, 0, c);
-        store_c1<4, true>(wrec, G_C1, c);
-      }
-      __syncwarp();
-      {  // rgb logits = c1 Wc1^T (cols 0..2 of an 8-wide tile)
-        float c[1][4];
-        zero_c1<1>(c);
-        warp_gemm1<4, 1, false, PREC3>(wrec, G_C1, sw + SWC1, LDC1, 0, 0, c);
-        float* q0 = wrec + g * GREC + G_RAW;
-        if (t == 0) {
-          q0[0] = c[0][0]; q0[1] = c[0][1];
-          q0[8 * GREC] = c[0][2]; q0[8 * GREC + 1] = c[0][3];
-        } else if (t == 1) {
-          q0[2] = c[0][0];
-          q0[8 * GREC + 2] = c[0][2];
-        }
-      }
-      __syncwarp();
-    }
+    if (warp_active) decoder_forward<PREC3, 1, true>(wrec, sw);
     if (active && half == 0) {
       rec[G_RAW + 3] = rec[G_SDF];
       if (P.raw) {
@@ -1430,7 +1324,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         const float RS = (float)P.Rg * (float)S;
         const float c_rgb = P.ls[0] * P.w_rgb * 2.0f / (3.0f * (float)P.Rg);
         const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
-        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * inv_nvalid : 0.f;
+        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * ln.inv_nvalid : 0.f;
         if (lane == 0) {
           atomicAdd(&s_loss[0], (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
                                          (o_b - tb_) * (o_b - tb_)));
@@ -1448,8 +1342,8 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         }
         qw = warp_sum(qw);
         float a_fs = 0.f, a_sdf = 0.f;
-        const float c_fs = P.ls[3] * P.w_fs * fs_w * 2.0f / RS;
-        const float c_sdf = P.ls[2] * P.w_sdf * sdf_w * 2.0f / RS;
+        const float c_fs = P.ls[3] * P.w_fs * ln.fs_w * 2.0f / RS;
+        const float c_sdf = P.ls[2] * P.w_sdf * ln.sdf_w * 2.0f / RS;
 #pragma unroll
         for (int i = 0; i < G_KPL; ++i) {
           const int kk = lane + 32 * i;
@@ -1487,20 +1381,9 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     if (!BWD) continue;  // the barrier at the top of the loop orders the next unit
     group_sync(grp);
     // ---------------- phase 3: backward ----------------------------------
-    const int npts8 = (npts + 7) & ~7;
-    // m-tile mt of a layer input covers its columns 16 mt .. 16 mt + 15 at record offset aoff;
-    // m-tiles [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form
     auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
-      if (!map_grads) return;
-#pragma unroll
-      for (int j = 0; j < G_SLOTS; ++j) {
-        const int id = gw + j * GW;
-        if (id >= lo && id < hi) {
-          const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
-          const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
-          dw_tile<BPREC3, GREC, true>(recs, npts8, aoff + 16 * mt, boff + 8 * nt, dwacc[j], bd);
-        }
-      }
+      if (map_grads)
+        dw_layer<BPREC3, true>(recs, npts, gw, GW, dwacc, lo, hi, aoff, boff, n_tiles_n, blob_mt);
     };
     // d w_col1 += c1^T draw   (8-wide n tile over raw[4] + 4 floats of the next record: columns
     dw_phase(0, 2, G_C1, G_RAW, 1, -1);  //  3..7 are never written out; the last record's
@@ -1521,73 +1404,51 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     // d w_col0 += [blob, geo, sdf]^T dc1pre   (row 63 is discarded at write-out)
     dw_phase(2, 18, 0, G_C1, 4, 0);
     group_sync(grp);
-    if (warp_active) {
-      // dgeo = dc1pre Wc0[:, 48:64]  -> dH = [dgeo(15), dsdf]
-      float c[2][4];
-      zero_c1<2>(c);
-      warp_gemm1<4, 2, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 48, c);
-      store_c1<2, false>(wrec, G_GEO, c);
-    }
+    if (warp_active) backward_geo<BPREC3, 1, true>(wrec, sw);
     __syncwarp();
     if (active && half == 0) rec[G_SDF] = draw3;
     group_sync(grp);
     // d w_sdf1 += h1^T dH
     dw_phase(18, 22, G_H1, G_GEO, 2, -1);
     group_sync(grp);
-    if (warp_active) {
-      // dh1pre = (h1 > 0) * (dH W1)
-      float c[4][4];
-      zero_c1<4>(c);
-      warp_gemm1<2, 4, true, BPREC3>(wrec, G_GEO, sw + SW1, LD1, 0, 0, c);
-#pragma unroll
-      for (int nt = 0; nt < 4; ++nt) {
-        float* q0 = wrec + g * GREC + G_H1 + nt * 8 + 2 * t;
-        float2 h0 = *reinterpret_cast<float2*>(q0);
-        float2 h8 = *reinterpret_cast<float2*>(q0 + 8 * GREC);
-        *reinterpret_cast<float2*>(q0) =
-            make_float2(h0.x > 0.f ? c[nt][0] : 0.f, h0.y > 0.f ? c[nt][1] : 0.f);
-        *reinterpret_cast<float2*>(q0 + 8 * GREC) =
-            make_float2(h8.x > 0.f ? c[nt][2] : 0.f, h8.y > 0.f ? c[nt][3] : 0.f);
-      }
-    }
+    if (warp_active) backward_h1<BPREC3, 1, true>(wrec, sw);
     group_sync(grp);
     // d w_sdf0 += x^T dh1pre
     dw_phase(22, 42, G_FEAT, G_H1, 4, 2);
     // (readers of C1 / GEO slots are done: dW phases 2 and 3 finished before the last barrier)
-    float cfeat[4][4];
-    zero_c1<4>(cfeat);
+    float cfeat[1][4][4];
+    zero_c(cfeat);
     if (warp_active) {
       if (need_dx) {
         // dblob = dc1pre Wc0[:, 0:48] + dh1pre W0[:, 32:80]  -> scratch (C1 slots 0..31, GEO 32..47)
         // in two passes (register budget): columns 32..47 go to the dead GEO slots at once,
         // columns 0..31 replace dc1pre after the last read of it
         {
-          float c[2][4];
-          zero_c1<2>(c);
-          warp_gemm1<4, 2, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 32, c);
-          warp_gemm1<4, 2, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 64, c);
-          store_c1<2, false>(wrec, G_GEO, c);
+          float c[1][2][4];
+          zero_c(c);
+          warp_gemm<4, 2, true, BPREC3, GREC>(wrec, G_C1, sw + SWC0, LDC0, 0, 32, c);
+          warp_gemm<4, 2, true, BPREC3, GREC>(wrec, G_H1, sw + SW0, LD0, 0, 64, c);
+          store_c<PLAIN, GREC>(wrec, G_GEO, c);
         }
         {
-          float c[4][4];
-          zero_c1<4>(c);
-          warp_gemm1<4, 4, true, BPREC3>(wrec, G_C1, sw + SWC0, LDC0, 0, 0, c);
-          warp_gemm1<4, 4, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 32, c);
+          float c[1][4][4];
+          zero_c(c);
+          warp_gemm<4, 4, true, BPREC3, GREC>(wrec, G_C1, sw + SWC0, LDC0, 0, 0, c);
+          warp_gemm<4, 4, true, BPREC3, GREC>(wrec, G_H1, sw + SW0, LD0, 0, 32, c);
           __syncwarp();
-          store_c1<4, false>(wrec, G_C1, c);
+          store_c<PLAIN, GREC>(wrec, G_C1, c);
         }
       }
       // dfeat = dh1pre W0[:, 0:32]
-      if (map_grads || need_dx) warp_gemm1<4, 4, true, BPREC3>(wrec, G_H1, sw + SW0, LD0, 0, 0, cfeat);
+      if (map_grads || need_dx) warp_gemm<4, 4, true, BPREC3, GREC>(wrec, G_H1, sw + SW0, LD0, 0, 0, cfeat);
     }
     group_sync(grp);  // every warp is past the x^T dh1pre tiles: the FEAT slots are free
-    if (warp_active && (map_grads || need_dx)) store_c1<4, false>(wrec, G_FEAT, cfeat);
+    if (warp_active && (map_grads || need_dx)) store_c<PLAIN, GREC>(wrec, G_FEAT, cfeat);
     group_sync(grp);
     // ---- hash backward, point-parallel and BALANCED: thread (pp, half) owns levels half, half+2, ..
     // of point pp = every 6th point of the unit per warp (a ray's samples behind the surface carry
     // no gradient: ray-major assignment would leave whole warps idle).  d loss / d xn comes from
-    // the Jacobian cached by the forward gather (no second gather); the table gradient is
-    // scattered with red.global.add.v2.
+    // a second gather of the corners; the table gradient is scattered with red.global.add.v2.
     {
       const int qd = gt >> 1;
       const int pp = (qd & 15) * GW + (qd >> 4);
@@ -1606,7 +1467,6 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         }
       }
       if (act2 && (map_grads || need_dx)) {
-        const float* jp = (need_dx && P.jac) ? P.jac + ((size_t)((size_t)r0 * S + pp) * 2 + half) * 48 : nullptr;
 #pragma unroll 1
         for (int i2 = 0; i2 < kL / 2; i2 += 2) {  // two levels per call: half + 2 i2, half + 2 i2 + 2
           LevelItems<2> it;
@@ -1616,18 +1476,10 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
             const float2 gv = *reinterpret_cast<const float2*>(rec2 + G_FEAT + 2 * l);
             it.g[e][0] = gv.x; it.g[e][1] = gv.y;
             it.on[e] = l < P.g.n_levels && (gv.x != 0.f || gv.y != 0.f);
-            if (jp && it.on[e]) {
-              const float2 j0 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e));
-              const float2 j1 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e) + 2);
-              const float2 j2 = *reinterpret_cast<const float2*>(jp + 6 * (i2 + e) + 4);
-              dxh[0] = fmaf(gv.x, j0.x, fmaf(gv.y, j1.y, dxh[0]));
-              dxh[1] = fmaf(gv.x, j0.y, fmaf(gv.y, j2.x, dxh[1]));
-              dxh[2] = fmaf(gv.x, j1.x, fmaf(gv.y, j2.y, dxh[2]));
-            }
           }
-          if ((map_grads || (need_dx && !jp)) && (it.on[0] || it.on[1])) {
+          if (it.on[0] || it.on[1]) {
             const float3 d3 = hash_backward_multi<2>(P.table, P.d_table, s_lv, half + 2 * i2, it,
-                                                     xq[0], xq[1], xq[2], need_dx && !jp,
+                                                     xq[0], xq[1], xq[2], need_dx,
                                                      map_grads, 2);
             dxh[0] += d3.x; dxh[1] += d3.y; dxh[2] += d3.z;
           }
@@ -1661,23 +1513,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     }
     if (need_dx) {
       group_sync(grp);
-      for (int q = gw; q < nr; q += GW) {
-        float a[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        for (int kk = lane; kk < S; kk += 32) {
-          const float* rp = recs + (size_t)(q * S + kk) * GREC + G_C1;
-#pragma unroll
-          for (int d = 0; d < 6; ++d) a[d] += rp[d];
-        }
-#pragma unroll
-        for (int d = 0; d < 6; ++d) a[d] = warp_sum(a[d]);
-        if (lane == 0) {
-#pragma unroll
-          for (int d = 0; d < 3; ++d) {
-            if (P.d_rays_o) P.d_rays_o[(r0 + q) * 3 + d] = a[d];
-            if (P.d_rays_d) P.d_rays_d[(r0 + q) * 3 + d] = a[3 + d];
-          }
-        }
-      }
+      for (int q = gw; q < nr; q += GW) ray_grads<true>(P, recs + (size_t)(q * S) * GREC, r0 + q, lane);
     }
   }
 
@@ -1708,24 +1544,10 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
         for (int j = 0; j < G_SLOTS; ++j) {
           const int id = gw + j * GW;
           if (id >= DW_TILES) continue;
+          float v[4];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float v = red[(id * 4 + i) * 32 + lane];
-            const int rloc = g + ((i & 2) ? 8 : 0), cloc = 2 * t + (i & 1);
-            if (id < 2) {  // d w_col1 [3][32]
-              const int in = 16 * id + rloc, out = cloc;
-              if (out < 3) red_add(P.d_w_col1 + out * 32 + in, v);
-            } else if (id < 18) {  // d w_col0 [32][63]
-              const int loc = id - 2, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
-              if (in < 63) red_add(P.d_w_col0 + out * 63 + in, v);
-            } else if (id < 22) {  // d w_sdf1 [16][32], stored column jp -> torch row (jp+1)&15
-              const int loc = id - 18, in = 16 * (loc / 2) + rloc, jp = 8 * (loc % 2) + cloc;
-              red_add(P.d_w_sdf1 + ((jp + 1) & 15) * 32 + in, v);
-            } else {  // d w_sdf0 [32][80]
-              const int loc = id - 22, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
-              red_add(P.d_w_sdf0 + out * 80 + in, v);
-            }
-          }
+          for (int i = 0; i < 4; ++i) v[i] = red[(id * 4 + i) * 32 + lane];
+          dw_store(P, id, v);
         }
       }
     }
@@ -1929,10 +1751,8 @@ __global__ void __launch_bounds__(128) k_query(const QueryParams Q) {
     const float v = Q.pts[(size_t)p * 3 + d];
     xn[d] = Q.normalised ? v : normalise(v, Q.g.bmin[d], Q.g.bmax[d]);
   }
-  Params P{};  // encode_point reads table / n_levels only
-  P.table = Q.table;
-  P.g.n_levels = Q.g.n_levels;
-  encode_point(P, s_lv, xn, rec);
+  encode<1>(Q.table, Q.g.n_levels, s_lv, xn, rec, 0);
+  blob_forward(xn, rec);
   if (Q.feat)
 #pragma unroll 4
     for (int j = 0; j < 32; ++j) Q.feat[(size_t)p * 32 + j] = rec[R_FEAT + j];
@@ -2000,24 +1820,9 @@ static int fill_grid(GridDev& g, const XrdHashGrid* h) {
 using namespace xrd;
 using namespace xrd::coslam;
 
-// Optional Jacobian cache of the grouped kernel (2 halves x 8 levels x 6 floats per sample point):
-// the forward gather stores d feat / d xn so that the backward needs no second gather for the ray
-// gradients.  The table is L2-resident and the cache is 384 B/point of extra traffic, so it is
-// off unless XRD_COSLAM_JAC is set; kept for tables that outgrow L2.
-static constexpr size_t kJacBytesPerPoint = 2 * 48 * sizeof(float);
-static constexpr size_t kJacMaxBytes = (size_t)512 << 20;  // beyond this the backward re-gathers
-static bool jac_enabled() {
-  static const bool on = getenv("XRD_COSLAM_JAC") != nullptr;
-  return on;
-}
-static size_t jac_bytes(int n_rays, int n_samples) {
-  if (!jac_enabled()) return 0;
-  const size_t b = (size_t)n_rays * n_samples * kJacBytesPerPoint;
-  return b <= kJacMaxBytes ? b : 0;
-}
 extern "C" size_t xrd_coslam_workspace_bytes(int n_rays, int n_samples) {
-  // [counts int[4] | loss_acc double[4] | z_vals R*S floats | Jacobian cache]
-  return 256 + align_up((size_t)n_rays * n_samples * sizeof(float), 256) + jac_bytes(n_rays, n_samples);
+  // [counts int[4] | loss_acc double[4] | z_vals R*S floats]
+  return 256 + align_up((size_t)n_rays * n_samples * sizeof(float), 256);
 }
 
 static int pick_rays_per_tile(int S, int requested) {
@@ -2025,6 +1830,47 @@ static int pick_rays_per_tile(int S, int requested) {
   // largest NR with NR*S <= 224 -> for S=43: 5 rays, 215 points, 224 threads
   int nr = 224 / S;
   return nr < 1 ? 1 : nr;  // S in (224, 256]: one ray per 256-thread tile
+}
+
+template <bool BWD, bool PREC3, bool BPREC3>
+struct TileKernel {
+  static constexpr auto fn = &k_fused<BWD, PREC3, BPREC3, BWD ? 6 : 1>;
+};
+template <bool BWD, bool PREC3, bool BPREC3>
+struct GroupedKernel {
+  static constexpr auto fn = &k_fused_g<BWD, PREC3, BPREC3>;
+};
+
+// The instantiation of fused kernel K for a pass.  cfg.precision: 0 = 3xTF32 everywhere, 1 =
+// 3xTF32 forward + TF32 backward, 2 = TF32 everywhere; NULL for a gradient pass in another mode.
+template <template <bool, bool, bool> class K>
+static decltype(K<false, false, false>::fn) fused_kernel(bool grads, int precision) {
+  if (!grads) return precision <= 1 ? K<false, true, false>::fn : K<false, false, false>::fn;
+  switch (precision) {
+    case 0: return K<true, true, true>::fn;
+    case 1: return K<true, true, false>::fn;
+    case 2: return K<true, false, false>::fn;
+    default: return nullptr;
+  }
+}
+
+// Launches a fused kernel with smem bytes of dynamic shared memory on min(ctas, SMs x resident
+// CTAs per SM) persistent CTAs.  XRD_E_SHAPE: no instantiation, or no CTA fits on an SM.
+template <typename... A>
+static int launch_fused(void (*kernel)(A...), int ctas, int threads, size_t smem,
+                        cudaStream_t stream, A... args) {
+  if (!kernel) return XRD_E_SHAPE;
+  XRD_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int occ = 0;
+  XRD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem));
+  if (occ < 1) return XRD_E_SHAPE;
+  const int max_ctas = num_sms() * occ;
+  {
+    KernelTimer kt(stream);
+    kernel<<<ctas < max_ctas ? ctas : max_ctas, threads, smem, stream>>>(args...);
+  }
+  XRD_LAUNCH_CHECK();
+  return XRD_OK;
 }
 
 extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
@@ -2102,7 +1948,6 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   } else {
     P.d_table = P.d_w_sdf0 = P.d_w_sdf1 = P.d_w_col0 = P.d_w_col1 = P.d_rays_o = P.d_rays_d = nullptr;
   }
-  P.jac = nullptr;
   const int sms = num_sms();
   // Kernel choice (rays_per_tile: 0 = automatic, -1 = tile kernel, -2 = grouped kernel, > 0 = tile
   // kernel with that many rays per tile).  Automatic: the grouped kernel runs the gradient pass
@@ -2120,88 +1965,39 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
     // grouped persistent kernel (k_fused_g): units of NR rays pulled from a queue
     P.NR = GP / S;
     P.n_tiles = (R + P.NR - 1) / P.NR;
-    P.jac = (grads && (grads->d_rays_o || grads->d_rays_d) && jac_bytes(R, S))
-                ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256 +
-                                           align_up((size_t)R * S * sizeof(float), 256))
-                : nullptr;
     int* queue = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 128);  // zeroed above
     // weights + NGROUPS x GP records + one z value per slot: 180 352 B.  Four groups would fit
     // (231 424 B) but need <= 80 registers per thread and spill more; with three, the ~48 KB
     // of shared memory left over serve as L1 for the gathers (1.25x the step rate on H100).
     const size_t smem_g = sizeof(float) * ((size_t)SW_TOTAL + (size_t)NGROUPS * GP * (GREC + 1));
+    const auto kernel = fused_kernel<GroupedKernel>(grads != nullptr, cfg->precision);
+    if (!kernel) return XRD_E_SHAPE;
     int dev = 0, smem_optin = 0;
+    cudaFuncAttributes fa;
     XRD_CUDA_TRY(cudaGetDevice(&dev));
     XRD_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int gridx = (P.n_tiles + NGROUPS - 1) / NGROUPS;
-    if (gridx > sms) gridx = sms;
-#define XRD_LAUNCH_G(KERNEL)                                                                      \
-  do {                                                                                            \
-    cudaFuncAttributes fa;                                                                        \
-    XRD_CUDA_TRY(cudaFuncGetAttributes(&fa, KERNEL));                                             \
-    if (smem_g + fa.sharedSizeBytes > (size_t)smem_optin) return XRD_E_SHAPE;                     \
-    XRD_CUDA_TRY(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                      (int)smem_g));                                              \
-    KernelTimer kt(stream);                                                                       \
-    KERNEL<<<gridx, GT * NGROUPS, smem_g, stream>>>(P, queue);                                    \
-  } while (0)
-    if (grads) {
-      switch (cfg->precision) {
-        case 0: XRD_LAUNCH_G((k_fused_g<true, true, true>)); break;
-        case 1: XRD_LAUNCH_G((k_fused_g<true, true, false>)); break;
-        case 2: XRD_LAUNCH_G((k_fused_g<true, false, false>)); break;
-        default: return XRD_E_SHAPE;
-      }
-      XRD_LAUNCH_CHECK();
-      FinalizeParams fp{loss_acc, P.counts, out->losses, P.Rg, S, cfg->w_rgb, cfg->w_depth, cfg->w_sdf, cfg->w_fs};
-      k_finalize<<<1, 32, 0, stream>>>(fp);
-      XRD_LAUNCH_CHECK();
-    } else {
-      if (cfg->precision <= 1) XRD_LAUNCH_G((k_fused_g<false, true, false>));
-      else XRD_LAUNCH_G((k_fused_g<false, false, false>));
-      XRD_LAUNCH_CHECK();
-    }
-#undef XRD_LAUNCH_G
-    return XRD_OK;
-  }
-  // tile kernel (k_fused): rays_per_tile > 0 selects its tile size, < 0 its default
-  int NR = pick_rays_per_tile(S, cfg->rays_per_tile);
-  if (NR < 1 || NR * S > 256) return XRD_E_SHAPE;
-  int threads = (NR * S + 31) / 32 * 32;
-  if (grads && threads < 224) threads = 224;  // 7+ warps own the 42 weight-gradient tiles (6 each)
-  P.NR = NR;
-  P.n_tiles = (R + NR - 1) / NR;
-  const size_t smem = sizeof(float) * ((size_t)SW_TOTAL + (size_t)(threads + 8) * REC + 6 * (size_t)NR * S);
-  const int nwarps = threads / 32;
-  const int slots = (DW_TILES + nwarps - 1) / nwarps;
-#define XRD_LAUNCH_FUSED(KERNEL)                                                                  \
-  do {                                                                                            \
-    XRD_CUDA_TRY(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
-                                      (int)smem));                                                \
-    int occ = 1;                                                                                  \
-    XRD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, KERNEL, threads, smem));     \
-    if (occ < 1) return XRD_E_SHAPE;                                                              \
-    int gridx = P.n_tiles < sms * occ ? P.n_tiles : sms * occ;                                    \
-    KernelTimer kt(stream);                                                                       \
-    KERNEL<<<gridx, threads, smem, stream>>>(P);                                                  \
-  } while (0)
-  if (grads) {
-    if (slots != 6) return XRD_E_SHAPE;  // >= 7 warps own the 42 weight-gradient tiles
-    switch (cfg->precision) {
-      case 0: XRD_LAUNCH_FUSED((k_fused<true, true, true, 6>)); break;
-      case 1: XRD_LAUNCH_FUSED((k_fused<true, true, false, 6>)); break;
-      case 2: XRD_LAUNCH_FUSED((k_fused<true, false, false, 6>)); break;
-      default: return XRD_E_SHAPE;
-    }
-    XRD_LAUNCH_CHECK();
-    FinalizeParams fp{loss_acc, P.counts, out->losses, P.Rg, S, cfg->w_rgb, cfg->w_depth, cfg->w_sdf, cfg->w_fs};
-    k_finalize<<<1, 32, 0, stream>>>(fp);
-    XRD_LAUNCH_CHECK();
+    XRD_CUDA_TRY(cudaFuncGetAttributes(&fa, kernel));
+    if (smem_g + fa.sharedSizeBytes > (size_t)smem_optin) return XRD_E_SHAPE;
+    st = launch_fused(kernel, (P.n_tiles + NGROUPS - 1) / NGROUPS, GT * NGROUPS, smem_g, stream, P,
+                      queue);
   } else {
-    if (cfg->precision <= 1) XRD_LAUNCH_FUSED((k_fused<false, true, false, 1>));
-    else XRD_LAUNCH_FUSED((k_fused<false, false, false, 1>));
-    XRD_LAUNCH_CHECK();
+    // tile kernel (k_fused): rays_per_tile > 0 selects its tile size, < 0 its default
+    const int NR = pick_rays_per_tile(S, cfg->rays_per_tile);
+    if (NR < 1 || NR * S > 256) return XRD_E_SHAPE;
+    int threads = (NR * S + 31) / 32 * 32;
+    if (grads && threads < 224) threads = 224;  // 7+ warps own the 42 weight-gradient tiles (6 each)
+    if (grads && (DW_TILES + threads / 32 - 1) / (threads / 32) != 6) return XRD_E_SHAPE;
+    P.NR = NR;
+    P.n_tiles = (R + NR - 1) / NR;
+    // weights + (threads + 8) records + per point z and xn
+    const size_t smem = sizeof(float) * ((size_t)SW_TOTAL + (size_t)(threads + 8) * REC + 6 * (size_t)NR * S);
+    st = launch_fused(fused_kernel<TileKernel>(grads != nullptr, cfg->precision), P.n_tiles, threads,
+                      smem, stream, P);
   }
-#undef XRD_LAUNCH_FUSED
+  if (st != XRD_OK || !grads) return st;
+  FinalizeParams fp{loss_acc, P.counts, out->losses, P.Rg, S, cfg->w_rgb, cfg->w_depth, cfg->w_sdf, cfg->w_fs};
+  k_finalize<<<1, 32, 0, stream>>>(fp);
+  XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
 
