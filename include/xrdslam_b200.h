@@ -234,7 +234,9 @@ typedef struct {
  * d_table and d_w_* are ACCUMULATED into (caller zeroes them: mapping-pose Adam
  * uses accum_step, Q11); d_rays_* are overwritten.  The five map gradients are
  * all-or-nothing: all NULL selects the pose-only pass used by tracking (no
- * scatter, no weight-gradient tiles). */
+ * scatter, no weight-gradient tiles).  d_table must be 16-byte aligned: two
+ * x-adjacent trilinear corners that share a 16-byte chunk are added with one
+ * vector reduction (XRD_E_SHAPE otherwise). */
 typedef struct {
   float* d_table;  /* [n_entries*2] */
   float* d_w_sdf0; /* [32,80] */
@@ -262,7 +264,7 @@ size_t xrd_coslam_smoothness_workspace_bytes(int sample_points);
 /* Smoothness / TV regulariser on the hash features (joint_encoding.py:165-197).
  * smooth_rand: HOST [6] = torch.rand(3) ++ torch.rand((1,1,1,3)).  Writes
  * weight*loss to DEVICE loss[0]; if d_table != NULL accumulates
- * grad_scale*weight*dloss/dtable into it. */
+ * grad_scale*weight*dloss/dtable into it (16-byte aligned, as in XrdCoslamGrads). */
 /* (xrd_coslam_smoothness_dev: the same with smooth_rand in DEVICE memory, read by the
  * kernels -- for CUDA-graph replay.) */
 int xrd_coslam_smoothness(const XrdHashGrid* grid, int sample_points,

@@ -23,7 +23,8 @@
 //              gradients in place; weight gradients are 16x8 MMA tiles with the
 //              points on the K axis, accumulated in registers for the whole launch;
 //              the hash backward runs in the MMA fragment layout (lane (g,t) owns
-//              level 4*nt+t of rows g, g+8) and scatters with red.global.add.v2.f32.
+//              level 4*nt+t of rows g, g+8) and scatters corner pairs: one red.global.add.v4.f32
+//              for two x-adjacent corners in one 16-byte chunk of d_table, red.v2 otherwise.
 //   k_fused_g  the same arithmetic through the same device functions, scheduled as
 //              independent groups of warps with named barriers, one m-tile per warp, a
 //              132-float record with OneBlob in compact form and a balanced
@@ -215,6 +216,57 @@ __device__ __forceinline__ uint32_t grid_index(const Lv& L, uint32_t x, uint32_t
   return index + L.offset;
 }
 
+// The 8 trilinear corners of cell c on level L: corner k is (c + (k & 1), c + (k >> 1 & 1),
+// c + (k >> 2)).
+__device__ __forceinline__ void corner_indices(const Lv& L, const uint32_t c[3], uint32_t idx[8]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+    idx[k] = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
+}
+
+// Corner pairs.  Corners k and k + 1 (k even) differ only in x.  On a hashed level x + 1 = x ^ 1
+// for even x, so the two are entries 2j and 2j + 1; on a dense level they are idx and idx + 1.
+// Level offsets are even (level sizes are multiples of 8 entries), so in both cases, and for the
+// wrap of out-of-box points on dense levels, the rule is: the pair is one 16-byte chunk of the
+// table iff i1 == (i0 ^ 1).  That holds for about half of all pairs.
+// d_table[i0] += g0, d_table[i1] += g1: one red.global.add.v4 for a pair in one chunk, two
+// red.global.add.v2 otherwise, as mutually exclusive predicated instructions (no divergent branch
+// per pair).  `d_table` must be 16-byte aligned (the launchers check it).  The gathers stay 8-byte
+// loads: paired 16-byte loads measured no faster in the forward and slower in the hash backward
+// (DESIGN.md section 4.1).
+__device__ __forceinline__ void scatter_corner_pair(float* __restrict__ d_table, uint32_t i0,
+                                                    uint32_t i1, float2 g0, float2 g1) {
+  const bool swap = i0 & 1u;  // in a chunk, i0 is the upper half when it is odd
+  const float2 lo = swap ? g1 : g0, hi = swap ? g0 : g1;
+  asm volatile(
+      "{\n\t.reg .pred pp;\n\t.reg .b32 t, e;\n\t.reg .u64 a0, a1;\n\t"
+      "xor.b32 t, %0, 1;\n\t"
+      "setp.eq.u32 pp, t, %1;\n\t"
+      "and.b32 e, %0, -2;\n\t"
+      "selp.b32 e, e, %0, pp;\n\t"
+      "mad.wide.u32 a0, e, 8, %2;\n\t"
+      "mad.wide.u32 a1, %1, 8, %2;\n\t"
+      "@pp red.global.add.v4.f32 [a0], {%3, %4, %5, %6};\n\t"
+      "@!pp red.global.add.v2.f32 [a0], {%7, %8};\n\t"
+      "@!pp red.global.add.v2.f32 [a1], {%9, %10};\n\t}"
+      ::"r"(i0), "r"(i1), "l"(d_table), "f"(lo.x), "f"(lo.y), "f"(hi.x), "f"(hi.y), "f"(g0.x),
+      "f"(g0.y), "f"(g1.x), "f"(g1.y)
+      : "memory");
+}
+
+// d_table[idx[k]] += wk (g0, g1) over the 8 corners, wk the trilinear weight of corner k for the
+// cell fractions w (rounded as in level_feature).
+__device__ __forceinline__ void scatter_corners(float* __restrict__ d_table, const uint32_t idx[8],
+                                                const float w[3], float g0, float g1) {
+#pragma unroll
+  for (int k = 0; k < 8; k += 2) {
+    const float wy = (k & 2) ? w[1] : 1.f - w[1], wz = (k & 4) ? w[2] : 1.f - w[2];
+    const float wa = (1.f - w[0]) * wy * wz, wb = w[0] * wy * wz;  // corners k, k + 1
+    scatter_corner_pair(d_table, idx[k], idx[k + 1], make_float2(wa * g0, wa * g1),
+                        make_float2(wb * g0, wb * g1));
+  }
+}
+
 __device__ __forceinline__ void pos_fract(float x, float scale, float& w, uint32_t& c) {
   float pos = fmaf(scale, x, 0.5f);
   float fl = floorf(pos);
@@ -319,13 +371,14 @@ __device__ __forceinline__ void blob_backward(const float xn[3], F dblob, float 
 }
 
 // the two features of level L at xn, trilinear over the 8 corners (all 8 loads issued first)
-__device__ __forceinline__ float2 level_feature(const float2* __restrict__ tab, const Lv& L,
+__device__ __forceinline__ float2 level_feature(const float* __restrict__ table, const Lv& L,
                                                 const float xn[3]) {
   float w[3];
   uint32_t c[3];
   pos_fract(xn[0], L.scale, w[0], c[0]);
   pos_fract(xn[1], L.scale, w[1], c[1]);
   pos_fract(xn[2], L.scale, w[2], c[2]);
+  const float2* __restrict__ tab = reinterpret_cast<const float2*>(table);
   float2 v[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k)
@@ -348,12 +401,11 @@ template <int LSTRIDE>
 __device__ __forceinline__ void encode(const float* __restrict__ table, int n_levels,
                                        const Lv* __restrict__ lv, const float xn[3],
                                        float* __restrict__ rec, int l0) {
-  const float2* __restrict__ tab = reinterpret_cast<const float2*>(table);
 #pragma unroll(4 / LSTRIDE)
   for (int i = 0; i < kL / LSTRIDE; ++i) {
     const int l = l0 + LSTRIDE * i;
     *reinterpret_cast<float2*>(rec + G_FEAT + 2 * l) =
-        (l < n_levels) ? level_feature(tab, lv[l], xn) : make_float2(0.f, 0.f);
+        (l < n_levels) ? level_feature(table, lv[l], xn) : make_float2(0.f, 0.f);
   }
 }
 
@@ -391,9 +443,7 @@ __device__ __noinline__ float3 hash_backward_multi(const float* __restrict__ tab
     uint32_t c[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) pos_fract(x[d], sc[h], w[h][d], c[d]);
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-      idx[h][k] = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
+    corner_indices(L, c, idx[h]);
   }
   float dx[3] = {0.f, 0.f, 0.f};
   if (need_dx) {
@@ -425,13 +475,7 @@ __device__ __noinline__ float3 hash_backward_multi(const float* __restrict__ tab
   if (scatter) {
 #pragma unroll
     for (int h = 0; h < NL; ++h) {
-      if (!on[h]) continue;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float wk = ((k & 1) ? w[h][0] : 1.f - w[h][0]) * ((k & 2) ? w[h][1] : 1.f - w[h][1]) *
-                         ((k & 4) ? w[h][2] : 1.f - w[h][2]);
-        red_add_v2(d_table + 2 * (size_t)idx[h][k], wk * g[h][0], wk * g[h][1]);
-      }
+      if (on[h]) scatter_corners(d_table, idx[h], w[h], g[h][0], g[h][1]);
     }
   }
   return make_float3(dx[0], dx[1], dx[2]);
@@ -1448,7 +1492,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     // ---- hash backward, point-parallel and BALANCED: thread (pp, half) owns levels half, half+2, ..
     // of point pp = every 6th point of the unit per warp (a ray's samples behind the surface carry
     // no gradient: ray-major assignment would leave whole warps idle).  d loss / d xn comes from
-    // a second gather of the corners; the table gradient is scattered with red.global.add.v2.
+    // a second gather of the corners; the table gradient is scattered in corner pairs.
     {
       const int qd = gt >> 1;
       const int pp = (qd & 15) * GW + (qd >> 4);
@@ -1612,22 +1656,7 @@ __global__ void __launch_bounds__(256) k_smooth_fwd(SmoothParams p) {
   const int iz = pt % n, iy = (pt / n) % n, ix = pt / (n * n);
   float xn[3];
   smooth_xn(p, ix, iy, iz, xn);
-  const float2* tab = reinterpret_cast<const float2*>(p.table);
-  float w[3];
-  uint32_t c[3];
-  const Lv L = s_lv[l];
-  for (int d = 0; d < 3; ++d) pos_fract(xn[d], L.scale, w[d], c[d]);
-  float f0 = 0.f, f1 = 0.f;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    uint32_t idx = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
-    float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
-               ((k & 4) ? w[2] : 1.f - w[2]);
-    float2 v = __ldg(&tab[idx]);
-    f0 = fmaf(wk, v.x, f0);
-    f1 = fmaf(wk, v.y, f1);
-  }
-  reinterpret_cast<float2*>(p.feat)[(size_t)pt * kL + l] = make_float2(f0, f1);
+  reinterpret_cast<float2*>(p.feat)[(size_t)pt * kL + l] = level_feature(p.table, s_lv[l], xn);
 }
 
 __global__ void __launch_bounds__(256) k_smooth_bwd(SmoothParams p) {
@@ -1666,13 +1695,9 @@ __global__ void __launch_bounds__(256) k_smooth_bwd(SmoothParams p) {
       uint32_t c[3];
       const Lv L = s_lv[l];
       for (int d = 0; d < 3; ++d) pos_fract(xn[d], L.scale, w[d], c[d]);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        uint32_t idx = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
-        float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
-                   ((k & 4) ? w[2] : 1.f - w[2]);
-        red_add_v2(p.d_table + 2 * (size_t)idx, wk * g0, wk * g1);
-      }
+      uint32_t idx[8];
+      corner_indices(L, c, idx);
+      scatter_corners(p.d_table, idx, w, g0, g1);
     }
   }
   // one double atomic per CTA (per warp it was ~15 k serialised atomics on one address)
@@ -1701,24 +1726,19 @@ __global__ void __launch_bounds__(256) k_encode(GridDev g, const float* table, c
   const int pt = q / kL, l = q % kL;
   if (pt >= n || l >= g.n_levels) return;
   const Lv L = s_lv[l];
-  const float2* tab = reinterpret_cast<const float2*>(table);
-  float w[3];
-  uint32_t c[3];
-  for (int d = 0; d < 3; ++d) pos_fract(x[pt * 3 + d], L.scale, w[d], c[d]);
-  float f0 = 0.f, f1 = 0.f;
+  const float xn[3] = {x[pt * 3], x[pt * 3 + 1], x[pt * 3 + 2]};
+  if (idx_out) {
+    float w[3];
+    uint32_t c[3], idx[8];
+    for (int d = 0; d < 3; ++d) pos_fract(xn[d], L.scale, w[d], c[d]);
+    corner_indices(L, c, idx);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    uint32_t idx = grid_index(L, c[0] + (k & 1), c[1] + ((k >> 1) & 1), c[2] + ((k >> 2) & 1));
-    if (idx_out) idx_out[((size_t)pt * g.n_levels + l) * 8 + k] = idx;
-    float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
-               ((k & 4) ? w[2] : 1.f - w[2]);
-    float2 v = __ldg(&tab[idx]);
-    f0 = fmaf(wk, v.x, f0);
-    f1 = fmaf(wk, v.y, f1);
+    for (int k = 0; k < 8; ++k) idx_out[((size_t)pt * g.n_levels + l) * 8 + k] = idx[k];
   }
   if (feat) {
-    feat[(size_t)pt * 2 * g.n_levels + 2 * l] = f0;
-    feat[(size_t)pt * 2 * g.n_levels + 2 * l + 1] = f1;
+    const float2 f = level_feature(table, L, xn);
+    feat[(size_t)pt * 2 * g.n_levels + 2 * l] = f.x;
+    feat[(size_t)pt * 2 * g.n_levels + 2 * l + 1] = f.y;
   }
 }
 
@@ -1814,6 +1834,9 @@ static int fill_grid(GridDev& g, const XrdHashGrid* h) {
   return XRD_OK;
 }
 
+// the corner-pair scatter adds to the table gradient in 16-byte chunks
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
 }  // namespace coslam
 }  // namespace xrd
 
@@ -1897,6 +1920,7 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
                       (grads->d_w_col1 != nullptr);
     if (n_map != 0 && n_map != 5) return XRD_E_NULL;
     if (n_map == 0 && !grads->d_rays_o && !grads->d_rays_d) return XRD_E_NULL;
+    if (grads->d_table && !aligned16(grads->d_table)) return XRD_E_SHAPE;
   }
   if (workspace_bytes < xrd_coslam_workspace_bytes(R, S)) return XRD_E_WORKSPACE;
 
@@ -1953,7 +1977,7 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   // kernel with that many rays per tile).  Automatic: the grouped kernel runs the gradient pass
   // once every group has >= 1 unit in flight after the first wave; the tile kernel runs small
   // batches (tracking) and forward-only rendering.  On H100 (400 W) the grouped kernel takes
-  // 0.514 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
+  // 0.477 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
   // random rays (mode 1) the two are close: tile / grouped fwd+bwd R = 1024: 214 / 195 us,
   // 4096: 462 / 468, 16384: 1470 / 1520, 65536: 5463 / 5818 us; the rule is unchanged.
   bool grouped = false;
@@ -2012,6 +2036,7 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
                            void* workspace, size_t workspace_bytes, void* stream_) {
   if (!grid || !grid->table || !smooth_rand || !loss || !workspace) return XRD_E_NULL;
   if (sample_points < 3) return XRD_E_SHAPE;
+  if (d_table && !aligned16(d_table)) return XRD_E_SHAPE;
   if (workspace_bytes < xrd_coslam_smoothness_workspace_bytes(sample_points)) return XRD_E_WORKSPACE;
   cudaStream_t stream = (cudaStream_t)stream_;
   SmoothParams p;
