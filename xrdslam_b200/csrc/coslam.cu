@@ -763,9 +763,19 @@ __device__ __forceinline__ LossNorm loss_norm(const int* __restrict__ counts) {
   return ln;
 }
 
-// This warp's share of one weight-gradient layer: tiles [lo, hi) of the 42, slot j holds tile
-// w + j * nw.  m-tile mt of the layer input covers its columns 16 mt .. 16 mt + 15 at record
-// offset aoff; m-tiles [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form.
+// Tile id of a weight-gradient layer whose tiles are [lo, hi) of the 42.  m-tile mt of the layer
+// input covers its columns 16 mt .. 16 mt + 15 at record offset aoff; m-tiles
+// [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form.
+template <bool PREC3, bool COMPACT>
+__device__ __forceinline__ void dw_layer_tile(const float* __restrict__ recs, int npts, int id,
+                                              int lo, int aoff, int boff, int n_tiles_n,
+                                              int blob_mt, float (&acc)[4]) {
+  const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
+  const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
+  dw_tile<PREC3, Rec<COMPACT>::N, COMPACT>(recs, npts, aoff + 16 * mt, boff + 8 * nt, acc, bd);
+}
+
+// This warp's share of one weight-gradient layer: slot j holds tile w + j * nw.
 template <bool PREC3, bool COMPACT, int SLOTS>
 __device__ __forceinline__ void dw_layer(const float* __restrict__ recs, int npts, int w, int nw,
                                          float (&acc)[SLOTS][4], int lo, int hi, int aoff,
@@ -773,11 +783,8 @@ __device__ __forceinline__ void dw_layer(const float* __restrict__ recs, int npt
 #pragma unroll
   for (int j = 0; j < SLOTS; ++j) {
     const int id = w + j * nw;
-    if (id >= lo && id < hi) {
-      const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
-      const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
-      dw_tile<PREC3, Rec<COMPACT>::N, COMPACT>(recs, npts, aoff + 16 * mt, boff + 8 * nt, acc[j], bd);
-    }
+    if (id >= lo && id < hi)
+      dw_layer_tile<PREC3, COMPACT>(recs, npts, id, lo, aoff, boff, n_tiles_n, blob_mt, acc[j]);
   }
 }
 
@@ -1195,6 +1202,43 @@ constexpr int GP = 96;       // record slots per group
 constexpr int NGROUPS = 3;
 constexpr int G_SLOTS = 7;   // 42 weight-gradient tiles / 6 warps
 constexpr int G_KPL = (GP + 31) / 32;  // samples per lane in the per-ray composite (S <= GP)
+// Weight-gradient accumulators: warp gw's slot 0 (tile gw) stays in registers for the whole
+// launch; tiles GW..41 are summed per CTA in shared memory, [tile - GW][4][32 lanes] (C-fragment
+// order: conflict-free).  All 28 values per thread held in registers across the loop do not fit
+// in 96 registers, and their spills to local memory compete with the gathers for L1.
+constexpr int G_DWBUF = (DW_TILES - GW) * 4 * 32;  // floats
+// dynamic shared memory: weights, NGROUPS x GP records + one z value per slot, and (gradient
+// passes with map gradients) the weight-gradient buffer
+constexpr size_t G_SMEM = sizeof(float) * ((size_t)SW_TOTAL + (size_t)NGROUPS * GP * (GREC + 1));
+constexpr size_t G_SMEM_DW = G_SMEM + sizeof(float) * G_DWBUF;
+// Stay in the 196 KB shared-memory configuration of an sm_90 SM (200 704 B): the next one up
+// (228 KB) would cut the L1 the gathers rely on from ~60 KB to ~28 KB.  560 B: the kernel's
+// static shared memory (s_lv, s_unit, s_loss); 1 KB: the per-CTA reservation.
+static_assert(G_SMEM_DW + 560 + 1024 <= 196 * 1024, "k_fused_g outgrows the 196 KB carveout");
+
+// Warp gw's share of one weight-gradient layer of k_fused_g (tiles gw + j GW in [lo, hi)): slot 0
+// accumulates into dw0, every other tile into a zeroed fragment that is then added to dwbuf (the
+// NGROUPS groups add to the same tiles).
+template <bool PREC3>
+__device__ __forceinline__ void dw_layer_g(const float* __restrict__ recs, int npts, int gw,
+                                           float (&dw0)[4], float* __restrict__ dwbuf, int lo,
+                                           int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < G_SLOTS; ++j) {
+    const int id = gw + j * GW;
+    if (id < lo || id >= hi) continue;
+    if (j == 0) {
+      dw_layer_tile<PREC3, true>(recs, npts, id, lo, aoff, boff, n_tiles_n, blob_mt, dw0);
+    } else {
+      float c[4] = {0.f, 0.f, 0.f, 0.f};
+      dw_layer_tile<PREC3, true>(recs, npts, id, lo, aoff, boff, n_tiles_n, blob_mt, c);
+      float* q = dwbuf + (id - GW) * 4 * 32 + lane;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) atomicAdd(q + 32 * i, c[i]);
+    }
+  }
+}
 
 __device__ __forceinline__ void group_sync(int grp) {
   asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(GT) : "memory");
@@ -1209,7 +1253,10 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   const int gw = gt >> 5, lane = gt & 31;
   float* recs = sw + SW_TOTAL + grp * (GP * GREC);
   float* zbuf = sw + SW_TOTAL + NGROUPS * (GP * GREC) + grp * GP;  // GP z values
+  float* dwbuf = sw + G_SMEM / sizeof(float);  // G_DWBUF, only when map_grads
   const int S = P.S;
+  const bool need_dx = BWD && ((P.d_rays_o != nullptr) || (P.d_rays_d != nullptr));
+  const bool map_grads = BWD && (P.d_table != nullptr);
 
   __shared__ Lv s_lv[kL];
   __shared__ int s_unit[NGROUPS];
@@ -1217,20 +1264,16 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
   load_levels(s_lv, P.g);
   if (tid < 4) s_loss[tid] = 0.0;
   for (int q = gt; q < GP * GREC; q += GT) recs[q] = 0.f;
+  if (map_grads)
+    for (int q = tid; q < G_DWBUF; q += blockDim.x) dwbuf[q] = 0.f;
   stage_weights(sw, P);
   const LossNorm ln = BWD ? loss_norm(P.counts) : LossNorm{};
-  float dwacc[G_SLOTS][4];
-#pragma unroll
-  for (int j = 0; j < G_SLOTS; ++j)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) dwacc[j][i] = 0.f;
+  float dw0[4] = {0.f, 0.f, 0.f, 0.f};  // weight-gradient tile gw
   __syncthreads();
 
   const int p = gt >> 1, half = gt & 1;       // gather phases: two threads per point
   float* rec = recs + p * GREC;
   float* wrec = recs + (gw * 16) * GREC;      // MMA phases: this warp's 16 records
-  const bool need_dx = BWD && ((P.d_rays_o != nullptr) || (P.d_rays_d != nullptr));
-  const bool map_grads = BWD && (P.d_table != nullptr);
   int prev_npts = 0;
 
   for (;;) {
@@ -1427,7 +1470,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     // ---------------- phase 3: backward ----------------------------------
     auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
       if (map_grads)
-        dw_layer<BPREC3, true>(recs, npts, gw, GW, dwacc, lo, hi, aoff, boff, n_tiles_n, blob_mt);
+        dw_layer_g<BPREC3>(recs, npts, gw, dw0, dwbuf, lo, hi, aoff, boff, n_tiles_n, blob_mt);
     };
     // d w_col1 += c1^T draw   (8-wide n tile over raw[4] + 4 floats of the next record: columns
     dw_phase(0, 2, G_C1, G_RAW, 1, -1);  //  3..7 are never written out; the last record's
@@ -1565,34 +1608,24 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     __syncthreads();
     if (tid < 4 && s_loss[tid] != 0.0) atomicAdd(&P.loss_acc[tid], s_loss[tid]);
     if (map_grads) {
-      // sum the weight-gradient tiles of the NGROUPS groups in shared memory (the record area is
-      // dead now), then one red.global per element and CTA
-      float* red = sw + SW_TOTAL;  // [42 tiles][4][32 lanes]
-      for (int gsel = 0; gsel < NGROUPS; ++gsel) {
-        if (grp == gsel) {
+      // the groups' register tiles 0..GW-1 go through the (dead) record area, [grp][tile][4][32];
+      // then one warp per tile and one red.global per element and CTA
+      float* red = sw + SW_TOTAL;
 #pragma unroll
-          for (int j = 0; j < G_SLOTS; ++j) {
-            const int id = gw + j * GW;
-            if (id >= DW_TILES) continue;
+      for (int i = 0; i < 4; ++i) red[((grp * GW + gw) * 4 + i) * 32 + lane] = dw0[i];
+      __syncthreads();
+      for (int id = tid >> 5; id < DW_TILES; id += NGROUPS * GW) {
+        float v[4];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float* q0 = red + (id * 4 + i) * 32 + lane;
-              *q0 = (gsel == 0) ? dwacc[j][i] : (*q0 + dwacc[j][i]);
-            }
+        for (int i = 0; i < 4; ++i) {
+          if (id < GW) {
+            v[i] = red[(id * 4 + i) * 32 + lane];
+            for (int gs = 1; gs < NGROUPS; ++gs) v[i] += red[((gs * GW + id) * 4 + i) * 32 + lane];
+          } else {
+            v[i] = dwbuf[(id - GW) * 4 * 32 + 32 * i + lane];
           }
         }
-        __syncthreads();
-      }
-      if (grp == 0) {
-#pragma unroll
-        for (int j = 0; j < G_SLOTS; ++j) {
-          const int id = gw + j * GW;
-          if (id >= DW_TILES) continue;
-          float v[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) v[i] = red[(id * 4 + i) * 32 + lane];
-          dw_store(P, id, v);
-        }
+        dw_store(P, id, v);
       }
     }
   }
@@ -1977,7 +2010,7 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   // kernel with that many rays per tile).  Automatic: the grouped kernel runs the gradient pass
   // once every group has >= 1 unit in flight after the first wave; the tile kernel runs small
   // batches (tracking) and forward-only rendering.  On H100 (400 W) the grouped kernel takes
-  // 0.477 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
+  // 0.433 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
   // random rays (mode 1) the two are close: tile / grouped fwd+bwd R = 1024: 214 / 195 us,
   // 4096: 462 / 468, 16384: 1470 / 1520, 65536: 5463 / 5818 us; the rule is unchanged.
   bool grouped = false;
@@ -1990,10 +2023,11 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
     P.NR = GP / S;
     P.n_tiles = (R + P.NR - 1) / P.NR;
     int* queue = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 128);  // zeroed above
-    // weights + NGROUPS x GP records + one z value per slot: 180 352 B.  Four groups would fit
-    // (231 424 B) but need <= 80 registers per thread and spill more; with three, the ~48 KB
-    // of shared memory left over serve as L1 for the gathers (1.25x the step rate on H100).
-    const size_t smem_g = sizeof(float) * ((size_t)SW_TOTAL + (size_t)NGROUPS * GP * (GREC + 1));
+    // weights + NGROUPS x GP records + one z value per slot: 180 352 B, plus 18 432 B of
+    // weight-gradient buffer when map gradients are on.  Four groups would fit (231 424 B) but
+    // need <= 80 registers per thread and spill more; with three, what the 196 KB configuration
+    // leaves of the SM's 256 KB serves as L1 for the gathers (1.25x the step rate on H100).
+    const size_t smem_g = P.d_table ? G_SMEM_DW : G_SMEM;
     const auto kernel = fused_kernel<GroupedKernel>(grads != nullptr, cfg->precision);
     if (!kernel) return XRD_E_SHAPE;
     int dev = 0, smem_optin = 0;
