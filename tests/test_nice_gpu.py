@@ -11,21 +11,32 @@ from helpers import max_abs, rel_err
 BOUND = np.array([[-2.0, 2.0], [-2.0, 2.0], [-2.0, 2.0]])
 
 
-def nice_pair(device, seed=0, grid_amp=30.0):
+def nice_pair(device, seed=0, grid_amp=30.0, bound=BOUND, coarse=False, b_scale=0.2):
+    import warnings
     from oracle.nice import NiceOracle
     from xrdslam_b200.camera import Camera
     from xrdslam_b200.conv_onet import ConvOnetConfig
-    ora = NiceOracle(BOUND, seed=seed)
+    # nn.Linear and xavier_uniform_ draw from the global generator: seed it, locally
+    with torch.random.fork_rng():
+        torch.manual_seed(seed)
+        ora = NiceOracle(bound, seed=seed, coarse=coarse)
     g = torch.Generator().manual_seed(seed + 5)
     with torch.no_grad():
         for k in ora.grids:
             ora.grids[k].mul_(grid_amp)
         for dec in (ora.middle, ora.fine, ora.color):
-            dec.B.mul_(0.2)  # keep sin() arguments moderate for a tight comparison
+            dec.B.mul_(b_scale)  # 0.2: keeps sin() arguments moderate for a tight comparison
             for lin in list(dec.fc_c) + list(dec.pts) + [dec.out]:
                 lin.bias.copy_(torch.randn(lin.bias.shape, generator=g) * 0.1)
-    model = ConvOnetConfig(mapping_frustum_feature_selection=False).setup(
-        camera=Camera(320., 320., 319.5, 239.5, 640, 480), bounding_box=BOUND)
+        if coarse:
+            for lin in list(ora.coarse.pts) + [ora.coarse.out]:
+                lin.bias.copy_(torch.randn(lin.bias.shape, generator=g) * 0.1)
+    with warnings.catch_warnings():
+        # no pretrained checkpoints in the tests
+        warnings.filterwarnings('ignore', message='ConvOnet: no pretrained checkpoint',
+                                category=RuntimeWarning)
+        model = ConvOnetConfig(coarse=coarse, mapping_frustum_feature_selection=False).setup(
+            camera=Camera(320., 320., 319.5, 239.5, 640, 480), bounding_box=bound)
     with torch.no_grad():
         for name in ('middle', 'fine', 'color'):
             o = getattr(ora, name)
@@ -36,6 +47,13 @@ def nice_pair(device, seed=0, grid_amp=30.0):
                 m.pts_linears[i].weight.copy_(o.pts[i].weight)
                 m.pts_linears[i].bias.copy_(o.pts[i].bias)
             m.output_linear.weight.copy_(o.out.weight); m.output_linear.bias.copy_(o.out.bias)
+        if coarse:
+            m = model.decoder.coarse_decoder
+            for i in range(5):
+                m.pts_linears[i].weight.copy_(ora.coarse.pts[i].weight)
+                m.pts_linears[i].bias.copy_(ora.coarse.pts[i].bias)
+            m.output_linear.weight.copy_(ora.coarse.out.weight)
+            m.output_linear.bias.copy_(ora.coarse.out.bias)
         for k in ora.grids:
             model.set_grid(k, ora.grids[k])
     assert torch.equal(model.bounding_box, ora.bound)

@@ -188,8 +188,9 @@ __device__ __forceinline__ void src_index(float x, int size, int& i0, float& f, 
   float ix = ((x + 1.f) / 2.f) * (float)(size - 1);
   mult = (float)(size - 1) / 2.f;
   const float hi = (float)(size - 1);
-  if (ix <= 0.f) { mult = (ix < 0.f) ? 0.f : mult; ix = fmaxf(ix, 0.f); }
-  if (ix >= hi) { mult = (ix > hi) ? 0.f : mult; ix = fminf(ix, hi); }
+  // clip_coordinates_set_grad: the coordinate gradient is 0 on the faces too (ix == 0, hi)
+  if (ix <= 0.f) { mult = 0.f; ix = fmaxf(ix, 0.f); }
+  if (ix >= hi) { mult = 0.f; ix = fminf(ix, hi); }
   const float fl = floorf(ix);
   i0 = (int)fl;
   f = ix - fl;
