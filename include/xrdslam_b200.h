@@ -547,6 +547,68 @@ int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map, const XrdVox
                          const XrdVoxRenderCfg* cfg, XrdVoxOut* out, XrdVoxGrads* grads,
                          void* workspace, size_t workspace_bytes, void* stream);
 
+/* Forward-only Decoder.get_values at points that carry a voxel (octree node) id, for mesh
+ * extraction.  Replaces slam/model_components/voxel_helpers_voxfusion.py:15-94 (get_scores,
+ * eval_points) and their get_features / trilinear_interp (:97-166); same arithmetic as the
+ * render path (one shared corner / weight routine, the same decoder GEMM chain).
+ *   res > 0, LATTICE mode (get_scores): n = number of voxels, vox DEVICE [n] node ids,
+ *       lin DEVICE [res] = torch.linspace(-0.5, 0.5, res) in fp32; point (b, i, j, k) is
+ *       xyz = lin[(i, j, k)] * voxel_size + centre[vox[b]] (fp32, rounded per operation).
+ *       Only the sdf head runs; sdf DEVICE [n][res][res][res] (meshgrid 'ij': i slowest) --
+ *       the marching-cubes volume layout.  xyz and rgb must be NULL.
+ *   res == 0, POINT mode (eval_points): n points, xyz DEVICE [n][3], vox DEVICE [n] node ids;
+ *       rgb DEVICE [n][3] (sigmoid colour), sdf DEVICE [n] or NULL.
+ * The workspace is sized for n_points = n * res^3 (lattice) or n (points). */
+size_t xrd_voxfusion_query_workspace_bytes(int n_points);
+int xrd_voxfusion_query(const XrdVoxMap* map, const XrdVoxDecoder* dec, float voxel_size, int n,
+                        const int32_t* vox, int res, const float* lin, const float* xyz,
+                        float* sdf, float* rgb, void* workspace, size_t workspace_bytes,
+                        void* stream);
+
+/* ---- Marching cubes ---------------------------------------------------------
+ *
+ *   xrd_mesh_mc_*  slam/common/mesher.py:206-238 (skimage.measure.marching_cubes over the
+ *                  Mesher's lattice, on the host after a D2H copy of every value) and
+ *                  slam/algorithms/voxfusion.py:250-278 (one skimage call per surface voxel in
+ *                  a Python loop).  One implementation for a batch of B independent volumes
+ *                  values DEVICE fp32 [B][nx][ny][nz] (x slowest), nx, ny, nz >= 2.
+ *
+ * Semantics:
+ *   - a corner is negative iff v < level; a lattice edge is crossed iff its two corners are on
+ *     different sides;
+ *   - each crossed edge gets exactly one vertex per volume, shared by every cube using it
+ *     (vertices are not shared across volumes);
+ *   - position along the edge v0 -> v1 (v0 at the lower lattice index): t = (level - v0) /
+ *     (v1 - v0); p = lattice index with t added on the edge's axis; world coordinate
+ *     ((p * spacing + shift) * scale) + origin[b], every operation fp32 round-to-nearest;
+ *   - vertex order (volume, flat lattice index of the edge's lower endpoint, axis x, y, z),
+ *     face order (volume, cube = flat index of its lower lattice point, triangle in the case);
+ *   - winding: the right-hand normal of every face points toward larger values (outward for
+ *     an SDF that is negative inside).  The case table (csrc/mc_table.cuh) is generated by
+ *     oracle/mc_table.py; ambiguous faces separate their two negative corners.
+ * Differences from skimage's Lewiner method are expected on ambiguous cubes only (asymptotic
+ * decider, extra interior vertex); the reference's two callers map to the affine as
+ *   Mesher:     spacing (x[2]-x[1], ...), shift (x[0], y[0], z[0]), scale 1, origin NULL;
+ *   Vox-Fusion: spacing 1/(res-1), shift -0.5, scale voxel_size, origin = voxel centres.
+ *
+ * Two phases: xrd_mesh_mc_count classifies the cubes, scans the per-point vertex and triangle
+ * counts into the workspace and writes the totals (V, F) to DEVICE counts[2]; the caller reads
+ * them, allocates verts f32 [V][3] and faces i32 [F][3], and calls xrd_mesh_mc_emit with the
+ * same values, shape, level and workspace.  Nothing is allocated inside. */
+typedef struct {
+  float spacing[3];
+  float shift[3];
+  float scale[3];
+  const float* origin;  /* DEVICE [B][3] or NULL (zero)                                   */
+} XrdMeshAffine;
+
+size_t xrd_mesh_mc_workspace_bytes(int B, int nx, int ny, int nz);
+int xrd_mesh_mc_count(const float* values, int B, int nx, int ny, int nz, float level,
+                      int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+int xrd_mesh_mc_emit(const float* values, int B, int nx, int ny, int nz, float level,
+                     const XrdMeshAffine* affine, float* verts, int32_t* faces, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -165,6 +165,11 @@ class XrdVoxGrads(C.Structure):
                 ('d_rays_o', vp), ('d_rays_d', vp)]
 
 
+class XrdMeshAffine(C.Structure):
+    _fields_ = [('spacing', C.c_float * 3), ('shift', C.c_float * 3), ('scale', C.c_float * 3),
+                ('origin', vp)]
+
+
 class XrdPointIndex(C.Structure):
     _fields_ = [('pos', vp), ('n_points', C.c_int), ('cell', C.c_float),
                 ('table_size', C.c_int), ('cell_start', vp), ('cell_end', vp),
@@ -274,6 +279,14 @@ SYMBOLS = {
         C.POINTER(XrdRays), C.POINTER(XrdVoxMap), C.POINTER(XrdVoxMarch),
         C.POINTER(XrdVoxMarchCfg), C.POINTER(XrdVoxDecoder), C.POINTER(XrdVoxRenderCfg),
         C.POINTER(XrdVoxOut), C.POINTER(XrdVoxGrads), vp, C.c_size_t, vp]),
+    'xrd_voxfusion_query_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'xrd_voxfusion_query': (C.c_int, [C.POINTER(XrdVoxMap), C.POINTER(XrdVoxDecoder), C.c_float,
+                                      C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    'xrd_mesh_mc_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'xrd_mesh_mc_count': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, vp,
+                                    C.c_size_t, vp]),
+    'xrd_mesh_mc_emit': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                   C.POINTER(XrdMeshAffine), vp, vp, vp, C.c_size_t, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

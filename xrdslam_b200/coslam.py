@@ -14,6 +14,7 @@ import torch
 from .algorithm import Algorithm, AlgorithmConfig
 from .common import get_camera_rays, get_rays, get_samples, rays_from_poses
 from .joint_encoding import JointEncodingConfig
+from .mesher import MesherConfig
 from .opt_pose import pose_matrices
 from .optimizers import AdamOptimizerConfig, Optimizers
 
@@ -60,6 +61,8 @@ class CoSLAMConfig(AlgorithmConfig):
     mapping_bound: List[List[float]] = field(
         default_factory=lambda: [[-3, 3], [-4, 2.5], [-2, 2.5]])
     optimizers: Dict[str, Any] = field(default_factory=_coslam_optimizers)
+    mesher: MesherConfig = field(default_factory=lambda: MesherConfig(
+        resolution=256, points_batch_size=30000))
     # run the mapping iterations as one CUDA graph each (coslam_graph.py)
     graph_mapping: bool = True
 
@@ -106,6 +109,9 @@ class CoSLAM(Algorithm):
                                              bounding_box=self.bounding_box)
         self.model.to(device)
         self.bundle_adjust = True
+        self.mesher = self.config.mesher.setup(camera=camera, bounding_box=self.bounding_box,
+                                               marching_cubes_bound=self.marching_cube_bound)
+        self.cur_mesh = None
         self.num_rays_to_save = int(self.camera.width * self.camera.height *
                                     self.config.rays_to_save_ratio)
         self.rays = None  # [n_kf * num_rays_to_save, 7] pinned host memory
@@ -336,3 +342,12 @@ class CoSLAM(Algorithm):
             color = torch.cat(colors, 0).reshape(self.camera.height,
                                                  self.camera.width, 3)
             return color.cpu().numpy(), depth.cpu().numpy()
+
+    # coslam.py:291-298
+    def get_mesh(self):
+        with self.lock:
+            self.cur_mesh = self.mesher.get_mesh(keyframe_graph=self.keyframe_graph,
+                                                 query_fn=self.model.query_fn,
+                                                 color_func=self.model.color_func,
+                                                 device=self.device)
+            return self.cur_mesh

@@ -339,23 +339,50 @@ struct Corner {
   float w[8];
   float p[3];
 };
-__device__ __forceinline__ void corners(const PointParams& P, int r, int k, float xyz[3], Corner& c) {
-  const float depth = P.smp_depth[(size_t)r * P.scap + k];
-  const int vox = P.smp_idx[(size_t)r * P.scap + k];
+// corner embedding ids and trilinear weights of point xyz inside voxel (node) vox
+__device__ __forceinline__ void corners_at(const float* centres, const int* vertex_idx,
+                                           float voxel_size, const float xyz[3], int vox,
+                                           Corner& c) {
 #pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    xyz[d] = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], depth));
-    // p = (xyz - centre) / voxel_size + 0.5
-    c.p[d] = __fadd_rn(__fdiv_rn(__fsub_rn(xyz[d], P.centres[vox * 3 + d]), P.voxel_size), 0.5f);
-  }
+  for (int d = 0; d < 3; ++d)  // p = (xyz - centre) / voxel_size + 0.5
+    c.p[d] = __fadd_rn(__fdiv_rn(__fsub_rn(xyz[d], centres[vox * 3 + d]), voxel_size), 0.5f);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    c.vid[i] = P.vertex_idx[vox * 8 + i];
+    c.vid[i] = vertex_idx[vox * 8 + i];
     const int qx = i >> 2, qy = (i >> 1) & 1, qz = i & 1;  // offset_points: x slowest
     const float wx = qx ? c.p[0] : 1.f - c.p[0];
     const float wy = qy ? c.p[1] : 1.f - c.p[1];
     const float wz = qz ? c.p[2] : 1.f - c.p[2];
     c.w[i] = wx * wy * wz;
+  }
+}
+
+// sample k of ray r: xyz = o + d * depth in its sampled voxel
+__device__ __forceinline__ void corners(const PointParams& P, int r, int k, float xyz[3], Corner& c) {
+  const float depth = P.smp_depth[(size_t)r * P.scap + k];
+  const int vox = P.smp_idx[(size_t)r * P.scap + k];
+#pragma unroll
+  for (int d = 0; d < 3; ++d)
+    xyz[d] = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], depth));
+  corners_at(P.centres, P.vertex_idx, P.voxel_size, xyz, vox, c);
+}
+
+// x = sum_i w_i emb[vid_i]  (get_embeddings' weighted sum over the 8 corners)
+__device__ __forceinline__ void trilerp_emb(const float* __restrict__ emb, const Corner& c,
+                                            float x[EMB]) {
+#pragma unroll
+  for (int q = 0; q < EMB; ++q) x[q] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4* e = reinterpret_cast<const float4*>(emb + (size_t)c.vid[i] * EMB);
+#pragma unroll
+    for (int q4 = 0; q4 < 4; ++q4) {
+      const float4 v = __ldg(&e[q4]);
+      x[4 * q4 + 0] = fmaf(c.w[i], v.x, x[4 * q4 + 0]);
+      x[4 * q4 + 1] = fmaf(c.w[i], v.y, x[4 * q4 + 1]);
+      x[4 * q4 + 2] = fmaf(c.w[i], v.z, x[4 * q4 + 2]);
+      x[4 * q4 + 3] = fmaf(c.w[i], v.w, x[4 * q4 + 3]);
+    }
   }
 }
 
@@ -368,22 +395,51 @@ __global__ void __launch_bounds__(T) k_vox_gather(const PointParams P) {
   Corner c;
   corners(P, P.pt_ray[p], P.pt_k[p], xyz, c);
   float x[EMB];
-#pragma unroll
-  for (int q = 0; q < EMB; ++q) x[q] = 0.f;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4* e = reinterpret_cast<const float4*>(P.emb + (size_t)c.vid[i] * EMB);
-#pragma unroll
-    for (int q4 = 0; q4 < 4; ++q4) {
-      const float4 v = __ldg(&e[q4]);
-      x[4 * q4 + 0] = fmaf(c.w[i], v.x, x[4 * q4 + 0]);
-      x[4 * q4 + 1] = fmaf(c.w[i], v.y, x[4 * q4 + 1]);
-      x[4 * q4 + 2] = fmaf(c.w[i], v.z, x[4 * q4 + 2]);
-      x[4 * q4 + 3] = fmaf(c.w[i], v.w, x[4 * q4 + 3]);
-    }
-  }
+  trilerp_emb(P.emb, c, x);
 #pragma unroll
   for (int q = 0; q < EMB; ++q) P.acts[(size_t)(ra_x() + q) * P.Pp + p] = x[q];
+}
+
+// mesh-extraction queries: points from a per-voxel lattice (res > 0) or an explicit list
+struct QueryParams {
+  int P, Pp, res;
+  const int* vox; const float* lin; const float* xyz;
+  const float* centres; const int* vertex_idx; const float* emb;
+  float voxel_size;
+  float* acts;
+};
+
+__global__ void __launch_bounds__(T) k_vox_query_gather(const QueryParams Q) {
+  const int p = blockIdx.x * T + threadIdx.x;
+  if (p >= Q.P) return;
+  float xyz[3];
+  int vox;
+  if (Q.res > 0) {  // get_scores: xyz = linspace(-.5, .5, res)[ijk] * voxel_size + centre
+    const int r3 = Q.res * Q.res * Q.res, l = p % r3;
+    vox = Q.vox[p / r3];
+    const int ijk[3] = {l / (Q.res * Q.res), (l / Q.res) % Q.res, l % Q.res};
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+      xyz[d] = __fadd_rn(__fmul_rn(Q.lin[ijk[d]], Q.voxel_size), Q.centres[vox * 3 + d]);
+  } else {
+    vox = Q.vox[p];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) xyz[d] = Q.xyz[(size_t)p * 3 + d];
+  }
+  Corner c;
+  corners_at(Q.centres, Q.vertex_idx, Q.voxel_size, xyz, vox, c);
+  float x[EMB];
+  trilerp_emb(Q.emb, c, x);
+#pragma unroll
+  for (int q = 0; q < EMB; ++q) Q.acts[(size_t)(ra_x() + q) * Q.Pp + p] = x[q];
+}
+
+// colour rows [3][P] -> [P][3]
+__global__ void __launch_bounds__(256) k_vox_rgb_rows(int P, const float* rows, float* rgb) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+#pragma unroll
+  for (int q = 0; q < 3; ++q) rgb[(size_t)p * 3 + q] = rows[(size_t)q * P + p];
 }
 
 // d(colour logits) = d_rgb * c (1 - c) -> rows rg_do (+ a zero 4th row); dsdf -> row rg_dso
@@ -724,7 +780,86 @@ VWs vws(int R, int Pn, int with_grads) {
   L.total = q;
   return L;
 }
+
+// Decoder.get_values (decoder_voxfusion.py:122-149) as GEMMs over [feature][point] rows of
+// `acts` (x already gathered into rows ra_x).  rgb == nullptr: the sdf head only.
+int decoder_forward(const XrdVoxDecoder* dec, float* acts, int Pp, int Pn, float* sdf, float* rgb,
+                    cudaStream_t stream) {
+  auto ar = [&](int row) { return acts + (size_t)row * Pp; };
+#define XRD_GEMM(...)                                         \
+  do {                                                        \
+    GemmArgs g_ = __VA_ARGS__;                                \
+    XRD_CUDA_TRY(launch_gemm(g_, stream));                    \
+  } while (0)
+  XRD_GEMM({W, Pn, EMB, dec->w0, EMB, 0, ar(ra_x()), Pp, ar(ra_h1()), Pp, dec->b0, ACT_RELU});
+  XRD_GEMM({W, Pn, W, dec->w1, W, 0, ar(ra_h1()), Pp, ar(ra_h2()), Pp, dec->b1, ACT_RELU});
+  // sdf_out: torch row 0 = sdf, rows 1..128 = feat
+  if (rgb)
+    XRD_GEMM({W, Pn, W, dec->ws + W, W, 0, ar(ra_h2()), Pp, ar(ra_feat()), Pp, dec->bs + 1, ACT_NONE});
+  if (sdf) XRD_GEMM({1, Pn, W, dec->ws, W, 0, ar(ra_h2()), Pp, sdf, Pn, dec->bs, ACT_NONE});
+  if (!rgb) return XRD_OK;
+  // colour: relu(wc0 [feat, x] + bc0) -> sigmoid(wc1 . + bc1)
+  XRD_GEMM({W, Pn, W + EMB, dec->wc0, W + EMB, 0, ar(ra_feat()), Pp, ar(ra_c1()), Pp, dec->bc0, ACT_RELU});
+  XRD_GEMM({3, Pn, W, dec->wc1, W, 0, ar(ra_c1()), Pp, rgb, Pn, dec->bc1, ACT_SIGMOID});
+#undef XRD_GEMM
+  return XRD_OK;
+}
+
+// query workspace: activation rows + colour rows [3][P]
+struct QWs {
+  size_t acts, rgb, total;
+};
+QWs qws(int Pn) {
+  QWs L;
+  const size_t P = (size_t)(Pn > 0 ? Pn : 1), Pp = align_up(P, 64);
+  size_t q = 0;
+  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
+  L.acts = take((size_t)ra_rows() * Pp * 4);
+  L.rgb = take(3 * P * 4);
+  L.total = q;
+  return L;
+}
 }  // namespace
+
+extern "C" size_t xrd_voxfusion_query_workspace_bytes(int n_points) { return qws(n_points).total; }
+
+extern "C" int xrd_voxfusion_query(const XrdVoxMap* map, const XrdVoxDecoder* dec, float voxel_size,
+                                   int n, const int32_t* vox, int res, const float* lin,
+                                   const float* xyz, float* sdf, float* rgb, void* workspace,
+                                   size_t workspace_bytes, void* stream_) {
+  if (!map || !dec || !vox || !workspace) return XRD_E_NULL;
+  if (!map->centres || !map->vertex_idx || !map->embeddings) return XRD_E_NULL;
+  if (n < 0 || res < 0) return XRD_E_SHAPE;
+  if (res > 0) {
+    if (!lin || !sdf) return XRD_E_NULL;
+    if (xyz || rgb) return XRD_E_SHAPE;
+    if ((long long)n * res * res * res > 0x7fffffffLL) return XRD_E_SHAPE;
+  } else if (!xyz || !rgb) {
+    return XRD_E_NULL;
+  }
+  const int Pn = res > 0 ? n * res * res * res : n;
+  if (Pn == 0) return XRD_OK;
+  const QWs L = qws(Pn);
+  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  char* ws = reinterpret_cast<char*>(workspace);
+  QueryParams Q;
+  Q.P = Pn; Q.Pp = (int)align_up((size_t)Pn, 64); Q.res = res;
+  Q.vox = vox; Q.lin = lin; Q.xyz = xyz;
+  Q.centres = map->centres; Q.vertex_idx = map->vertex_idx; Q.emb = map->embeddings;
+  Q.voxel_size = voxel_size;
+  Q.acts = reinterpret_cast<float*>(ws + L.acts);
+  k_vox_query_gather<<<(Pn + T - 1) / T, T, 0, stream>>>(Q);
+  XRD_LAUNCH_CHECK();
+  float* rgb_rows = rgb ? reinterpret_cast<float*>(ws + L.rgb) : nullptr;
+  const int st = decoder_forward(dec, Q.acts, Q.Pp, Pn, sdf, rgb_rows, stream);
+  if (st != XRD_OK) return st;
+  if (rgb) {
+    k_vox_rgb_rows<<<(Pn + 255) / 256, 256, 0, stream>>>(Pn, rgb_rows, rgb);
+    XRD_LAUNCH_CHECK();
+  }
+  return XRD_OK;
+}
 
 extern "C" size_t xrd_voxfusion_render_workspace_bytes(int n_rays, int n_points, int with_grads) {
   return vws(n_rays, n_points, with_grads).total;
@@ -766,24 +901,13 @@ extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
   Q.need_dp = 0;
   // decoder (decoder_voxfusion.py:122-149) as GEMMs over [feature][point] rows
   auto ar = [&](int row) { return Q.acts + (size_t)row * Pp; };
-#define XRD_GEMM(...)                                         \
-  do {                                                        \
-    GemmArgs g_ = __VA_ARGS__;                                \
-    XRD_CUDA_TRY(launch_gemm(g_, stream));                    \
-  } while (0)
   {
   // timed bracket = the forward decoder chain: gather + 6 GEMM launches (bench.py's roofline)
   KernelTimer kt(stream);
   k_vox_gather<<<(Pn + T - 1) / T, T, 0, stream>>>(Q);
   XRD_LAUNCH_CHECK();
-  XRD_GEMM({W, Pn, EMB, dec->w0, EMB, 0, ar(ra_x()), Pp, ar(ra_h1()), Pp, dec->b0, ACT_RELU});
-  XRD_GEMM({W, Pn, W, dec->w1, W, 0, ar(ra_h1()), Pp, ar(ra_h2()), Pp, dec->b1, ACT_RELU});
-  // sdf_out: torch row 0 = sdf, rows 1..128 = feat
-  XRD_GEMM({W, Pn, W, dec->ws + W, W, 0, ar(ra_h2()), Pp, ar(ra_feat()), Pp, dec->bs + 1, ACT_NONE});
-  XRD_GEMM({1, Pn, W, dec->ws, W, 0, ar(ra_h2()), Pp, Q.sdf, Pn, dec->bs, ACT_NONE});
-  // colour: relu(wc0 [feat, x] + bc0) -> sigmoid(wc1 . + bc1)
-  XRD_GEMM({W, Pn, W + EMB, dec->wc0, W + EMB, 0, ar(ra_feat()), Pp, ar(ra_c1()), Pp, dec->bc0, ACT_RELU});
-  XRD_GEMM({3, Pn, W, dec->wc1, W, 0, ar(ra_c1()), Pp, Q.rgb, Pn, dec->bc1, ACT_SIGMOID});
+  const int st = decoder_forward(dec, Q.acts, Pp, Pn, Q.sdf, Q.rgb, stream);
+  if (st != XRD_OK) return st;
   }
 
   RayParams Y;

@@ -308,6 +308,55 @@ class SparseVoxel(Model):
         check('xrd_voxfusion_render', st)
         return o, g
 
+    # ------------------------------------------------ mesh-extraction queries ---
+    QUERY_POINTS = 1 << 18  # points per xrd_voxfusion_query call (~0.55 GB of activations)
+
+    def _query(self, n, vox, res=0, lin=None, xyz=None, sdf=None, rgb=None, ws=None):
+        lib = _cabi.lib()
+        dev = self.embeddings.device
+        dts = [t.detach() for t in self.decoder.tensors()]
+        dec = _dec_struct(dts, XrdVoxDecoder)
+        mp = self._map_struct(self.embeddings.detach())
+        with torch.cuda.device(dev):
+            st = lib.xrd_voxfusion_query(C.byref(mp), C.byref(dec), self.config.voxel_size, n,
+                                         ptr(vox), res, ptr(lin), ptr(xyz), ptr(sdf), ptr(rgb),
+                                         ptr(ws), ws.numel(),
+                                         torch.cuda.current_stream(dev).cuda_stream)
+        check('xrd_voxfusion_query', st)
+
+    def get_scores(self, vox_ids, res=8):
+        """voxel_helpers_voxfusion.py:15-59: sdf f32 [B,res,res,res] on the lattice
+        linspace(-0.5, 0.5, res)^3 * voxel_size + centre of every voxel (DEVICE node ids
+        vox_ids [B]); the colour head is skipped."""
+        dev = self.embeddings.device
+        ids = vox_ids.to(dev, torch.int32).contiguous()
+        B = ids.shape[0]
+        lin = torch.linspace(-.5, .5, res).to(dev)  # torch's symmetric fp32 linspace, on the host
+        sdf = torch.empty(B, res, res, res, dtype=torch.float32, device=dev)
+        per = max(1, self.QUERY_POINTS // res ** 3)
+        nb = _cabi.lib().xrd_voxfusion_query_workspace_bytes(min(B, per) * res ** 3)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        for s in range(0, B, per):
+            c = min(per, B - s)
+            self._query(c, ids[s:s + c], res, lin, sdf=sdf[s:s + c], ws=ws)
+        return sdf
+
+    def eval_points(self, xyz, vox_ids):
+        """voxel_helpers_voxfusion.py:62-94: colour f32 [P,3] at DEVICE points xyz [P,3] inside
+        voxels vox_ids [P] (node ids)."""
+        dev = self.embeddings.device
+        pts = xyz.detach().to(dev, torch.float32).contiguous()
+        ids = vox_ids.to(dev, torch.int32).contiguous()
+        P = pts.shape[0]
+        rgb = torch.empty(P, 3, dtype=torch.float32, device=dev)
+        per = self.QUERY_POINTS
+        nb = _cabi.lib().xrd_voxfusion_query_workspace_bytes(min(P, per))
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        for s in range(0, P, per):
+            c = min(per, P - s)
+            self._query(c, ids[s:s + c], xyz=pts[s:s + c], rgb=rgb[s:s + c], ws=ws)
+        return rgb
+
     # --------------------------------------------------------- Model API ---
     def get_outputs(self, input) -> Dict[str, Union[torch.Tensor, List]]:
         """sparse_voxel.py:152-159 (returns None when no ray hits a voxel, :179-181)."""

@@ -86,3 +86,64 @@ class VoxFusion(Algorithm):
     def render_img(self, c2w, gt_depth=None, idx=None):
         with self.lock, torch.no_grad():
             return self._render_full(c2w, gt_depth)
+
+    # voxfusion.py:171-176
+    def get_mesh(self):
+        with self.lock, torch.no_grad():
+            return self.extract_mesh(clean_mesh=False, require_color=True, res=8)
+
+    def surface_voxels(self):
+        """Surface leaves (voxfusion.py:180-185): node ids i64 [B], voxel rows f32 [B,4] (x, y,
+        z, side) and centres f32 [B,3], on the device."""
+        model = self.model
+        if model._dev_svo is not None:
+            voxels, _, features = model._dev_svo.export()
+        else:
+            voxels, _, features = (t.to(self.device) for t in model.export_octree())
+        keep = ~features.eq(-1).any(-1)
+        ids = torch.nonzero(keep).squeeze(1)
+        return ids, voxels[ids], model.map_states['voxel_center_xyz'][ids]
+
+    @torch.no_grad()
+    def extract_mesh(self, res=8, clean_mesh=False, require_color=False):
+        """voxfusion.py:178-248 -> TriMesh (None without a surface).  One batched lattice query
+        over every surface voxel, one batched marching cubes (vertices are not shared between
+        voxels, like the reference's per-voxel meshes), and the vertex -> voxel lookup
+        `points // voxel_size == voxels[:, :3]` as a sort + searchsorted over integer keys.
+        clean_mesh is a no-op in the reference as well (its TODO)."""
+        from .mesher import TriMesh, colors_to_u8, marching_cubes
+        if self.model.map_states is None:
+            return None
+        ids, voxels, centres = self.surface_voxels()
+        if ids.numel() == 0:
+            return None
+        vs = self.model.config.voxel_size
+        sdf = self.model.get_scores(ids, res)
+        s = 1.0 / (res - 1)
+        verts, faces = marching_cubes(sdf, 0.0, (s, s, s), shift=(-0.5,) * 3, scale=(vs,) * 3,
+                                      origin=centres)
+        if verts.shape[0] == 0:
+            return None
+        colors = None
+        if require_color:
+            colors = colors_to_u8(self.vertex_colors(verts, ids, voxels)).cpu().numpy()
+        return TriMesh(verts.cpu().numpy(), faces.cpu().numpy(), vertex_colors=colors)
+
+    def vertex_colors(self, verts, ids, voxels):
+        """voxfusion.py:205-239: colour f32 [V,3] of each vertex from the surface voxel with
+        voxels[:, :3] == verts // voxel_size (a vertex on a voxel face goes to the neighbour
+        its floor names), 0 where no surface voxel matches."""
+        keys = _voxel_keys(voxels[:, :3])
+        order = torch.argsort(keys)
+        skeys = keys[order]
+        q = _voxel_keys(verts // self.model.config.voxel_size)
+        pos = torch.searchsorted(skeys, q).clamp(max=skeys.shape[0] - 1)
+        hit = skeys[pos] == q
+        rgb = self.model.eval_points(verts, ids[order[pos]])
+        return torch.where(hit[:, None], rgb, torch.zeros_like(rgb))
+
+
+def _voxel_keys(v):
+    """int64 key of integer-valued voxel coordinates f32 [N,3] (|coordinate| < 2^20)."""
+    k = v.to(torch.int64) + (1 << 20)
+    return (k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2]
