@@ -609,6 +609,101 @@ int xrd_mesh_mc_emit(const float* values, int B, int nx, int ny, int nz, float l
                      const XrdMeshAffine* affine, float* verts, int32_t* faces, void* workspace,
                      size_t workspace_bytes, void* stream);
 
+/* ---- TSDF fusion (Point-SLAM get_mesh) -----------------------------------------
+ *
+ *   xrd_tsdf_alloc_*, xrd_tsdf_integrate  slam/common/common.py:622-657 (get_mesh_from_RGBD:
+ *                  open3d ScalableTSDFVolume(voxel_length 4/512, sdf_trunc 0.04, RGB8) and one
+ *                  volume.integrate per keyframe, on the host)
+ *   xrd_tsdf_mc_*  slam/common/common.py:658 (volume.extract_triangle_mesh)
+ *   xrd_tsdf_components  slam/common/common.py:666-677 (clean_mesh:
+ *                  trimesh.graph.connected_components over the mesh edges)
+ *
+ * open3d and trimesh are not vendored; the semantics below are this library's own.  Where a
+ * choice follows open3d it is marked [from memory -- unverified]; parity with open3d is
+ * unpinned.  A numpy restatement (oracle/tsdf.py) matches the kernels bit for bit.
+ *
+ * Volume.  Blocks of 16^3 voxels, voxel edge vl = voxel_length, block edge bl = 16 * vl
+ * [open3d's default block resolution, from memory -- unverified].  Block (bx, by, bz) is keyed
+ * by ((bx + 2^20) << 42) | ((by + 2^20) << 21) | (bz + 2^20) (21 signed bits per axis, int64,
+ * |b| < 2^20).  Voxel (i, j, k) of a block (x slowest, flat index i*256 + j*16 + k) has the
+ * centre b*bl + (i + 0.5)*vl per axis; it stores tsdf f32 (0 initially), weight f32 (0) and
+ * colour f32 [3] on the 0..255 scale (0).
+ *
+ * Inputs.  K frames: depth DEVICE f32 [K][H][W] (0 = invalid; d > depth_trunc counts as 0),
+ * colour DEVICE u8 [K][H][W][3], c2w DEVICE f32 [K][3][4] (camera to world, open3d axes: x
+ * right, y down, z forward) and w2c DEVICE f32 [K][3][4] (its inverse).  Camera coordinates
+ * of pixel (u, v) at depth d: x = ((u - cx) * d) / fx, y = ((v - cy) * d) / fy, z = d.  A
+ * [3][4] transform T maps p to ((T[r][0]*p0 + T[r][1]*p1) + T[r][2]*p2) + T[r][3].
+ *
+ * Allocation.  Every pixel with u % stride == 0, v % stride == 0 and a valid depth is
+ * back-projected with c2w to p; per axis the blocks floor((p - sdf_trunc) / bl) ..
+ * floor((p + sdf_trunc) / bl) are touched by the frame (at most 2 per axis: 2 * sdf_trunc <
+ * bl is required).  Points whose blocks leave the key range are skipped.  The allocated set is
+ * the sorted unique union of the touched keys; block ids are ranks in it.  Each block carries a
+ * touched-frame bitmask u32 [ceil(K/32)] (bit k%32 of word k/32).
+ *
+ * Integration [ScalableTSDFVolume semantics: a frame updates only the blocks it touched, from
+ * memory -- unverified].  For every voxel of every block, for the block's frames in order:
+ *   (x, y, z) = w2c * centre; skip if z <= 0;
+ *   u = floor(fx * x / z + cx + 0.5), v = floor(fy * y / z + cy + 0.5) (nearest pixel, halves
+ *   up); skip unless 0 <= u < W, 0 <= v < H and the depth d there is valid;
+ *   sdf = (d - z) * sqrt(((u - cx) / fx)^2 + ((v - cy) / fy)^2 + 1); skip if sdf <= -sdf_trunc;
+ *   t = min(1, sdf / sdf_trunc); tsdf = (tsdf * w + t) / (w + 1); colour = (colour * w +
+ *   c_k) / (w + 1) per channel; w = w + 1.
+ * Every fp32 operation is rounded to nearest in the order written (no contraction).
+ *
+ * Extraction.  A cube is anchored at every voxel of every block; its corners (i + di, j + dj,
+ * k + dk) with an index of 16 lie in the +x / +y / +z neighbour blocks.  A cube is used iff all
+ * 8 corners exist (allocated) with weight > 0; its case comes from csrc/mc_table.cuh with a
+ * corner negative iff tsdf < 0.  A crossed edge gets one vertex iff a used cube references it;
+ * the vertex belongs to the edge's lower voxel (possibly in a neighbour block), so vertices are
+ * shared across block seams.  Along the edge v0 -> v1: t = (0 - v0) / (v1 - v0); position
+ * ((c * vl + vl * 0.5) * 1) + b * bl per axis with c the lower voxel's local index plus t on the
+ * edge's axis (the mesh.cu affine); colour (c0 + t * (c1 - c0)) / 255.  Vertex order (block id,
+ * voxel, axis), face order (block id, voxel, triangle), both from exclusive scans; right-hand
+ * normals point toward positive tsdf (free space, the camera).  As with xrd_mesh_mc_*, a cube
+ * face whose four edges are crossed can carry a triangle of the case table flat in that face,
+ * which the cube on the other side emits reversed (rare: < 0.1% of faces on the synthetic room).
+ *
+ * Components.  labels[v] = the smallest vertex id connected to v through face edges (v itself
+ * for a vertex in no face); deterministic.  faces must index [0, n_verts).
+ *
+ * Two phases per pass as for xrd_mesh_mc_*: xrd_tsdf_alloc_count writes the block count to
+ * DEVICE n_blocks[1]; the caller allocates keys i64 [n_blocks] and masks u32 [n_blocks][ceil(K/
+ * 32)] and calls xrd_tsdf_alloc_emit with the same inputs' shape, params and workspace.
+ * xrd_tsdf_mc_count writes (V, F) to DEVICE counts[2]; xrd_tsdf_mc_emit fills verts f32 [V][3],
+ * colors f32 [V][3] and faces i32 [F][3] from the same keys, tsdf and workspace.  integrate
+ * updates tsdf / weight / color_acc ([n_blocks * 4096], [.], [. * 3]) of the blocks in keys in
+ * place with the masks' frames; n_blocks * 4096 < 2^31.  Nothing is allocated inside. */
+typedef struct {
+  float voxel_length;
+  float sdf_trunc;
+  float depth_trunc;
+  float fx, fy, cx, cy;
+  int stride; /* allocation samples every stride-th pixel in u and v                    */
+} XrdTsdfParams;
+
+size_t xrd_tsdf_alloc_workspace_bytes(int K, int H, int W, int stride);
+int xrd_tsdf_alloc_count(const float* depth, const float* c2w, int K, int H, int W,
+                         const XrdTsdfParams* params, int32_t* n_blocks, void* workspace,
+                         size_t workspace_bytes, void* stream);
+int xrd_tsdf_alloc_emit(int K, int H, int W, const XrdTsdfParams* params, int n_blocks,
+                        int64_t* keys, uint32_t* masks, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int xrd_tsdf_integrate(const int64_t* keys, const uint32_t* masks, int n_blocks,
+                       const float* depth, const uint8_t* color, const float* w2c, int K, int H,
+                       int W, const XrdTsdfParams* params, float* tsdf, float* weight,
+                       float* color_acc, void* stream);
+size_t xrd_tsdf_mc_workspace_bytes(int n_blocks);
+int xrd_tsdf_mc_count(const int64_t* keys, int n_blocks, const float* tsdf, const float* weight,
+                      int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+int xrd_tsdf_mc_emit(const int64_t* keys, int n_blocks, const float* tsdf,
+                     const float* color_acc, const XrdTsdfParams* params, float* verts,
+                     float* colors, int32_t* faces, void* workspace, size_t workspace_bytes,
+                     void* stream);
+int xrd_tsdf_components(const int32_t* faces, int n_faces, int n_verts, int32_t* labels,
+                        void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -170,6 +170,12 @@ class XrdMeshAffine(C.Structure):
                 ('origin', vp)]
 
 
+class XrdTsdfParams(C.Structure):
+    _fields_ = [('voxel_length', C.c_float), ('sdf_trunc', C.c_float), ('depth_trunc', C.c_float),
+                ('fx', C.c_float), ('fy', C.c_float), ('cx', C.c_float), ('cy', C.c_float),
+                ('stride', C.c_int)]
+
+
 class XrdPointIndex(C.Structure):
     _fields_ = [('pos', vp), ('n_points', C.c_int), ('cell', C.c_float),
                 ('table_size', C.c_int), ('cell_start', vp), ('cell_end', vp),
@@ -287,6 +293,18 @@ SYMBOLS = {
                                     C.c_size_t, vp]),
     'xrd_mesh_mc_emit': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                    C.POINTER(XrdMeshAffine), vp, vp, vp, C.c_size_t, vp]),
+    'xrd_tsdf_alloc_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    'xrd_tsdf_alloc_count': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int,
+                                       C.POINTER(XrdTsdfParams), vp, vp, C.c_size_t, vp]),
+    'xrd_tsdf_alloc_emit': (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(XrdTsdfParams),
+                                      C.c_int, vp, vp, vp, C.c_size_t, vp]),
+    'xrd_tsdf_integrate': (C.c_int, [vp, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int,
+                                     C.POINTER(XrdTsdfParams), vp, vp, vp, vp]),
+    'xrd_tsdf_mc_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'xrd_tsdf_mc_count': (C.c_int, [vp, C.c_int, vp, vp, vp, vp, C.c_size_t, vp]),
+    'xrd_tsdf_mc_emit': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(XrdTsdfParams), vp, vp, vp, vp,
+                                   C.c_size_t, vp]),
+    'xrd_tsdf_components': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

@@ -247,3 +247,41 @@ def get_camera_rays(H, W, fx, fy=None, cx=None, cy=None, type='OpenGL'):
     if type == 'OpenCV':
         return torch.stack([(i - cx) / fx, (j - cy) / fy, torch.ones_like(i)], -1)
     raise NotImplementedError(type)
+
+
+# ---- Point-SLAM mesh (common.py:622-711): TSDF fusion of the keyframes on the device ----------
+def get_mesh_from_RGBD(camera, keyframe_graph, scale=1, frame_tensor=None, device='cuda:0'):
+    """get_mesh_from_RGBD (common.py:622-663) on csrc/tsdf.cu: every keyframe, with its current
+    pose, is fused into a block-sparse TSDF volume (voxel_length 4/512 * scale, sdf_trunc 0.04 *
+    scale, colours (rgb * 255) as uint8); the coloured mesh is translated by compensate_vector.
+    -> TriMesh of DEVICE arrays (verts f32 [V,3], faces i32 [F,3], colours f32 [V,3] in [0,1]).
+    ``frame_tensor(frame, 'depth' | 'rgb')`` supplies the device images (Algorithm._frame_tensor
+    keeps them resident); by default they are uploaded here."""
+    from .mesher import TriMesh
+    from .tsdf import TSDFVolume, o3d_poses
+    if frame_tensor is None:
+        frame_tensor = lambda f, w: torch.as_tensor(np.asarray(getattr(f, w), dtype=np.float32)
+                                                    ).to(device)
+    c2w, w2c = o3d_poses([kf.get_pose().detach().cpu().numpy() for kf in keyframe_graph])
+    depth = torch.stack([frame_tensor(kf, 'depth') for kf in keyframe_graph])
+    color = torch.stack([(frame_tensor(kf, 'rgb') * 255).to(torch.uint8) for kf in keyframe_graph])
+    volume = TSDFVolume(voxel_length=4.0 * scale / 512.0, sdf_trunc=0.04 * scale,
+                        device=depth.device)
+    volume.integrate(depth, color, c2w, (camera.fx, camera.fy, camera.cx, camera.cy), w2c=w2c)
+    verts, faces, colors = volume.extract_triangle_mesh()
+    # address the misalignment in open3d marching cubes (common.py:637-639, fp32 here)
+    compensate = torch.tensor([-0.0 * scale / 512.0, 2.5 * scale / 512.0, -2.5 * scale / 512.0],
+                              dtype=torch.float32, device=verts.device)
+    return TriMesh(verts + compensate, faces, vertex_colors=colors)
+
+
+def clean_mesh(mesh, min_len=100):
+    """clean_mesh (common.py:666-711) on the device arrays of get_mesh_from_RGBD: weld
+    bit-identical vertices, keep the connected components with >= min_len vertices, drop
+    faces that repeat a vertex and duplicate faces (semantics in include/xrdslam_b200.h;
+    trimesh's tolerance-based merge is not reproduced).  -> TriMesh of HOST arrays with uint8
+    colours (mesher.colors_to_u8)."""
+    from .mesher import TriMesh, colors_to_u8
+    from .tsdf import clean_mesh_arrays
+    v, f, c = clean_mesh_arrays(mesh.vertices, mesh.faces, mesh.vertex_colors, min_len)
+    return TriMesh(v.cpu().numpy(), f.cpu().numpy(), vertex_colors=colors_to_u8(c).cpu().numpy())

@@ -69,6 +69,7 @@ class PointSLAMConfig(AlgorithmConfig):
     pointcloud_radius_query: float = 0.08
     pointcloud_radius_query_ratio: int = 2
     pointcloud_color_grad_threshold: float = 0.15
+    clean_mesh: bool = True
     optimizers: Dict[str, Any] = field(default_factory=_point_optimizers)
 
 
@@ -220,3 +221,26 @@ class PointSLAM(Algorithm):
                 per_pixel = {'batch_dynamic_r':
                              self.dynamic_r_query_allkeyframe[str(int(idx))].reshape(-1).float()}
             return self._render_full(c2w, gt_depth, extra={'stage': 'color'}, per_pixel=per_pixel)
+
+    # point_slam.py:426-435
+    def get_mesh(self):
+        """TSDF fusion of the keyframes (common.get_mesh_from_RGBD), cleaned with clean_mesh
+        when config.clean_mesh (vertices, faces, uint8 colours) or else vertices and faces only,
+        as the reference's Trimesh(vertices, faces).  None without keyframes or surface."""
+        from .common import clean_mesh, get_mesh_from_RGBD
+        from .mesher import TriMesh
+        with self.lock, torch.no_grad():
+            if not self.keyframe_graph:
+                return None
+            mesh = get_mesh_from_RGBD(self.camera, self.keyframe_graph,
+                                      frame_tensor=self._frame_tensor)
+            if mesh.faces.shape[0] == 0:
+                return None
+            if self.config.clean_mesh:
+                mesh = clean_mesh(mesh)
+                if mesh.faces.shape[0] == 0:
+                    return None
+            else:
+                mesh = TriMesh(mesh.vertices.cpu().numpy(), mesh.faces.cpu().numpy())
+            self.cur_mesh = mesh
+            return mesh
