@@ -704,6 +704,63 @@ int xrd_tsdf_mc_emit(const int64_t* keys, int n_blocks, const float* tsdf,
 int xrd_tsdf_components(const int32_t* faces, int n_faces, int n_verts, int32_t* labels,
                         void* stream);
 
+/* ---- Mesh culling (cull_mesh) ---------------------------------------------------
+ *
+ *   xrd_cull_visible  slam/common/common.py:714-783 (cull_mesh's per-frame loop: every vertex
+ *                     projected into every frame, an H2D copy of the vertices and a D2H copy of
+ *                     the mask per frame, ANDed on the host)
+ *   xrd_cull_count / xrd_cull_emit  common.py:784-787 (whole_mask[faces].all(1),
+ *                     mesh.update_faces, mesh.remove_unreferenced_vertices)
+ *
+ * Visibility.  verts DEVICE f32 [V][3] (the reference's .float() of the vertices); w2c DEVICE
+ * f32 [F][3][4], rows 0..2 of torch.inverse(c2w) of each frame (computed by the caller with that
+ * call); depth DEVICE f32 [F][H][W].  A [3][4] row applied to (x, y, z, 1) is ((T0*x + T1*y) +
+ * T2*z) + T3.  Per frame: cam = w2c (x, y, z, 1); xc = -cam.x, yc = cam.y, zc = cam.z;
+ * u' = fx*xc + cx*zc, v' = fy*yc + cy*zc (K's zero products are left out: a +-0 term changes no
+ * decision); z = zc + f32(1e-5); u = u' / z, v = v' / z.  The frame sees the vertex iff
+ *   0 <= -z, 0 < u < W, 0 < v < H   and, with eval_rec, d + truncation >= -z,
+ * where d = grid_sample(depth, 2 * (u / W, v / H) - 1, bilinear, padding 'zeros',
+ * align_corners=True): the source coordinate is ((g + 1) / 2) * (size - 1) per axis (so the
+ * pixel sampled is u * (W - 1) / W), corners (floor, floor + 1), weights nw = (x1 - ix) * (y1 -
+ * iy), ne = (ix - x0) * (y1 - iy), sw = (x1 - ix) * (iy - y0), se = (ix - x0) * (iy - y0), and
+ * d = ((nw*D_nw + ne*D_ne) + sw*D_sw) + se*D_se over the corners inside the image (zeros
+ * padding; invalid pixels, depth 0, take part).  [torch's scalar unnormalise and blend order,
+ * from memory -- unverified; torch's own kernels may contract or reorder, so bit parity with
+ * torch is unpinned.]  Every fp32 operation is rounded to nearest in the order written (no
+ * contraction).  The frustum tests come first: depth is read only for a vertex inside the image;
+ * behind the camera, at z ~ 0 and with a non-finite u or v the tests are false.
+ * seen u8 [V] is OR-ed in place (set to 1, never cleared); vertices already seen are skipped,
+ * so the result does not depend on how the frames are split over calls.  1 <= F <=
+ * XRD_CULL_MAX_FRAMES (the poses are staged in shared memory).
+ *
+ * Compaction.  A face is kept iff one of its vertices is seen (the reference removes the faces
+ * whose three vertices are all unseen); a vertex is kept iff a kept face references it (a seen
+ * vertex in no kept face is dropped, an unseen vertex of a kept face stays).  Both keep their
+ * order; faces are remapped to the kept vertices; colours (color_bytes bytes per vertex, any
+ * element type, or 0 = none) follow their vertices.  trimesh's tolerance merge in
+ * mesh.process(validate=False) is not reproduced (culling creates no new duplicates).
+ * xrd_cull_count writes (V', F', n_bad) to DEVICE counts[3], n_bad = faces with an index
+ * outside [0, V) (neither kept nor read; the caller treats n_bad > 0 as an error); the caller
+ * allocates verts f32 [V'][3], faces i32 [F'][3] and colours u8 [V'][color_bytes] and calls
+ * xrd_cull_emit with the same sizes and workspace (any output may be NULL).  Nothing is allocated
+ * inside. */
+#define XRD_CULL_MAX_FRAMES 1024
+typedef struct {
+  int H, W;
+  float fx, fy, cx, cy; /* rounded to f32 like the reference's K.float()                      */
+  float truncation;     /* f32, default 0.06                                                  */
+  int eval_rec;         /* 0: the depth term is dropped                                       */
+} XrdCullParams;
+
+int xrd_cull_visible(const float* verts, int n_verts, const float* w2c, const float* depth,
+                     int n_frames, const XrdCullParams* params, uint8_t* seen, void* stream);
+size_t xrd_cull_workspace_bytes(int n_verts, int n_faces);
+int xrd_cull_count(const uint8_t* seen, int n_verts, const int32_t* faces, int n_faces,
+                   int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+int xrd_cull_emit(const float* verts, const uint8_t* colors, int color_bytes, int n_verts,
+                  const int32_t* faces, int n_faces, float* out_verts, uint8_t* out_colors,
+                  int32_t* out_faces, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -176,6 +176,15 @@ class XrdTsdfParams(C.Structure):
                 ('stride', C.c_int)]
 
 
+XRD_CULL_MAX_FRAMES = 1024
+
+
+class XrdCullParams(C.Structure):
+    _fields_ = [('H', C.c_int), ('W', C.c_int), ('fx', C.c_float), ('fy', C.c_float),
+                ('cx', C.c_float), ('cy', C.c_float), ('truncation', C.c_float),
+                ('eval_rec', C.c_int)]
+
+
 class XrdPointIndex(C.Structure):
     _fields_ = [('pos', vp), ('n_points', C.c_int), ('cell', C.c_float),
                 ('table_size', C.c_int), ('cell_start', vp), ('cell_end', vp),
@@ -305,6 +314,12 @@ SYMBOLS = {
     'xrd_tsdf_mc_emit': (C.c_int, [vp, C.c_int, vp, vp, C.POINTER(XrdTsdfParams), vp, vp, vp, vp,
                                    C.c_size_t, vp]),
     'xrd_tsdf_components': (C.c_int, [vp, C.c_int, C.c_int, vp, vp]),
+    'xrd_cull_visible': (C.c_int, [vp, C.c_int, vp, vp, C.c_int, C.POINTER(XrdCullParams), vp,
+                                   vp]),
+    'xrd_cull_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int]),
+    'xrd_cull_count': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, C.c_size_t, vp]),
+    'xrd_cull_emit': (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp,
+                                C.c_size_t, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

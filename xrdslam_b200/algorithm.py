@@ -162,6 +162,22 @@ class Algorithm():
         from .io_formats import save_eval_tar
         return save_eval_tar(self, out_dir, idx)
 
+    def save_final_mesh(self, out_dir, dataset):
+        """The meshes `ds-eval` reads (tracker.py:388-400): get_mesh() once, written as
+        `<out_dir>/final_mesh.ply`, and its cull_mesh against every frame of `dataset` with the
+        estimated poses and eval_rec=True as `<out_dir>/final_mesh_rec.ply`.  -> the two paths,
+        or None when there is no mesh."""
+        import os
+        from .common import cull_mesh
+        mesh = self.get_mesh()
+        if mesh is None:
+            return None
+        os.makedirs(out_dir, exist_ok=True)
+        path = mesh.export(os.path.join(out_dir, 'final_mesh.ply'))
+        culled = cull_mesh(dataset, mesh, estimate_c2w_list=self.get_estimate_c2w_list(),
+                           eval_rec=True, device=self.device)
+        return path, culled.export(os.path.join(out_dir, 'final_mesh_rec.ply'))
+
     def is_separate_LR(self):
         with self.lock:
             return self.config.separate_LR

@@ -285,3 +285,169 @@ def clean_mesh(mesh, min_len=100):
     from .tsdf import clean_mesh_arrays
     v, f, c = clean_mesh_arrays(mesh.vertices, mesh.faces, mesh.vertex_colors, min_len)
     return TriMesh(v.cpu().numpy(), f.cpu().numpy(), vertex_colors=colors_to_u8(c).cpu().numpy())
+
+
+# ---- cull_mesh (common.py:714-789): the frames' visibility test on the device -----------------
+CULL_CHUNK = 16  # frames per depth upload and visibility launch
+
+
+def cull_w2c(c2w):
+    """Rows 0..2 of torch.inverse(c2w) for one f32 [4,4] DEVICE pose, as cull_mesh computes it
+    (common.py:745).  linalg.inv_ex is the same inverse without the host-synchronising error
+    check."""
+    return torch.linalg.inv_ex(c2w)[0][:3]
+
+
+def _cull_inputs(dataset, estimate_c2w_list, i):
+    _, _, depth, c2w = dataset[i]
+    if estimate_c2w_list is not None:
+        c2w = estimate_c2w_list[i]
+    return torch.as_tensor(depth), torch.as_tensor(c2w)
+
+
+def cull_visibility(dataset, vertices, estimate_c2w_list=None, eval_rec=False, truncation=0.06,
+                    device='cuda:0', chunk=CULL_CHUNK):
+    """seen u8 [V] on the device: 1 where some frame i < n_imgs sees the vertex (cull_mesh's
+    ~whole_mask, semantics in include/xrdslam_b200.h, csrc/cull.cu).  Frames go to the device
+    `chunk` at a time through two pinned host buffers and two device buffers, the upload of a
+    chunk on a side stream overlapping the visibility launch of the previous one; depth already
+    on the device is copied device to device.  Device memory beyond the vertices and `seen` is
+    2 * chunk * (H * W + 16) floats, whatever n_imgs is.  No host synchronisation per frame:
+    the host waits only before refilling a pinned buffer, for that buffer's previous upload."""
+    import ctypes as C
+    from . import _cabi
+    from ._cabi import XRD_CULL_MAX_FRAMES, XrdCullParams
+    dev = torch.device(device)
+    if dev.type != 'cuda':
+        raise RuntimeError('xrdslam_b200 has no CPU path: cull_mesh runs on a CUDA device')
+    n_imgs = len(estimate_c2w_list) if estimate_c2w_list is not None else len(dataset)
+    cam = dataset.get_camera()
+    H, W = int(cam.height), int(cam.width)
+    P = XrdCullParams(H, W, float(cam.fx), float(cam.fy), float(cam.cx), float(cam.cy),
+                      float(truncation), int(bool(eval_rec)))
+    verts = _as_dev(vertices, dev).reshape(-1, 3).contiguous()
+    V = verts.shape[0]
+    seen = torch.zeros(V, dtype=torch.uint8, device=dev)
+    if V == 0 or n_imgs == 0:
+        return seen
+    chunk = max(1, min(int(chunk), XRD_CULL_MAX_FRAMES, n_imgs))
+    lib = _cabi.lib()
+    with torch.cuda.device(dev):
+        main = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(dev)
+        depth_d = [torch.empty(chunk, H, W, device=dev) for _ in range(2)]
+        pose_d = [torch.empty(chunk, 4, 4, device=dev) for _ in range(2)]
+        depth_h = [None, None]
+        pose_h = [torch.empty(chunk, 4, 4).pin_memory() for _ in range(2)]
+        w2c = torch.empty(chunk, 3, 4, device=dev)
+        # the buffers come from the caller's stream: work still queued there may use their
+        # memory (a freed block's previous owner), so the side stream starts after it
+        side.wait_stream(main)
+        uploaded = [None, None]   # side stream: the buffers' last upload is done
+        consumed = [None, None]   # main stream: the buffers' last launch is done
+        for k, s in enumerate(range(0, n_imgs, chunk)):
+            b, n = k % 2, min(chunk, n_imgs - s)
+            if uploaded[b] is not None:
+                uploaded[b].synchronize()
+            on_dev = []
+            for j in range(n):
+                depth, c2w = _cull_inputs(dataset, estimate_c2w_list, s + j)
+                if tuple(depth.shape) != (H, W) or c2w.numel() != 16:
+                    raise ValueError(f'frame {s + j}: depth must be [{H},{W}] and c2w [4,4], got '
+                                     f'{tuple(depth.shape)} and {tuple(c2w.shape)}')
+                if depth.is_cuda:
+                    on_dev.append((depth_d[b][j], depth))
+                else:
+                    if depth_h[b] is None:
+                        depth_h[b] = torch.empty(chunk, H, W).pin_memory()
+                    depth_h[b][j].copy_(depth)
+                if c2w.is_cuda:
+                    on_dev.append((pose_d[b][j], c2w.reshape(4, 4)))
+                else:
+                    pose_h[b][j].copy_(c2w.reshape(4, 4))
+            ev = torch.cuda.Event()
+            with torch.cuda.stream(side):
+                if consumed[b] is not None:
+                    side.wait_event(consumed[b])
+                if depth_h[b] is not None:
+                    depth_d[b][:n].copy_(depth_h[b][:n], non_blocking=True)
+                pose_d[b][:n].copy_(pose_h[b][:n], non_blocking=True)
+                ev.record(side)
+            uploaded[b] = ev
+            main.wait_event(ev)
+            for dst, t in on_dev:   # device-resident inputs: on the main stream, after the upload
+                dst.copy_(t)
+            for j in range(n):
+                w2c[j].copy_(cull_w2c(pose_d[b][j]))
+            _cabi.check('xrd_cull_visible', lib.xrd_cull_visible(
+                _cabi.ptr(verts), V, _cabi.ptr(w2c), _cabi.ptr(depth_d[b]), n,
+                C.byref(P), _cabi.ptr(seen), main.cuda_stream))
+            consumed[b] = torch.cuda.Event()
+            consumed[b].record(main)
+    return seen
+
+
+def cull_compact(seen, vertices, faces, colors=None):
+    """update_faces(~whole_mask[faces].all(1)) + remove_unreferenced_vertices on DEVICE arrays
+    (csrc/cull.cu, order-preserving): -> (verts f32 [V',3], faces i32 [F',3], colours [V',...] of
+    the input's dtype or None).  One host read: the counts."""
+    from . import _cabi
+    dev = seen.device
+    V = seen.shape[0]
+    verts = vertices.to(dev, torch.float32).reshape(-1, 3).contiguous()
+    faces = faces.to(dev, torch.int32).reshape(-1, 3).contiguous()
+    nF = faces.shape[0]
+    if verts.shape[0] != V:
+        raise ValueError(f'{verts.shape[0]} vertices but a mask of {V}')
+    cb, cbytes = 0, None
+    if colors is not None:
+        colors = colors.to(dev).contiguous()
+        if colors.shape[0] != V:
+            raise ValueError('vertex_colors must have one row per vertex')
+        row = int(np.prod(colors.shape[1:], dtype=np.int64))
+        cb = row * colors.element_size()
+        cbytes = colors.reshape(V, row).view(torch.uint8)   # [V, cb]: any element type
+    lib = _cabi.lib()
+    nb = lib.xrd_cull_workspace_bytes(V, nF)
+    if nb == 0:
+        raise ValueError(f'cull_mesh: unsupported mesh size V={V}, F={nF}')
+    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    counts = torch.empty(3, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        s = torch.cuda.current_stream(dev).cuda_stream
+        _cabi.check('xrd_cull_count', lib.xrd_cull_count(
+            _cabi.ptr(seen), V, _cabi.ptr(faces), nF, _cabi.ptr(counts), _cabi.ptr(ws), nb, s))
+        V2, F2, bad = counts.tolist()
+        if bad:
+            raise ValueError(f'cull_mesh: {bad} faces index outside [0, {V})')
+        out_v = torch.empty(V2, 3, dtype=torch.float32, device=dev)
+        out_f = torch.empty(F2, 3, dtype=torch.int32, device=dev)
+        out_c = torch.empty(V2, cb, dtype=torch.uint8, device=dev) if colors is not None else None
+        _cabi.check('xrd_cull_emit', lib.xrd_cull_emit(
+            _cabi.ptr(verts), _cabi.ptr(cbytes), cb, V, _cabi.ptr(faces), nF, _cabi.ptr(out_v),
+            _cabi.ptr(out_c), _cabi.ptr(out_f), _cabi.ptr(ws), nb, s))
+    if colors is not None:
+        out_c = out_c.view(colors.dtype).reshape((V2, ) + tuple(colors.shape[1:]))
+    return out_v, out_f, out_c
+
+
+def cull_mesh(dataset, mesh, estimate_c2w_list=None, eval_rec=False, truncation=0.06,
+              device='cuda:0', chunk=CULL_CHUNK):
+    """cull_mesh (common.py:714-789) on the device: the faces of `mesh` (TriMesh of host numpy
+    or device tensor arrays, colours optional) that some frame i < n_imgs sees, n_imgs =
+    len(estimate_c2w_list) if given else len(dataset); frame i's depth is dataset[i][2] and its
+    pose estimate_c2w_list[i] if given else dataset[i][3].  With eval_rec a vertex hidden more
+    than `truncation` behind the frame's depth is not seen.  -> TriMesh of HOST arrays (f32
+    vertices); the input mesh is not modified.  trimesh's tolerance merge (process) is not
+    reproduced.  Host reads: the mesh counts, once."""
+    from .mesher import TriMesh
+    dev = torch.device(device)
+    tensor = lambda a: (torch.from_numpy(np.ascontiguousarray(a)) if isinstance(a, np.ndarray)
+                        else torch.as_tensor(a))
+    verts = tensor(mesh.vertices).to(dev, torch.float32).reshape(-1, 3)
+    faces = tensor(mesh.faces).to(dev, torch.int32).reshape(-1, 3)
+    colors = None if mesh.vertex_colors is None else tensor(mesh.vertex_colors)
+    seen = cull_visibility(dataset, verts, estimate_c2w_list, eval_rec, truncation, dev, chunk)
+    v, f, c = cull_compact(seen, verts, faces, colors)
+    return TriMesh(v.cpu().numpy(), f.cpu().numpy(),
+                   vertex_colors=None if c is None else c.cpu().numpy())
