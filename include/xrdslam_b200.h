@@ -761,6 +761,120 @@ int xrd_cull_emit(const float* verts, const uint8_t* colors, int color_bytes, in
                   const int32_t* faces, int n_faces, float* out_verts, uint8_t* out_colors,
                   int32_t* out_faces, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Reconstruction metrics (ds-eval) -------------------------------------------
+ *
+ *   xrd_eval_surface_* scripts/utils/eval_recon.py:120-124 (trimesh.sample.sample_surface) and
+ *                      evaluate_3d_reconstruction.py:182-201 (open3d sample_points_uniformly)
+ *   xrd_nn_*           eval_recon.py:29-47 (scipy cKDTree queries), open3d's
+ *                      compute_point_cloud_distance (evaluation.py:78-82) and the KD-tree
+ *                      correspondences of open3d's point-to-point registration_icp
+ *   xrd_eval_*_stats   the means / counts of those distances and ICP's correspondence sums
+ *   xrd_eval_transform trimesh's apply_transform of the mesh vertices
+ *
+ * Surface sampling.  xrd_eval_surface_prepare: verts DEVICE f32 [V][3], faces DEVICE i32 [F][3]
+ * (F >= 1, V >= 1, else XRD_E_SHAPE at once).  Face areas are float64: with a = v0 and the fp32
+ * coordinates widened exactly, e1 = v1 - a, e2 = v2 - a, c = e1 x e2 (each component
+ * e1y*e2z - e1z*e2y etc.), area = 0.5 * sqrt((cx*cx + cy*cy) + cz*cz).  cum DEVICE f64 [F] is
+ * their inclusive prefix in chunks of XRD_EVAL_AREA_CHUNK faces: sequential inside a chunk,
+ * plus the chunk's offset (the sequential sum of the earlier chunks' totals) in one final add
+ * (off + local); total DEVICE f64 [1] = the sum of the chunk totals.  status DEVICE i32 [1]
+ * becomes XRD_E_SHAPE when a vertex coordinate is not finite, a face index lies outside
+ * [0, V) (its area is not read) or the total is not finite and > 0; 0 otherwise.  The caller
+ * reads status and treats a non-zero value as the call's error; xrd_eval_sample_surface writes
+ * nothing while status is non-zero, so it never reads a bad face.
+ * xrd_eval_sample_surface writes out f32 [n][3] (and face_ids i32 [n], optional):
+ *   XRD_EVAL_TRIMESH (trimesh sample_surface; from memory, unverified): uniforms [n][3] =
+ *     (u0, u1, u2); face = first t with cum[t] >= u0 * total (f64; searchsorted 'left',
+ *     clamped to F - 1); if u1 + u2 > 1 (fp32) both become |u - 1|;
+ *     p = v0 + (u1 * (v1 - v0) + u2 * (v2 - v0)) per axis in fp32.
+ *   XRD_EVAL_OPEN3D (open3d sample_points_uniformly; from memory, unverified): sample k belongs
+ *     to the first face t with round((cum[t] / total) * n) > k (f64, round half away from
+ *     zero), so face t receives [round(C_{t-1} n), round(C_t n)) deterministically;
+ *     uniforms [n][2] = (r1, r2); s = sqrt(r1), a = 1 - s, b = s * (1 - r2), c = s * r2;
+ *     p = (a * v0 + b * v1) + c * v2 per axis in fp32.
+ * uniforms DEVICE f32 (parity mode) or NULL: then sample k draws philox4(seed, k) (common.cuh)
+ * and uses its first three (two) values.  The reference's draws are unseeded and its prefix
+ * sums are sequential, so the metrics are statistically equivalent to the reference's, not
+ * equal.  All fp32 / fp64 operations round to nearest in the order written.
+ *
+ * Exact nearest neighbour.  An index over target points P [N][3] is a dense grid over their
+ * bounding box: xrd_nn_layout (host, deterministic in N and the f64 box) picks the smallest cell
+ * h (64-step bisection) with prod_a (floor(ext_a / h) + 1) <= 2N cells and at most
+ * XRD_NN_MAX_DIM per axis, so the index is O(N); a box of zero extent gets h = 1 and one cell.
+ * Above the cells sit n_levels occupancy levels of an implicit octree (level l has
+ * ceil(dims / 2^l) nodes per axis, up to one root node).  xrd_nn_build bins every point by
+ * floor((x - origin) * inv_h) (fp32, clamped to the grid), radix-sorts (cell, id) so ids
+ * ascend inside a cell, and writes cell_ptr [n_cells + 1] (exclusive prefix of the counts),
+ * sorted f32 [N][4] = (x, y, z, id as int bits) and occ u8 [occ_bytes].  The caller allocates
+ * those three after xrd_nn_layout and reads the box once on the host.
+ * xrd_nn_query: for each query q the nearest target by
+ *   dx = q - p (fp32), d2 = (dx*dx + dy*dy) + dz*dz (fp32, round to nearest, no FMA),
+ *   ties on d2 to the smallest target id; dist = sqrt_rn(d2), ids = the target id.
+ * radius <= 0 or infinite: unbounded.  radius > 0: only targets with d2 <= fl(radius * radius)
+ * qualify; with none, ids = -1 and dist = +inf.  The search descends the octree near-first and
+ * skips a node whose box (padded by `pad`, larger than any rounding of the binning) lies
+ * further than the best d2 with a relative margin of 2e-5, so the result is the minimum of
+ * (d2, id) over all targets whatever the order and however the queries are split over calls.
+ * Queries outside the box start at the root like any other; work is bounded by the occupied
+ * nodes near the answer, not by the empty space in between.
+ *
+ * Reductions.  Element i of n goes to partial i / XRD_EVAL_RED_CHUNK; inside a partial thread
+ * t (of 256) sums its elements in index order, then a fixed shared-memory tree; the partials
+ * are summed in index order.  All sums are f64 (round to nearest), so a result is
+ * bit-identical run to run and depends only on the element values.
+ * xrd_eval_dist_stats: out DEVICE f64 [3] = (sum d, sum d*d, count of d < tau in fp32).
+ * xrd_eval_icp_stats: for each i with ids[i] >= 0 (s = src[i], t = tgt[ids[i]], both widened
+ * exactly to f64): out DEVICE f64 [17] = (count, sum s [3], sum t [3], sum s_a t_b [3][3]
+ * row-major, sum d*d).  Both take workspace >= xrd_eval_reduce_workspace_bytes(n).
+ * xrd_eval_transform: out = fp32(((T0 x + T1 y) + T2 z) + T3) per row, computed in f64 with
+ * the fp32 input widened exactly; T HOST f64 [3][4] (rows 0..2 of the 4x4, row-major), read
+ * before the call returns.  out may alias points.
+ * xrd_debug_nn_counters: DEVICE u64 [2] or NULL; when set, every later xrd_nn_query on this
+ * thread adds (octree nodes entered, target points tested) into it (thread-local, like the
+ * error state).  Nothing is allocated inside. */
+#define XRD_EVAL_AREA_CHUNK 256
+#define XRD_EVAL_RED_CHUNK 4096
+#define XRD_EVAL_TRIMESH 0
+#define XRD_EVAL_OPEN3D 1
+#define XRD_NN_MAX_DIM 32768
+#define XRD_NN_MAX_LEVELS 16
+typedef struct {
+  float origin[3];             /* f32(bbox_min)                                             */
+  float h, inv_h;              /* cell edge, f32(1 / h)                                     */
+  float pad;                   /* node boxes are widened by this much on every side         */
+  int dims[3];                 /* cells per axis                                            */
+  int n_cells, n_levels;       /* n_levels: octree levels above the cells (0 = one cell)    */
+  int level_off[XRD_NN_MAX_LEVELS]; /* offset of level l (1..n_levels) in occ             */
+  int occ_bytes;
+  int n_points;
+  const int32_t* cell_ptr;     /* DEVICE [n_cells + 1]                                      */
+  const uint8_t* occ;          /* DEVICE [occ_bytes] (may be NULL when n_levels == 0)       */
+  const float* sorted;         /* DEVICE [n_points][4], 16-byte aligned                     */
+} XrdNnIndex;
+
+size_t xrd_eval_surface_workspace_bytes(int n_faces);
+int xrd_eval_surface_prepare(const float* verts, int n_verts, const int32_t* faces, int n_faces,
+                             double* cum, double* total, int32_t* status, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int xrd_eval_sample_surface(const float* verts, const int32_t* faces, int n_faces,
+                            const double* cum, const double* total, const int32_t* status,
+                            int mode, int n_samples, const float* uniforms, uint64_t seed,
+                            float* out, int32_t* face_ids, void* stream);
+int xrd_nn_layout(int n_points, const double* bbox_min, const double* bbox_max,
+                  XrdNnIndex* index);
+size_t xrd_nn_build_workspace_bytes(const XrdNnIndex* index);
+int xrd_nn_build(const float* points, const XrdNnIndex* index, void* workspace,
+                 size_t workspace_bytes, void* stream);
+int xrd_nn_query(const XrdNnIndex* index, const float* queries, int n_queries, float radius,
+                 float* dist, int32_t* ids, void* stream);
+int xrd_debug_nn_counters(unsigned long long* counters);
+size_t xrd_eval_reduce_workspace_bytes(int n);
+int xrd_eval_dist_stats(const float* dist, int n, float tau, double* out, void* workspace,
+                        size_t workspace_bytes, void* stream);
+int xrd_eval_icp_stats(const float* src, const float* tgt, const int32_t* ids, const float* dist,
+                       int n, double* out, void* workspace, size_t workspace_bytes, void* stream);
+int xrd_eval_transform(const float* points, int n, const double* T, float* out, void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

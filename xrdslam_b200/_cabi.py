@@ -185,6 +185,18 @@ class XrdCullParams(C.Structure):
                 ('eval_rec', C.c_int)]
 
 
+XRD_EVAL_TRIMESH, XRD_EVAL_OPEN3D = 0, 1
+XRD_NN_MAX_LEVELS = 16
+
+
+class XrdNnIndex(C.Structure):
+    _fields_ = [('origin', C.c_float * 3), ('h', C.c_float), ('inv_h', C.c_float),
+                ('pad', C.c_float), ('dims', C.c_int * 3), ('n_cells', C.c_int),
+                ('n_levels', C.c_int), ('level_off', C.c_int * XRD_NN_MAX_LEVELS),
+                ('occ_bytes', C.c_int), ('n_points', C.c_int), ('cell_ptr', vp), ('occ', vp),
+                ('sorted', vp)]
+
+
 class XrdPointIndex(C.Structure):
     _fields_ = [('pos', vp), ('n_points', C.c_int), ('cell', C.c_float),
                 ('table_size', C.c_int), ('cell_start', vp), ('cell_end', vp),
@@ -320,6 +332,21 @@ SYMBOLS = {
     'xrd_cull_count': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, C.c_size_t, vp]),
     'xrd_cull_emit': (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp,
                                 C.c_size_t, vp]),
+    'xrd_eval_surface_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'xrd_eval_surface_prepare': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_size_t,
+                                           vp]),
+    'xrd_eval_sample_surface': (C.c_int, [vp, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp,
+                                          C.c_uint64, vp, vp, vp]),
+    'xrd_nn_layout': (C.c_int, [C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                C.POINTER(XrdNnIndex)]),
+    'xrd_nn_build_workspace_bytes': (C.c_size_t, [C.POINTER(XrdNnIndex)]),
+    'xrd_nn_build': (C.c_int, [vp, C.POINTER(XrdNnIndex), vp, C.c_size_t, vp]),
+    'xrd_nn_query': (C.c_int, [C.POINTER(XrdNnIndex), vp, C.c_int, C.c_float, vp, vp, vp]),
+    'xrd_debug_nn_counters': (C.c_int, [vp]),
+    'xrd_eval_reduce_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'xrd_eval_dist_stats': (C.c_int, [vp, C.c_int, C.c_float, vp, vp, C.c_size_t, vp]),
+    'xrd_eval_icp_stats': (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_size_t, vp]),
+    'xrd_eval_transform': (C.c_int, [vp, C.c_int, C.POINTER(C.c_double), vp, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

@@ -114,32 +114,104 @@ def write_ply(path, vertices, faces=None, colors=None):
     return path
 
 
+_PLY_SCALARS = {'char': 'i1', 'int8': 'i1', 'uchar': 'u1', 'uint8': 'u1', 'short': '<i2',
+                'int16': '<i2', 'ushort': '<u2', 'uint16': '<u2', 'int': '<i4', 'int32': '<i4',
+                'uint': '<u4', 'uint32': '<u4', 'float': '<f4', 'float32': '<f4',
+                'double': '<f8', 'float64': '<f8'}
+_PLY_COUNTS = ('uchar', 'uint8', 'ushort', 'uint16', 'int', 'int32', 'uint', 'uint32')
+_PLY_INDICES = ('int', 'int32', 'uint', 'uint32')
+
+
 def read_ply(path):
-    """Reader for the files `write_ply` (and trimesh / open3d with the same properties) produce:
+    """Binary little-endian PLY reader: the files `write_ply` (and trimesh / open3d with the same
+    properties) produce and ground-truth meshes as Replica ships them.  Vertex properties may be
+    any scalar type; faces are `list uchar|ushort|int|uint int|uint vertex_indices|vertex_index`
+    with any other face properties (scalars or lists) skipped.  ASCII and big-endian files and
+    other elements after the faces' are rejected with ValueError.
     -> (vertices f32 [n,3], faces i32 [m,3] or None, colors u8 [n,3] or None)."""
     with open(path, 'rb') as fh:
         data = fh.read()
-    end = data.index(b'end_header\n') + len(b'end_header\n')
-    lines = data[:end].decode('ascii').strip().split('\n')
-    assert lines[0] == 'ply' and lines[1].startswith('format binary_little_endian')
-    nv = nf = 0
-    vprops, cur = [], None
+    if not data.startswith(b'ply'):
+        raise ValueError(f'{path}: not a PLY file')
+    try:
+        end = data.index(b'end_header\n') + len(b'end_header\n')
+    except ValueError:
+        raise ValueError(f'{path}: PLY header has no end_header') from None
+    lines = [ln.strip() for ln in data[:end].decode('ascii').strip().split('\n')]
+    fmt = lines[1].split()
+    if fmt[:2] != ['format', 'binary_little_endian']:
+        raise ValueError(f'{path}: only binary_little_endian PLY is read, not {lines[1]!r}')
+    elements, cur = [], None
     for ln in lines[2:]:
         t = ln.split()
+        if not t or t[0] in ('comment', 'obj_info', 'end_header'):
+            continue
         if t[0] == 'element':
-            cur = t[1]
-            if cur == 'vertex':
-                nv = int(t[2])
-            elif cur == 'face':
-                nf = int(t[2])
-        elif t[0] == 'property' and cur == 'vertex':
-            vprops.append((t[2], {'float': '<f4', 'uchar': 'u1', 'double': '<f8'}[t[1]]))
-    dt = np.dtype(vprops)
-    rec = np.frombuffer(data, dtype=dt, count=nv, offset=end)
-    v = np.stack([rec['x'], rec['y'], rec['z']], -1).astype(np.float32)
-    c = np.stack([rec['red'], rec['green'], rec['blue']], -1) if 'red' in dt.names else None
-    f = None
-    if nf:
-        fdt = np.dtype([('n', 'u1'), ('i', '<i4', (3,))])
-        f = np.frombuffer(data, dtype=fdt, count=nf, offset=end + nv * dt.itemsize)['i'].copy()
-    return v, f, c
+            cur = (t[1], int(t[2]), [])
+            elements.append(cur)
+        elif t[0] == 'property':
+            if cur is None:
+                raise ValueError(f'{path}: property before any element')
+            if t[1] == 'list':
+                if t[2] not in _PLY_SCALARS or t[3] not in _PLY_SCALARS:
+                    raise ValueError(f'{path}: unsupported list property {ln!r}')
+                cur[2].append(('list', t[4], t[2], t[3]))
+            else:
+                if t[1] not in _PLY_SCALARS:
+                    raise ValueError(f'{path}: unsupported property type {ln!r}')
+                cur[2].append(('scalar', t[2], t[1]))
+    off = end
+    v = f = c = None
+    for name, count, props in elements:
+        if name == 'vertex':
+            if any(p[0] == 'list' for p in props):
+                raise ValueError(f'{path}: list properties on vertices are not supported')
+            dt = np.dtype([(p[1], _PLY_SCALARS[p[2]]) for p in props])
+            rec = np.frombuffer(data, dtype=dt, count=count, offset=off)
+            off += count * dt.itemsize
+            v = np.stack([rec['x'], rec['y'], rec['z']], -1).astype(np.float32)
+            if 'red' in dt.names:
+                c = np.stack([rec['red'], rec['green'], rec['blue']], -1).astype(np.uint8)
+        elif name == 'face':
+            f, off = _read_faces(path, data, off, count, props)
+        elif count:
+            raise ValueError(f'{path}: unsupported element {name!r}')
+    if v is None:
+        raise ValueError(f'{path}: no vertex element')
+    return v, (f if f is not None and len(f) else None), c
+
+
+def _read_faces(path, data, off, count, props):
+    lists = [p for p in props if p[0] == 'list' and p[1] in ('vertex_indices', 'vertex_index')]
+    if len(lists) != 1 or lists[0][2] not in _PLY_COUNTS or lists[0][3] not in _PLY_INDICES:
+        raise ValueError(f'{path}: faces need one list uchar|ushort|int|uint int|uint '
+                         'vertex_indices property')
+    if all(p[0] == 'scalar' or p is lists[0] for p in props):
+        # fixed-size records when every face is a triangle: one vectorised read
+        fields = []
+        for k, p in enumerate(props):
+            if p is lists[0]:
+                fields += [('n', _PLY_SCALARS[p[2]]), ('i', _PLY_SCALARS[p[3]], (3,))]
+            else:
+                fields.append((f's{k}', _PLY_SCALARS[p[2]]))
+        fdt = np.dtype(fields)
+        if off + count * fdt.itemsize <= len(data):
+            rec = np.frombuffer(data, dtype=fdt, count=count, offset=off)
+            if count == 0 or np.all(rec['n'] == 3):
+                return rec['i'].astype(np.int32), off + count * fdt.itemsize
+    faces = np.empty((count, 3), np.int32)
+    for r in range(count):
+        for p in props:
+            if p[0] == 'scalar':
+                off += np.dtype(_PLY_SCALARS[p[2]]).itemsize
+                continue
+            cdt, idt = np.dtype(_PLY_SCALARS[p[2]]), np.dtype(_PLY_SCALARS[p[3]])
+            n = int(np.frombuffer(data, cdt, 1, off)[0])
+            off += cdt.itemsize
+            vals = np.frombuffer(data, idt, n, off)
+            off += n * idt.itemsize
+            if p is lists[0]:
+                if n != 3:
+                    raise ValueError(f'{path}: face {r} has {n} vertices, only triangles are read')
+                faces[r] = vals
+    return faces, off

@@ -83,3 +83,46 @@ def make_sequence(n_frames, width=640, height=480, offset=(0.0, 0.0, 0.0)):
     frames = [render_frame(cam, p, offset=offset, seed=k)
               for k, p in enumerate(poses)]
     return cam, poses, frames
+
+
+def _grid_rect(origin, u, v, nu, nv):
+    """A rectangle origin + [0,1]u + [0,1]v as an (nu x nv)-cell triangle grid."""
+    a, b = np.meshgrid(np.linspace(0.0, 1.0, nu + 1), np.linspace(0.0, 1.0, nv + 1), indexing='ij')
+    verts = origin + a.reshape(-1, 1) * u + b.reshape(-1, 1) * v
+    idx = np.arange((nu + 1) * (nv + 1)).reshape(nu + 1, nv + 1)
+    q = np.stack([idx[:-1, :-1], idx[1:, :-1], idx[1:, 1:], idx[:-1, 1:]], -1).reshape(-1, 4)
+    faces = np.concatenate([q[:, [0, 1, 2]], q[:, [0, 2, 3]]])
+    return verts, faces
+
+
+def room_mesh(spacing=0.1):
+    """The analytic scene (ROOM's six walls and the BOXES' faces that do not lie on a wall) as a
+    triangle mesh with vertices about `spacing` apart: -> (verts f32 [V,3], faces i32 [F,3]).
+    The ground truth the reconstruction tests score against."""
+    verts, faces, base = [], [], 0
+
+    def box_faces(box, skip_walls):
+        for ax in range(3):
+            u_ax, v_ax = [a for a in range(3) if a != ax]
+            for side in range(2):
+                if skip_walls and box[ax, side] in (ROOM[ax, 0], ROOM[ax, 1]):
+                    continue
+                o = box[:, 0].astype(np.float64).copy()
+                o[ax] = box[ax, side]
+                u = np.zeros(3)
+                v = np.zeros(3)
+                u[u_ax] = box[u_ax, 1] - box[u_ax, 0]
+                v[v_ax] = box[v_ax, 1] - box[v_ax, 0]
+                yield o, u, v
+
+    rects = list(box_faces(ROOM, False))
+    for b in BOXES:
+        rects += list(box_faces(b, True))
+    for o, u, v in rects:
+        nu = max(1, int(round(np.linalg.norm(u) / spacing)))
+        nv = max(1, int(round(np.linalg.norm(v) / spacing)))
+        vv, ff = _grid_rect(o, u, v, nu, nv)
+        verts.append(vv)
+        faces.append(ff + base)
+        base += len(vv)
+    return np.concatenate(verts).astype(np.float32), np.concatenate(faces).astype(np.int32)
