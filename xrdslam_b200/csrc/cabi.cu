@@ -1,5 +1,5 @@
-// Host-side utilities of the C-ABI (no kernels): version, device check,
-// torch.linspace restatement, tcnn hash-grid level layout.
+// Host-side utilities of the C-ABI: version, device check, torch.linspace restatement, tcnn
+// hash-grid level layout, and the scan-totals copy shared by the compaction entry points.
 #include <math.h>
 #include <stdint.h>
 
@@ -22,6 +22,17 @@ int num_sms() {
     cached[dev] = n;
   }
   return cached[dev];
+}
+
+__global__ void k_copy_totals(int32_t* counts, const int* a, const int* b) {
+  counts[0] = *a;
+  if (b) counts[1] = *b;
+}
+
+int copy_totals(int32_t* counts, const int* a, const int* b, cudaStream_t stream) {
+  k_copy_totals<<<1, 1, 0, stream>>>(counts, a, b);
+  XRD_LAUNCH_CHECK();
+  return XRD_OK;
 }
 }  // namespace xrd
 

@@ -36,7 +36,63 @@ inline int cuda_fail(cudaError_t e) {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// blocks of `threads` threads that cover n items
+inline unsigned blocks(long long n, int threads = 256) { return (unsigned)((n + threads - 1) / threads); }
+
 int num_sms();
+
+// counts[0] = *a and, if b is not null, counts[1] = *b, in one launch on stream: copies the totals
+// at the end of exclusive scans to the caller.
+int copy_totals(int32_t* counts, const int* a, const int* b, cudaStream_t stream);
+
+// cub temp storage carved from a workspace, as the cub call takes it
+struct CubTemp { void* ptr; size_t bytes; };
+
+// Carves a caller-owned workspace into typed arrays, each starting on a 256-byte boundary.  A
+// workspace layout derives from it and takes its arrays in member initialisers, so the declaration
+// order is the layout.  With a null base the pointers are null and only the bytes are counted, so
+// the same layout sizes the workspace (xrd_*_workspace_bytes) and carves it (the entry point).
+class Carver {
+ public:
+  // bytes the layout needs; 0 if a cub query failed
+  size_t bytes() const { return err_ == cudaSuccess ? used_ : 0; }
+  // XRD_OK if the layout fits in workspace_bytes
+  int check(size_t workspace_bytes) const {
+    if (err_ != cudaSuccess) return cuda_fail(err_);
+    return workspace_bytes < used_ ? XRD_E_WORKSPACE : XRD_OK;
+  }
+
+ protected:
+  explicit Carver(void* base) : base_(static_cast<char*>(base)) {}
+  // n elements of T, padded to a multiple of 256 bytes
+  template <class T> T* take(size_t n) { return at<T>(align_up(n * sizeof(T), 256)); }
+  // n elements of T that end the workspace: no padding after them
+  template <class T> T* take_last(size_t n) { return at<T>(n * sizeof(T)); }
+  // Temp storage for the largest of several cub algorithms, each sized by a callable
+  // cudaError_t(size_t& bytes) that runs it with a null temp pointer.  A failed query leaves the
+  // layout unsizable.
+  template <class... Q> CubTemp cub(Q... queries) {
+    size_t bytes = 0;
+    auto query = [&](auto& q) {
+      size_t b = 0;
+      if (const cudaError_t e = q(b)) err_ = e;
+      if (b > bytes) bytes = b;
+    };
+    (query(queries), ...);
+    return {take<char>(bytes), bytes};
+  }
+
+ private:
+  // the next `bytes` of the workspace as a T*
+  template <class T> T* at(size_t bytes) {
+    const size_t off = used_;
+    used_ += bytes;
+    return base_ ? reinterpret_cast<T*>(base_ + off) : nullptr;
+  }
+  char* base_;
+  size_t used_ = 0;
+  cudaError_t err_ = cudaSuccess;
+};
 
 // ---------------------------------------------------------------- device ---
 #ifdef __CUDACC__

@@ -1876,9 +1876,17 @@ static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 using namespace xrd;
 using namespace xrd::coslam;
 
+// A 256-byte header that one memset clears: counts int[4] at +0, loss_acc double[4] at +64 and the
+// grouped kernel's work queue at +128.  Then z_vals, R*S floats.
+struct StepWs : Carver {
+  StepWs(void* base, int n_rays, int n_samples)
+      : Carver(base), hdr(take<char>(256)), z(take<float>((size_t)n_rays * n_samples)) {}
+  char* hdr;
+  float* z;
+};
+
 extern "C" size_t xrd_coslam_workspace_bytes(int n_rays, int n_samples) {
-  // [counts int[4] | loss_acc double[4] | z_vals R*S floats]
-  return 256 + align_up((size_t)n_rays * n_samples * sizeof(float), 256);
+  return StepWs(nullptr, n_rays, n_samples).bytes();
 }
 
 static int pick_rays_per_tile(int S, int requested) {
@@ -1955,17 +1963,17 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
     if (n_map == 0 && !grads->d_rays_o && !grads->d_rays_d) return XRD_E_NULL;
     if (grads->d_table && !aligned16(grads->d_table)) return XRD_E_SHAPE;
   }
-  if (workspace_bytes < xrd_coslam_workspace_bytes(R, S)) return XRD_E_WORKSPACE;
+  const StepWs L(workspace, R, S);
+  if (int st = L.check(workspace_bytes)) return st;
 
-  int* counts = reinterpret_cast<int*>(workspace);  // n_fs, n_sdf, n_valid
-  double* loss_acc = reinterpret_cast<double*>(reinterpret_cast<char*>(workspace) + 64);
-  float* z_ws = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  float* z_vals = out->z_vals ? out->z_vals : z_ws;
+  int* counts = reinterpret_cast<int*>(L.hdr);  // n_fs, n_sdf, n_valid
+  double* loss_acc = reinterpret_cast<double*>(L.hdr + 64);
+  float* z_vals = out->z_vals ? out->z_vals : L.z;
   const int phase = cfg->phase;  // 0: sample+render, 1: sample only, 2: render only
   if (phase < 0 || phase > 2) return XRD_E_SHAPE;
   if (phase != 0 && !out->z_vals) return XRD_E_NULL;
   if (phase == 1 && !cfg->counts_out) return XRD_E_NULL;
-  XRD_CUDA_TRY(cudaMemsetAsync(workspace, 0, 256, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.hdr, 0, 256, stream));
   if (phase == 1) {
     counts = cfg->counts_out;
     XRD_CUDA_TRY(cudaMemsetAsync(counts, 0, 4 * sizeof(int), stream));
@@ -2022,7 +2030,7 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
     // grouped persistent kernel (k_fused_g): units of NR rays pulled from a queue
     P.NR = GP / S;
     P.n_tiles = (R + P.NR - 1) / P.NR;
-    int* queue = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 128);  // zeroed above
+    int* queue = reinterpret_cast<int*>(L.hdr + 128);  // zeroed above
     // weights + NGROUPS x GP records + one z value per slot: 180 352 B, plus 18 432 B of
     // weight-gradient buffer when map gradients are on.  Four groups would fit (231 424 B) but
     // need <= 80 registers per thread and spill more; with three, what the 196 KB configuration
@@ -2059,9 +2067,16 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   return XRD_OK;
 }
 
+// loss_acc in a 256-byte header, then the features of the n^3 cells, n = sample_points - 1
+struct SmoothWs : Carver {
+  SmoothWs(void* base, int sample_points) : Carver(base), n((size_t)(sample_points - 1)) {}
+  const size_t n;
+  double* loss_acc = take<double>(1);
+  float* feat = take_last<float>(n * n * n * 32);
+};
+
 extern "C" size_t xrd_coslam_smoothness_workspace_bytes(int sample_points) {
-  size_t n = (size_t)(sample_points - 1);
-  return 256 + n * n * n * 32 * sizeof(float);
+  return SmoothWs(nullptr, sample_points).bytes();
 }
 
 static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double voxel_size,
@@ -2071,7 +2086,8 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
   if (!grid || !grid->table || !smooth_rand || !loss || !workspace) return XRD_E_NULL;
   if (sample_points < 3) return XRD_E_SHAPE;
   if (d_table && !aligned16(d_table)) return XRD_E_SHAPE;
-  if (workspace_bytes < xrd_coslam_smoothness_workspace_bytes(sample_points)) return XRD_E_WORKSPACE;
+  const SmoothWs L(workspace, sample_points);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
   SmoothParams p;
   int st = fill_grid(p.g, grid);
@@ -2090,12 +2106,12 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
   }
   p.margin = margin;
   p.rand_dev = rand_on_device ? smooth_rand : nullptr;
-  p.loss_acc = reinterpret_cast<double*>(workspace);
-  p.feat = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  p.loss_acc = L.loss_acc;
+  p.feat = L.feat;
   p.d_table = d_table;
   const double sp3 = (double)sample_points * sample_points * sample_points;
   p.coef = (float)((double)grad_scale * (double)weight / sp3);
-  XRD_CUDA_TRY(cudaMemsetAsync(workspace, 0, 256, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.loss_acc, 0, 256, stream));
   const int N = p.n * p.n * p.n;
   const int blocks = (N * kL + 255) / 256;
   k_smooth_fwd<<<blocks, 256, 0, stream>>>(p);

@@ -113,10 +113,6 @@ __global__ void __launch_bounds__(256) k_cull_faces(const uint8_t* __restrict__ 
   if (k) ref[id[0]] = ref[id[1]] = ref[id[2]] = 1;  // same value from every writer
 }
 
-__global__ void k_cull_totals(const int* vbase, int V, const int* fbase, int Fn, int32_t* counts) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) { counts[0] = vbase[V]; counts[1] = fbase[Fn]; }
-}
-
 __global__ void __launch_bounds__(256) k_cull_emit_verts(const float* __restrict__ verts,
                                                          const uint8_t* __restrict__ colors,
                                                          int color_bytes, int V,
@@ -149,32 +145,23 @@ __global__ void __launch_bounds__(256) k_cull_emit_faces(const int32_t* __restri
     out_faces[(size_t)o * 3 + m] = vbase[__ldg(faces + (size_t)f * 3 + m)];
 }
 
-struct Ws {
-  size_t keep, fbase, ref, vbase, scan, scan_bytes, total;
+struct Ws : Carver {
+  Ws(void* base, int V, int Fn) : Carver(base), V(V), Fn(Fn) {}
+  const int V, Fn;
+  int *keep = take<int>(Fn + 1), *fbase = take<int>(Fn + 1);
+  int *ref = take<int>(V + 1), *vbase = take<int>(V + 1);
+  CubTemp scan = cub(
+      [&](size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, Fn + 1);
+      },
+      [&](size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, V + 1);
+      });
 };
-
-Ws ws_layout(int V, int Fn) {
-  Ws L;
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.keep = take((size_t)(Fn + 1) * 4);
-  L.fbase = take((size_t)(Fn + 1) * 4);
-  L.ref = take((size_t)(V + 1) * 4);
-  L.vbase = take((size_t)(V + 1) * 4);
-  size_t a = 0, b = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, a, (const int*)nullptr, (int*)nullptr, Fn + 1);
-  cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, V + 1);
-  L.scan_bytes = a > b ? a : b;
-  L.scan = take(L.scan_bytes);
-  L.total = q;
-  return L;
-}
 
 bool sizes_ok(int V, int Fn) { return V >= 0 && Fn >= 0 && V < 0x7fffffff && Fn < 0x7fffffff; }
 
 bool params_ok(const XrdCullParams& P) { return P.H >= 1 && P.W >= 1; }
-
-unsigned blocks(long long n) { return (unsigned)((n + 255) / 256); }
 
 }  // namespace cull
 }  // namespace xrd
@@ -199,7 +186,7 @@ extern "C" int xrd_cull_visible(const float* verts, int n_verts, const float* w2
 
 extern "C" size_t xrd_cull_workspace_bytes(int n_verts, int n_faces) {
   if (!sizes_ok(n_verts, n_faces)) return 0;
-  return ws_layout(n_verts, n_faces).total;
+  return Ws(nullptr, n_verts, n_faces).bytes();
 }
 
 extern "C" int xrd_cull_count(const uint8_t* seen, int n_verts, const int32_t* faces, int n_faces,
@@ -208,26 +195,19 @@ extern "C" int xrd_cull_count(const uint8_t* seen, int n_verts, const int32_t* f
   if (!counts || !workspace || (n_verts > 0 && !seen) || (n_faces > 0 && !faces))
     return XRD_E_NULL;
   if (!sizes_ok(n_verts, n_faces)) return XRD_E_SHAPE;
-  const Ws L = ws_layout(n_verts, n_faces);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  Ws L(workspace, n_verts, n_faces);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  int* keep = reinterpret_cast<int*>(ws + L.keep);
-  int* fbase = reinterpret_cast<int*>(ws + L.fbase);
-  int* ref = reinterpret_cast<int*>(ws + L.ref);
-  int* vbase = reinterpret_cast<int*>(ws + L.vbase);
-  XRD_CUDA_TRY(cudaMemsetAsync(ref, 0, (size_t)(n_verts + 1) * 4, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.ref, 0, (size_t)(n_verts + 1) * 4, stream));
   XRD_CUDA_TRY(cudaMemsetAsync(counts, 0, 3 * sizeof(int32_t), stream));
   k_cull_faces<<<blocks((long long)n_faces + 1), 256, 0, stream>>>(seen, n_verts, faces, n_faces,
-                                                                   keep, ref, counts + 2);
+                                                                   L.keep, L.ref, counts + 2);
   XRD_LAUNCH_CHECK();
-  size_t sb = L.scan_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.scan, sb, keep, fbase, n_faces + 1, stream));
-  sb = L.scan_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.scan, sb, ref, vbase, n_verts + 1, stream));
-  k_cull_totals<<<1, 32, 0, stream>>>(vbase, n_verts, fbase, n_faces, counts);
-  XRD_LAUNCH_CHECK();
-  return XRD_OK;
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.scan.ptr, L.scan.bytes, L.keep, L.fbase,
+                                             n_faces + 1, stream));
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.scan.ptr, L.scan.bytes, L.ref, L.vbase,
+                                             n_verts + 1, stream));
+  return copy_totals(counts, L.vbase + n_verts, L.fbase + n_faces, stream);
 }
 
 extern "C" int xrd_cull_emit(const float* verts, const uint8_t* colors, int color_bytes,
@@ -239,22 +219,18 @@ extern "C" int xrd_cull_emit(const float* verts, const uint8_t* colors, int colo
   if ((out_verts && n_verts > 0 && !verts) || (out_faces && n_faces > 0 && !faces) ||
       (out_colors && color_bytes > 0 && n_verts > 0 && !colors))
     return XRD_E_NULL;
-  const Ws L = ws_layout(n_verts, n_faces);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const Ws L(workspace, n_verts, n_faces);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  const int* keep = reinterpret_cast<const int*>(ws + L.keep);
-  const int* fbase = reinterpret_cast<const int*>(ws + L.fbase);
-  const int* vbase = reinterpret_cast<const int*>(ws + L.vbase);
   if (!color_bytes) out_colors = nullptr;
   if (n_verts > 0 && (out_verts || out_colors)) {
     k_cull_emit_verts<<<blocks(n_verts), 256, 0, stream>>>(verts, colors, color_bytes, n_verts,
-                                                           vbase, out_verts, out_colors);
+                                                           L.vbase, out_verts, out_colors);
     XRD_LAUNCH_CHECK();
   }
   if (n_faces > 0 && out_faces) {
-    k_cull_emit_faces<<<blocks(n_faces), 256, 0, stream>>>(faces, n_faces, keep, fbase, vbase,
-                                                           out_faces);
+    k_cull_emit_faces<<<blocks(n_faces), 256, 0, stream>>>(faces, n_faces, L.keep, L.fbase,
+                                                           L.vbase, out_faces);
     XRD_LAUNCH_CHECK();
   }
   return XRD_OK;

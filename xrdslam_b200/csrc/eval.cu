@@ -28,8 +28,6 @@ constexpr int kChunk = XRD_EVAL_AREA_CHUNK;    // faces per sequential prefix-su
 constexpr int kRedChunk = XRD_EVAL_RED_CHUNK;  // elements per reduction partial
 constexpr int kRedThreads = 256;
 
-unsigned blocks(long long n, int t = 256) { return (unsigned)((n + t - 1) / t); }
-
 // ---------------------------------------------------------------- surface sampling ---
 __device__ __forceinline__ double face_area(const float* __restrict__ V, int a, int b, int c) {
   const double ax = V[3 * a], ay = V[3 * a + 1], az = V[3 * a + 2];
@@ -380,30 +378,31 @@ __global__ void __launch_bounds__(256) k_transform(const float* __restrict__ in,
 int n_chunks(int nF) { return (nF + kChunk - 1) / kChunk; }
 int n_partials(int n) { return n <= 0 ? 1 : (n + kRedChunk - 1) / kRedChunk; }
 
-struct NnWs {
-  size_t keys, keys2, ids, ids2, counts, sort, sort_bytes, scan, scan_bytes, total;
+struct NnWs : Carver {
+  NnWs(void* base, int n, int n_cells) : Carver(base), n(n), n_cells(n_cells) {}
+  const int n, n_cells;
+  int *keys = take<int>(n), *keys2 = take<int>(n), *ids = take<int>(n), *ids2 = take<int>(n);
+  int* counts = take<int>(n_cells + 1);
+  CubTemp sort = cub([&](size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(nullptr, b, (const int*)nullptr, (int*)nullptr,
+                                           (const int*)nullptr, (int*)nullptr, n);
+  });
+  CubTemp scan = cub([&](size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, n_cells + 1);
+  });
 };
 
-NnWs nn_ws(int n, int n_cells) {
-  NnWs L;
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.keys = take((size_t)n * 4);
-  L.keys2 = take((size_t)n * 4);
-  L.ids = take((size_t)n * 4);
-  L.ids2 = take((size_t)n * 4);
-  L.counts = take((size_t)(n_cells + 1) * 4);
-  L.sort_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, L.sort_bytes, (const int*)nullptr, (int*)nullptr,
-                                  (const int*)nullptr, (int*)nullptr, n);
-  L.sort = take(L.sort_bytes);
-  L.scan_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, L.scan_bytes, (const int*)nullptr, (int*)nullptr,
-                                n_cells + 1);
-  L.scan = take(L.scan_bytes);
-  L.total = q;
-  return L;
-}
+// area prefix sums: one double per chunk of faces
+struct SurfaceWs : Carver {
+  SurfaceWs(void* base, int n_faces) : Carver(base), tot(take<double>(n_chunks(n_faces))) {}
+  double* tot;
+};
+
+// reduction partials: 17 doubles (the most a reduction has) per chunk
+struct ReduceWs : Carver {
+  ReduceWs(void* base, int n) : Carver(base), part(take_last<double>((size_t)n_partials(n) * 17)) {}
+  double* part;
+};
 
 long long cells_for(const double ext[3], double h, int dims[3]) {
   long long c = 1;
@@ -429,7 +428,7 @@ using namespace xrd::eval;
 
 extern "C" size_t xrd_eval_surface_workspace_bytes(int n_faces) {
   if (n_faces < 1) return 0;
-  return align_up((size_t)n_chunks(n_faces) * sizeof(double), 256) + 256;
+  return SurfaceWs(nullptr, n_faces).bytes();
 }
 
 extern "C" int xrd_eval_surface_prepare(const float* verts, int n_verts, const int32_t* faces,
@@ -437,9 +436,10 @@ extern "C" int xrd_eval_surface_prepare(const float* verts, int n_verts, const i
                                         void* workspace, size_t workspace_bytes, void* stream_) {
   if (n_faces < 1 || n_verts < 1) return XRD_E_SHAPE;
   if (!verts || !faces || !cum || !total || !status || !workspace) return XRD_E_NULL;
-  if (workspace_bytes < xrd_eval_surface_workspace_bytes(n_faces)) return XRD_E_WORKSPACE;
+  const SurfaceWs L(workspace, n_faces);
+  if (int st = L.check(workspace_bytes)) return st;
+  double* tot = L.tot;
   cudaStream_t s = (cudaStream_t)stream_;
-  double* tot = reinterpret_cast<double*>(workspace);
   const int nc = n_chunks(n_faces);
   XRD_CUDA_TRY(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
   k_check_verts<<<blocks(3LL * n_verts), 256, 0, s>>>(verts, n_verts, status);
@@ -523,7 +523,7 @@ extern "C" int xrd_nn_layout(int n_points, const double* bbox_min, const double*
 
 extern "C" size_t xrd_nn_build_workspace_bytes(const XrdNnIndex* index) {
   if (!index || index->n_points < 1 || index->n_cells < 1) return 0;
-  return nn_ws(index->n_points, index->n_cells).total;
+  return NnWs(nullptr, index->n_points, index->n_cells).bytes();
 }
 
 extern "C" int xrd_nn_build(const float* points, const XrdNnIndex* index, void* workspace,
@@ -531,34 +531,26 @@ extern "C" int xrd_nn_build(const float* points, const XrdNnIndex* index, void* 
   if (!points || !index || !workspace) return XRD_E_NULL;
   const XrdNnIndex I = *index;
   if (!index_ok(I)) return I.cell_ptr && I.sorted ? XRD_E_SHAPE : XRD_E_NULL;
-  const NnWs L = nn_ws(I.n_points, I.n_cells);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  NnWs L(workspace, I.n_points, I.n_cells);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t s = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  int* keys = reinterpret_cast<int*>(ws + L.keys);
-  int* keys2 = reinterpret_cast<int*>(ws + L.keys2);
-  int* ids = reinterpret_cast<int*>(ws + L.ids);
-  int* ids2 = reinterpret_cast<int*>(ws + L.ids2);
-  int* counts = reinterpret_cast<int*>(ws + L.counts);
   const int n = I.n_points;
-  XRD_CUDA_TRY(cudaMemsetAsync(counts, 0, (size_t)(I.n_cells + 1) * 4, s));
-  k_nn_keys<<<blocks(n), 256, 0, s>>>(points, n, I, keys, ids, counts);
+  XRD_CUDA_TRY(cudaMemsetAsync(L.counts, 0, (size_t)(I.n_cells + 1) * 4, s));
+  k_nn_keys<<<blocks(n), 256, 0, s>>>(points, n, I, L.keys, L.ids, L.counts);
   XRD_LAUNCH_CHECK();
   int end_bit = 1;
   while (end_bit < 31 && (I.n_cells - 1) >> end_bit) ++end_bit;
-  size_t sb = L.sort_bytes;
-  XRD_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.sort, sb, keys, keys2, ids, ids2, n, 0,
-                                               end_bit, s));
-  sb = L.scan_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.scan, sb, counts,
+  XRD_CUDA_TRY(cub::DeviceRadixSort::SortPairs(L.sort.ptr, L.sort.bytes, L.keys, L.keys2, L.ids,
+                                               L.ids2, n, 0, end_bit, s));
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.scan.ptr, L.scan.bytes, L.counts,
                                              const_cast<int32_t*>(I.cell_ptr), I.n_cells + 1, s));
-  k_nn_gather<<<blocks(n), 256, 0, s>>>(points, n, ids2, reinterpret_cast<float4*>(
-                                                              const_cast<float*>(I.sorted)));
+  k_nn_gather<<<blocks(n), 256, 0, s>>>(points, n, L.ids2, reinterpret_cast<float4*>(
+                                                                const_cast<float*>(I.sorted)));
   XRD_LAUNCH_CHECK();
   if (I.n_levels > 0) {
     uint8_t* occ = const_cast<uint8_t*>(I.occ);
     XRD_CUDA_TRY(cudaMemsetAsync(occ, 0, (size_t)I.occ_bytes, s));
-    k_nn_occupancy<<<blocks(I.n_cells), 256, 0, s>>>(I, counts, occ);
+    k_nn_occupancy<<<blocks(I.n_cells), 256, 0, s>>>(I, L.counts, occ);
     XRD_LAUNCH_CHECK();
   }
   return XRD_OK;
@@ -585,16 +577,17 @@ extern "C" int xrd_debug_nn_counters(unsigned long long* counters) {
 
 extern "C" size_t xrd_eval_reduce_workspace_bytes(int n) {
   if (n < 0) return 0;
-  return (size_t)n_partials(n) * 17 * sizeof(double);
+  return ReduceWs(nullptr, n).bytes();
 }
 
 extern "C" int xrd_eval_dist_stats(const float* dist, int n, float tau, double* out,
                                    void* workspace, size_t workspace_bytes, void* stream_) {
   if (!out || !workspace || (n > 0 && !dist)) return XRD_E_NULL;
   if (n < 0) return XRD_E_SHAPE;
-  if (workspace_bytes < xrd_eval_reduce_workspace_bytes(n)) return XRD_E_WORKSPACE;
+  const ReduceWs L(workspace, n);
+  if (int st = L.check(workspace_bytes)) return st;
+  double* part = L.part;
   cudaStream_t s = (cudaStream_t)stream_;
-  double* part = reinterpret_cast<double*>(workspace);
   const int np = n_partials(n);
   k_dist_partials<<<np, kRedThreads, 0, s>>>(dist, n, tau, part);
   XRD_LAUNCH_CHECK();
@@ -608,9 +601,10 @@ extern "C" int xrd_eval_icp_stats(const float* src, const float* tgt, const int3
                                   size_t workspace_bytes, void* stream_) {
   if (!out || !workspace || (n > 0 && (!src || !tgt || !ids || !dist))) return XRD_E_NULL;
   if (n < 0) return XRD_E_SHAPE;
-  if (workspace_bytes < xrd_eval_reduce_workspace_bytes(n)) return XRD_E_WORKSPACE;
+  const ReduceWs L(workspace, n);
+  if (int st = L.check(workspace_bytes)) return st;
+  double* part = L.part;
   cudaStream_t s = (cudaStream_t)stream_;
-  double* part = reinterpret_cast<double*>(workspace);
   const int np = n_partials(n);
   k_icp_partials<<<np, kRedThreads, 0, s>>>(src, tgt, ids, dist, n, part);
   XRD_LAUNCH_CHECK();

@@ -929,33 +929,28 @@ using namespace xrd;
 using namespace xrd::nice;
 
 namespace {
-struct WsLayout {
-  size_t hdr, z, occ_mid, occ_fine, rgb, d_occ, d_rgb, masks, dp, gd, gc, tmp, depth, var, orgb, acts, total;
+struct Ws : Carver {
+  Ws(void* base, int R, int S, int with_grads)
+      : Carver(base), R(R), P((size_t)R * S), g(with_grads != 0) {}
+  const size_t R, P;
+  const bool g;
+  float* maxd = take<float>(1);  // alone in a 256-byte header
+  double* z = take<double>(P);
+  float *occ_mid = take<float>(P), *occ_fine = take<float>(P), *rgb = take<float>(3 * P);
+  double *depth = take<double>(R), *var = take<double>(R);  // per-ray rows, reserved and unused
+  float* orgb = take<float>(R * 3);
+  // with_grads only
+  float *d_occ = g ? take<float>(P) : nullptr, *d_rgb = g ? take<float>(3 * P) : nullptr;
+  uint32_t* masks = g ? take<uint32_t>(3 * 5 * P) : nullptr;
+  float* dp = g ? take<float>(3 * P) : nullptr;
+  float *gd = g ? take<float>(R) : nullptr, *gc = g ? take<float>(R * 3) : nullptr;
+  double* tmp = g ? take<double>(R) : nullptr;
+  float* acts = g ? take<float>((size_t)n_rows(32) * align_up(P, 64)) : nullptr;
 };
-WsLayout ws_layout(int R, int S, int with_grads) {
-  WsLayout L;
-  const size_t P = (size_t)R * S, Pp = align_up(P, 64);
-  size_t q = 0;
-  auto take = [&](size_t bytes) { size_t o = q; q += align_up(bytes, 256); return o; };
-  L.hdr = take(256);
-  L.z = take(P * 8);
-  L.occ_mid = take(P * 4); L.occ_fine = take(P * 4); L.rgb = take(3 * P * 4);
-  L.depth = take((size_t)R * 8); L.var = take((size_t)R * 8); L.orgb = take((size_t)R * 12);
-  L.d_occ = L.d_rgb = L.masks = L.dp = L.gd = L.gc = L.tmp = L.acts = 0;
-  if (with_grads) {
-    L.d_occ = take(P * 4); L.d_rgb = take(3 * P * 4);
-    L.masks = take(3 * 5 * P * 4);
-    L.dp = take(3 * P * 4);
-    L.gd = take((size_t)R * 4); L.gc = take((size_t)R * 12); L.tmp = take((size_t)R * 8);
-    L.acts = take((size_t)n_rows(32) * Pp * 4);
-  }
-  L.total = q;
-  return L;
-}
 }  // namespace
 
 extern "C" size_t xrd_nice_workspace_bytes(int n_rays, int n_samples_total, int with_grads) {
-  return ws_layout(n_rays, n_samples_total, with_grads).total;
+  return Ws(nullptr, n_rays, n_samples_total, with_grads).bytes();
 }
 
 extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
@@ -974,27 +969,25 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   if (decoders[0].n_out != 1 || decoders[1].n_out != 1 || decoders[2].n_out != 4) return XRD_E_SHAPE;
   if (grads && (!rays->target_s || !out->losses)) return XRD_E_NULL;
   if (grads && !cfg->is_mapping && R > 8192) return XRD_E_SHAPE;  // single-block median
-  const WsLayout L = ws_layout(R, S, grads != nullptr);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const Ws L(workspace, R, S, grads != nullptr);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   const int P = R * S, Pp = (int)align_up((size_t)P, 64);
-  double* z = out->z_vals ? out->z_vals : reinterpret_cast<double*>(ws + L.z);
-  float* maxd = reinterpret_cast<float*>(ws + L.hdr);
-  float* occ_mid = reinterpret_cast<float*>(ws + L.occ_mid);
-  float* occ_fine = reinterpret_cast<float*>(ws + L.occ_fine);
-  float* rgb = reinterpret_cast<float*>(ws + L.rgb);
+  double* z = out->z_vals ? out->z_vals : L.z;
+  float* occ_mid = L.occ_mid;
+  float* occ_fine = L.occ_fine;
+  float* rgb = L.rgb;
   const int stage = cfg->stage;
 
   if (!cfg->max_depth_global) {
-    k_maxdepth<<<1, 1024, 0, stream>>>(rays->target_d, R, maxd);
+    k_maxdepth<<<1, 1024, 0, stream>>>(rays->target_d, R, L.maxd);
     XRD_LAUNCH_CHECK();
   }
   SampleParams sp;
   sp.R = R; sp.ns = cfg->n_samples; sp.nsurf = cfg->n_surface; sp.no_depth = 0;
   sp.rays_o = rays->rays_o; sp.rays_d = rays->rays_d; sp.target_d = rays->target_d;
   for (int d = 0; d < 3; ++d) { sp.bmin[d] = cfg->bound_min[d]; sp.bmax[d] = cfg->bound_max[d]; }
-  sp.maxd = cfg->max_depth_global ? cfg->max_depth_global : maxd; sp.z = z;
+  sp.maxd = cfg->max_depth_global ? cfg->max_depth_global : L.maxd; sp.z = z;
   sp.t_uniform = cfg->t_uniform; sp.t_surface = cfg->t_surface;
   k_sample<<<(R + 3) / 4, 128, 0, stream>>>(sp);
   XRD_LAUNCH_CHECK();
@@ -1010,9 +1003,9 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
     if (d == 1) { D.gb.data = grids[0].data; D.gb.nx = grids[0].nx; D.gb.ny = grids[0].ny; D.gb.nz = grids[0].nz; }
     D.dec = decoders[d];
     for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
-    D.masks = grads ? reinterpret_cast<uint32_t*>(ws + L.masks) + (size_t)d * 5 * P : nullptr;
+    D.masks = grads ? L.masks + (size_t)d * 5 * P : nullptr;
     D.acts = nullptr; D.Pp = Pp;
-    D.dp = grads ? reinterpret_cast<float*>(ws + L.dp) : nullptr;
+    D.dp = L.dp;
     D.need_dp = grads && (grads->d_rays_o || grads->d_rays_d);
     D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
     return D;
@@ -1027,7 +1020,7 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
     if (d == 0) D.out[0] = occ_mid;
     if (d == 1) D.out[0] = occ_fine;
     if (d == 2) { D.out[0] = rgb; D.out[1] = rgb + P; D.out[2] = rgb + 2 * (size_t)P; D.out[3] = nullptr; }
-    if (d == 2 && train_color) D.acts = reinterpret_cast<float*>(ws + L.acts);
+    if (d == 2 && train_color) D.acts = L.acts;
     const size_t smem = dec_smem(decoders[d].c_dim);
     XRD_CUDA_TRY(cudaFuncSetAttribute(k_decoder_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     KernelTimer kt(stream);
@@ -1052,24 +1045,24 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   LP.handle_dynamic = cfg->handle_dynamic; LP.use_color_in_tracking = cfg->use_color_in_tracking;
   LP.w_color = cfg->w_color; LP.target_s = rays->target_s; LP.target_d = rays->target_d;
   LP.rgb = out->rgb; LP.depth = out->depth; LP.var = out->uncertainty;
-  LP.gd = reinterpret_cast<float*>(ws + L.gd); LP.gc = reinterpret_cast<float*>(ws + L.gc);
-  LP.tmp = reinterpret_cast<double*>(ws + L.tmp); LP.losses = out->losses;
+  LP.gd = L.gd; LP.gc = L.gc;
+  LP.tmp = L.tmp; LP.losses = out->losses;
   k_loss<<<1, 1024, 0, stream>>>(LP);
   XRD_LAUNCH_CHECK();
 
   C.gd = LP.gd; C.gc = LP.gc;
-  C.d_occ = reinterpret_cast<float*>(ws + L.d_occ);
+  C.d_occ = L.d_occ;
   if (stage == XRD_NICE_COLOR)
-    for (int c = 0; c < 3; ++c) C.d_rgb[c] = reinterpret_cast<float*>(ws + L.d_rgb) + (size_t)c * P;
+    for (int c = 0; c < 3; ++c) C.d_rgb[c] = L.d_rgb + (size_t)c * P;
   k_composite<true><<<(R + 3) / 4, 128, 0, stream>>>(C);
   XRD_LAUNCH_CHECK();
 
-  XRD_CUDA_TRY(cudaMemsetAsync(ws + L.dp, 0, 3 * (size_t)P * 4, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   for (int d = 0; d <= stage; ++d) {
     DecParams D = dec_params(d);
     if (d < 2) D.dout[0] = C.d_occ;
     else { D.dout[0] = C.d_rgb[0]; D.dout[1] = C.d_rgb[1]; D.dout[2] = C.d_rgb[2]; D.dout[3] = nullptr; }
-    if (d == 2 && train_color) D.acts = reinterpret_cast<float*>(ws + L.acts);
+    if (d == 2 && train_color) D.acts = L.acts;
     const size_t smem = dec_smem(decoders[d].c_dim);
     XRD_CUDA_TRY(cudaFuncSetAttribute(k_decoder_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_decoder_bwd<<<gridx, T, smem, stream>>>(D);
@@ -1078,8 +1071,8 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
 
   if (train_color) {
     const XrdNiceDecoderGrads* G = grads->d_color;
-    const float* A = reinterpret_cast<const float*>(ws + L.acts);
-    const uint32_t* mk = reinterpret_cast<const uint32_t*>(ws + L.masks) + (size_t)2 * 5 * P;
+    const float* A = L.acts;
+    const uint32_t* mk = L.masks + (size_t)2 * 5 * P;
     const int cd = 32;
     DwParams Q;
     Q.n_jobs = 0; Q.P = P; Q.Pp = Pp;
@@ -1109,8 +1102,8 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
     XRD_CUDA_TRY(launch_dw(Q, stream));
   }
   if (grads->d_rays_o || grads->d_rays_d) {
-    k_rayreduce<<<(R + 3) / 4, 128, 0, stream>>>(R, S, P, z, reinterpret_cast<const float*>(ws + L.dp),
-                                                 grads->d_rays_o, grads->d_rays_d);
+    k_rayreduce<<<(R + 3) / 4, 128, 0, stream>>>(R, S, P, z, L.dp, grads->d_rays_o,
+                                                 grads->d_rays_d);
     XRD_LAUNCH_CHECK();
   }
   return XRD_OK;
@@ -1126,9 +1119,16 @@ static __global__ void k_query_pack(int P, const float* occ_mid, const float* oc
   *reinterpret_cast<float4*>(raw + (size_t)p * 4) = o;
 }
 
+struct QueryWs : Carver {
+  QueryWs(void* base, int n_points) : Carver(base), P((size_t)n_points) {}
+  const size_t P;
+  double* z = take<double>(P);
+  float *zero_d = take<float>(3 * P), *occ_mid = take<float>(P), *occ_fine = take<float>(P);
+  float* rgb = take<float>(3 * P);
+};
+
 extern "C" size_t xrd_nice_query_workspace_bytes(int n_points) {
-  const size_t P = (size_t)n_points;
-  return align_up(P * 8, 256) + align_up(P * 12, 256) + 2 * align_up(P * 4, 256) + align_up(P * 12, 256);
+  return QueryWs(nullptr, n_points).bytes();
 }
 
 extern "C" int xrd_nice_query(const float* points, int n_points, const XrdNiceGrid grids[3],
@@ -1138,24 +1138,19 @@ extern "C" int xrd_nice_query(const float* points, int n_points, const XrdNiceGr
   if (!points || !grids || !decoders || !bound_min || !bound_max || !raw || !workspace) return XRD_E_NULL;
   if (n_points <= 0) return XRD_OK;
   if (stage < XRD_NICE_MIDDLE || stage > XRD_NICE_COLOR) return XRD_E_SHAPE;
-  if (workspace_bytes < xrd_nice_query_workspace_bytes(n_points)) return XRD_E_WORKSPACE;
+  const QueryWs L(workspace, n_points);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
   const int P = n_points;
-  char* ws = reinterpret_cast<char*>(workspace);
-  double* z = reinterpret_cast<double*>(ws); ws += align_up((size_t)P * 8, 256);
-  float* zero_d = reinterpret_cast<float*>(ws); ws += align_up((size_t)P * 12, 256);
-  float* occ_mid = reinterpret_cast<float*>(ws); ws += align_up((size_t)P * 4, 256);
-  float* occ_fine = reinterpret_cast<float*>(ws); ws += align_up((size_t)P * 4, 256);
-  float* rgb = reinterpret_cast<float*>(ws);
   // point = rays_o + rays_d * z with rays_o = the query point, rays_d = 0, z = 0 (exact)
-  XRD_CUDA_TRY(cudaMemsetAsync(z, 0, (size_t)P * 8, stream));
-  XRD_CUDA_TRY(cudaMemsetAsync(zero_d, 0, (size_t)P * 12, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.z, 0, (size_t)P * 8, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.zero_d, 0, (size_t)P * 12, stream));
   const int sms = num_sms();
   const int n_tiles = (P + T - 1) / T;
   const int gridx = n_tiles < sms ? n_tiles : sms;
   for (int d = 0; d <= stage; ++d) {
     DecParams D;
-    D.P = P; D.S = 1; D.z = z; D.rays_o = points; D.rays_d = zero_d;
+    D.P = P; D.S = 1; D.z = L.z; D.rays_o = points; D.rays_d = L.zero_d;
     for (int k = 0; k < 3; ++k) { D.bmin[k] = bound_min[k]; D.bmax[k] = bound_max[k]; }
     D.ga.data = grids[d].data; D.ga.nx = grids[d].nx; D.ga.ny = grids[d].ny; D.ga.nz = grids[d].nz;
     D.ga.grad = nullptr;
@@ -1163,9 +1158,9 @@ extern "C" int xrd_nice_query(const float* points, int n_points, const XrdNiceGr
     if (d == 1) { D.gb.data = grids[0].data; D.gb.nx = grids[0].nx; D.gb.ny = grids[0].ny; D.gb.nz = grids[0].nz; }
     D.dec = decoders[d];
     for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
-    if (d == 0) D.out[0] = occ_mid;
-    if (d == 1) D.out[0] = occ_fine;
-    if (d == 2) { D.out[0] = rgb; D.out[1] = rgb + P; D.out[2] = rgb + 2 * (size_t)P; }
+    if (d == 0) D.out[0] = L.occ_mid;
+    if (d == 1) D.out[0] = L.occ_fine;
+    if (d == 2) { D.out[0] = L.rgb; D.out[1] = L.rgb + P; D.out[2] = L.rgb + 2 * (size_t)P; }
     D.masks = nullptr; D.acts = nullptr; D.Pp = (int)align_up((size_t)P, 64); D.dp = nullptr; D.need_dp = 0;
     D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
     const size_t smem = sizeof(float) * ((size_t)woff(decoders[d].c_dim).total + (size_t)(E + CMAX) * T);
@@ -1173,14 +1168,15 @@ extern "C" int xrd_nice_query(const float* points, int n_points, const XrdNiceGr
     k_decoder_fwd<<<gridx, T, smem, stream>>>(D);
     XRD_LAUNCH_CHECK();
   }
-  k_query_pack<<<(P + 255) / 256, 256, 0, stream>>>(P, occ_mid, stage >= XRD_NICE_FINE ? occ_fine : nullptr,
-                                                    stage == XRD_NICE_COLOR ? rgb : nullptr, raw);
+  k_query_pack<<<(P + 255) / 256, 256, 0, stream>>>(P, L.occ_mid,
+                                                    stage >= XRD_NICE_FINE ? L.occ_fine : nullptr,
+                                                    stage == XRD_NICE_COLOR ? L.rgb : nullptr, raw);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
 
 extern "C" size_t xrd_nice_coarse_workspace_bytes(int n_rays, int n_samples, int with_grads) {
-  return ws_layout(n_rays, n_samples, with_grads).total;
+  return Ws(nullptr, n_rays, n_samples, with_grads).bytes();
 }
 
 // Stage 'coarse' (conv_onet.py:137-138,397-402; decoder_nice.py:389-393): 32 uniform samples up
@@ -1198,13 +1194,12 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   const int R = rays->n_rays, S = cfg->n_samples;
   if (R <= 0) return XRD_OK;
   if (S < 2 || S > 64) return XRD_E_SHAPE;
-  const WsLayout L = ws_layout(R, S, with_grads);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const Ws L(workspace, R, S, with_grads);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   const int P = R * S, Pp = (int)align_up((size_t)P, 64);
-  double* z = out->z_vals ? out->z_vals : reinterpret_cast<double*>(ws + L.z);
-  float* occ = reinterpret_cast<float*>(ws + L.occ_mid);
+  double* z = out->z_vals ? out->z_vals : L.z;
+  float* occ = L.occ_mid;
 
   SampleParams sp;
   sp.R = R; sp.ns = S; sp.nsurf = 0; sp.no_depth = 1;
@@ -1222,9 +1217,9 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   D.gb.data = nullptr; D.gb.grad = nullptr; D.gb.nx = D.gb.ny = D.gb.nz = 1;
   for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
   D.out[0] = occ;
-  D.masks = with_grads ? reinterpret_cast<uint32_t*>(ws + L.masks) : nullptr;
+  D.masks = L.masks;
   D.acts = nullptr; D.Pp = Pp;
-  D.dp = with_grads ? reinterpret_cast<float*>(ws + L.dp) : nullptr;
+  D.dp = L.dp;
   D.need_dp = with_grads && (d_rays_o || d_rays_d);
   D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
   D.dec = XrdNiceDecoder{};
@@ -1258,22 +1253,21 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   LP.R = R; LP.is_mapping = 1; LP.with_color = 0; LP.handle_dynamic = 0; LP.use_color_in_tracking = 0;
   LP.w_color = 0.f; LP.target_s = rays->target_s; LP.target_d = rays->target_d;
   LP.rgb = out->rgb; LP.depth = out->depth; LP.var = out->uncertainty;
-  LP.gd = reinterpret_cast<float*>(ws + L.gd); LP.gc = reinterpret_cast<float*>(ws + L.gc);
-  LP.tmp = reinterpret_cast<double*>(ws + L.tmp); LP.losses = out->losses;
+  LP.gd = L.gd; LP.gc = L.gc;
+  LP.tmp = L.tmp; LP.losses = out->losses;
   k_loss<<<1, 1024, 0, stream>>>(LP);
   XRD_LAUNCH_CHECK();
   C.gd = LP.gd; C.gc = LP.gc;
-  C.d_occ = reinterpret_cast<float*>(ws + L.d_occ);
+  C.d_occ = L.d_occ;
   k_composite<true><<<(R + 3) / 4, 128, 0, stream>>>(C);
   XRD_LAUNCH_CHECK();
-  XRD_CUDA_TRY(cudaMemsetAsync(ws + L.dp, 0, 3 * (size_t)P * 4, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   D.dout[0] = C.d_occ;
   XRD_CUDA_TRY(cudaFuncSetAttribute(k_coarse<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_coarse<true><<<gridx, T, smem, stream>>>(D, W);
   XRD_LAUNCH_CHECK();
   if (d_rays_o || d_rays_d) {
-    k_rayreduce<<<(R + 3) / 4, 128, 0, stream>>>(R, S, P, z, reinterpret_cast<const float*>(ws + L.dp),
-                                                 d_rays_o, d_rays_d);
+    k_rayreduce<<<(R + 3) / 4, 128, 0, stream>>>(R, S, P, z, L.dp, d_rays_o, d_rays_d);
     XRD_LAUNCH_CHECK();
   }
   return XRD_OK;

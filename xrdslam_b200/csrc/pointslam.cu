@@ -552,8 +552,14 @@ static __global__ void k_ix_sort(int table, const int* start, const int* end, in
 }  // namespace point
 }  // namespace xrd
 
+struct KnnWs : Carver {
+  KnnWs(void* base, int table_size)
+      : Carver(base), count(take<int>((size_t)table_size)), cursor(take<int>((size_t)table_size)) {}
+  int *count, *cursor;
+};
+
 extern "C" size_t xrd_pointslam_knn_build_workspace_bytes(int table_size) {
-  return 2 * align_up((size_t)table_size * sizeof(int), 256);
+  return KnnWs(nullptr, table_size).bytes();
 }
 
 extern "C" int xrd_pointslam_knn_build(const float* pos, int n_points, float cell, int table_size,
@@ -563,11 +569,10 @@ extern "C" int xrd_pointslam_knn_build(const float* pos, int n_points, float cel
   if (n_points > 0 && (!pos || !sorted_ids)) return XRD_E_NULL;
   if (table_size < 1 || table_size > (1 << 24) || (table_size & (table_size - 1)) || !(cell > 0.f))
     return XRD_E_SHAPE;
-  if (workspace_bytes < xrd_pointslam_knn_build_workspace_bytes(table_size)) return XRD_E_WORKSPACE;
+  const KnnWs L(workspace, table_size);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  int* count = reinterpret_cast<int*>(workspace);
-  int* cursor = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) +
-                                       align_up((size_t)table_size * sizeof(int), 256));
+  int *count = L.count, *cursor = L.cursor;
   const float inv = (1.0f / cell);
   XRD_CUDA_TRY(cudaMemsetAsync(count, 0, (size_t)table_size * sizeof(int), stream));
   if (n_points > 0) {
@@ -605,41 +610,37 @@ extern "C" int xrd_pointslam_knn_query(const XrdPointIndex* index, const float* 
 }
 
 namespace {
-struct PWs {
-  size_t z, D, I, nn, c, has, occ, d_occ, dc, dp, gd, tmp, masks;
+struct PWs : Carver {
+  PWs(void* base, int R, int S, int stage, int with_grads)
+      : Carver(base), R(R), P((size_t)R * S), g(with_grads != 0), col(stage == 1) {}
+  const size_t R, P, Pp_ = (P + 3) / 4 * 4, Np = 8 * Pp_;
+  const bool g, col;
+  const int Pp = (int)Pp_;
+  float *z = take<float>(P), *D = take<float>(P * KNN);
+  int *I = take<int>(P * KNN), *nn = take<int>(P);
+  float* c = take<float>(CD * P);
+  unsigned char* has = take<unsigned char>(P);
+  float* occ = take<float>(P);
+  // with_grads only
+  float *d_occ = g ? take<float>(P) : nullptr, *dc = g ? take<float>(CD * P) : nullptr;
+  float *dp = g ? take<float>(3 * P) : nullptr, *gd = g ? take<float>(R) : nullptr;
+  float* tmp = g ? take<float>(R) : nullptr;
+  uint32_t* masks = g ? take<uint32_t>(5 * P) : nullptr;
+  float* grgb = g ? take<float>(R * 3) : nullptr;
   // stage colour ([rows][Pp] / [rows][8 Pp] float arrays)
-  size_t wn, Xn, Hn, Fn, cc, X3, act, H, T, rgb3, d_raw3, g0, g1, gp, dX3, dcc, dFn, dHn, dXn, grgb;
-  size_t total;
-  int Pp;
+  float* wn = col ? take<float>(8 * Pp_) : nullptr;
+  float *Xn = rows(CNI, Np), *Hn = rows(CW, Np), *Fn = rows(CD, Np), *cc = rows(CD, Pp_);
+  float *X3 = rows(CX3, Pp_), *act = rows(5 * CW, Pp_), *H = rows(4 * CW, Pp_), *T = rows(CW, Pp_);
+  float* rgb3 = rows(3, Pp_);
+  // stage colour with_grads only
+  float *d_raw3 = grows(3, Pp_), *g0 = grows(CW, Pp_), *g1 = grows(CW, Pp_), *gp = grows(CW, Pp_);
+  float *dX3 = grows(CX3, Pp_), *dcc = grows(CD, Pp_), *dFn = grows(CD, Np), *dHn = grows(CW, Np);
+  float* dXn = grows(CNI, Np);
+
+ private:
+  float* rows(size_t n, size_t w) { return col ? take<float>(n * w) : nullptr; }
+  float* grows(size_t n, size_t w) { return col && g ? take<float>(n * w) : nullptr; }
 };
-PWs pws(int R, int S, int stage, int with_grads) {
-  PWs L{};
-  const size_t P = (size_t)R * S;
-  const size_t Pp = (P + 3) / 4 * 4, Np = 8 * Pp;
-  L.Pp = (int)Pp;
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.z = take(P * 4); L.D = take(P * KNN * 4); L.I = take(P * KNN * 4); L.nn = take(P * 4);
-  L.c = take(CD * P * 4); L.has = take(P); L.occ = take(P * 4);
-  if (with_grads) {
-    L.d_occ = take(P * 4); L.dc = take(CD * P * 4); L.dp = take(3 * P * 4);
-    L.gd = take((size_t)R * 4); L.tmp = take((size_t)R * 4); L.masks = take(5 * P * 4);
-    L.grgb = take((size_t)R * 3 * 4);
-  }
-  if (stage == 1) {
-    L.wn = take(8 * Pp * 4); L.Xn = take(CNI * Np * 4); L.Hn = take(CW * Np * 4);
-    L.Fn = take(CD * Np * 4); L.cc = take(CD * Pp * 4); L.X3 = take(CX3 * Pp * 4);
-    L.act = take(5 * CW * Pp * 4); L.H = take(4 * CW * Pp * 4); L.T = take(CW * Pp * 4);
-    L.rgb3 = take(3 * Pp * 4);
-    if (with_grads) {
-      L.d_raw3 = take(3 * Pp * 4); L.g0 = take(CW * Pp * 4); L.g1 = take(CW * Pp * 4);
-      L.gp = take(CW * Pp * 4); L.dX3 = take(CX3 * Pp * 4); L.dcc = take(CD * Pp * 4);
-      L.dFn = take(CD * Np * 4); L.dHn = take(CW * Np * 4); L.dXn = take(CNI * Np * 4);
-    }
-  }
-  L.total = q;
-  return L;
-}
 
 #define XRD_GEMM(...)                                         \
   do {                                                        \
@@ -648,11 +649,10 @@ PWs pws(int R, int S, int stage, int with_grads) {
   } while (0)
 
 // ---- stage colour: forward -----------------------------------------------------------------
-int color_forward(const ColorP& C0, const PWs& L, char* ws, int P, cudaStream_t stream) {
+int color_forward(const ColorP& C0, const PWs& L, int P, cudaStream_t stream) {
   const XrdPointColorDecoder& d = C0.dec;
   const int Pp = L.Pp, Np = 8 * Pp;
-  auto F = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
-  float *Xn = F(L.Xn), *Hn = F(L.Hn), *Fn = F(L.Fn), *cc = F(L.cc), *X3 = F(L.X3), *T = F(L.T);
+  float *Xn = L.Xn, *Hn = L.Hn, *Fn = L.Fn, *cc = L.cc, *X3 = L.X3, *T = L.T;
   // only the first P of every Pp-wide slot holds data; the neighbour GEMMs (and their weight
   // gradients) run over the padded width: pad columns must be zero
   if (Pp != P) XRD_CUDA_TRY(cudaMemsetAsync(Xn, 0, (size_t)CNI * Np * sizeof(float), stream));
@@ -663,30 +663,29 @@ int color_forward(const ColorP& C0, const PWs& L, char* ws, int P, cudaStream_t 
   k_nb_reduce<<<(P + 127) / 128, 128, 0, stream>>>(C0);
   XRD_LAUNCH_CHECK();
   // trunk: inputs  emb(40) | H0 | H1 | X3 = [emb, H2](168) | H3 ; outputs H0 H1 H2(in X3) H3 H4
-  float* Hs[5] = {F(L.H), F(L.H) + (size_t)CW * Pp, X3 + (size_t)2 * CE * Pp,
-                  F(L.H) + (size_t)2 * CW * Pp, F(L.H) + (size_t)3 * CW * Pp};
+  float* Hs[5] = {L.H, L.H + (size_t)CW * Pp, X3 + (size_t)2 * CE * Pp,
+                  L.H + (size_t)2 * CW * Pp, L.H + (size_t)3 * CW * Pp};
   const float* in[5] = {X3, Hs[0], Hs[1], X3, Hs[3]};
   const int kin[5] = {2 * CE, CW, CW, CX3, CW};
   for (int i = 0; i < 5; ++i) {
     XRD_GEMM({CW, P, CD, d.wc[i], CD, 0, cc, Pp, T, Pp, d.bc[i], ACT_NONE, nullptr, 0, nullptr, 0, 0});
     XRD_GEMM({CW, P, kin[i], d.w[i], kin[i], 0, in[i], Pp, Hs[i], Pp, d.b[i], ACT_SOFTPLUS100, T, Pp,
-              F(L.act) + (size_t)i * CW * Pp, Pp, 0});
+              L.act + (size_t)i * CW * Pp, Pp, 0});
   }
-  XRD_GEMM({3, P, CW, d.wo, CW, 0, Hs[4], Pp, F(L.rgb3), Pp, d.bo, ACT_SIGMOID, nullptr, 0, nullptr, 0, 0});
+  XRD_GEMM({3, P, CW, d.wo, CW, 0, Hs[4], Pp, L.rgb3, Pp, d.bo, ACT_SIGMOID, nullptr, 0, nullptr, 0, 0});
   return XRD_OK;
 }
 
 // ---- stage colour: backward (d_raw3 -> decoder grads, d col_feats, d p) ----------------------
-int color_backward(ColorP C, const PWs& L, char* ws, int P, const XrdPointColorDecoderGrads* G,
+int color_backward(ColorP C, const PWs& L, int P, const XrdPointColorDecoderGrads* G,
                    cudaStream_t stream) {
   const XrdPointColorDecoder& d = C.dec;
   const int Pp = L.Pp, Np = 8 * Pp;
-  auto F = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
-  float *Xn = F(L.Xn), *Hn = F(L.Hn), *cc = F(L.cc), *X3 = F(L.X3);
-  float *g0 = F(L.g0), *g1 = F(L.g1), *gp = F(L.gp), *dX3 = F(L.dX3), *dcc = F(L.dcc);
-  float *dFn = F(L.dFn), *dHn = F(L.dHn), *dXn = F(L.dXn), *d_raw3 = F(L.d_raw3);
-  float* Hs[5] = {F(L.H), F(L.H) + (size_t)CW * Pp, X3 + (size_t)2 * CE * Pp,
-                  F(L.H) + (size_t)2 * CW * Pp, F(L.H) + (size_t)3 * CW * Pp};
+  float *Xn = L.Xn, *Hn = L.Hn, *cc = L.cc, *X3 = L.X3;
+  float *g0 = L.g0, *g1 = L.g1, *gp = L.gp, *dX3 = L.dX3, *dcc = L.dcc;
+  float *dFn = L.dFn, *dHn = L.dHn, *dXn = L.dXn, *d_raw3 = L.d_raw3;
+  float* Hs[5] = {L.H, L.H + (size_t)CW * Pp, X3 + (size_t)2 * CE * Pp,
+                  L.H + (size_t)2 * CW * Pp, L.H + (size_t)3 * CW * Pp};
   const float* in[5] = {X3, Hs[0], Hs[1], X3, Hs[3]};
   const int kin[5] = {2 * CE, CW, CW, CX3, CW};
   DwParams Dw;
@@ -721,7 +720,7 @@ int color_backward(ColorP C, const PWs& L, char* ws, int P, const XrdPointColorD
     // fc_c branch: dc += wc_i^T dH_i
     XRD_GEMM({CD, P, CW, d.wc[i], CD, 1, dH[i], Pp, dcc, Pp, nullptr, ACT_NONE, nullptr, 0, nullptr, 0, i == 4 ? 0 : 1});
     const size_t n = (size_t)CW * Pp;
-    k_dsoftplus<<<592, 256, 0, stream>>>(n, dH[i], F(L.act) + (size_t)i * CW * Pp, gp);
+    k_dsoftplus<<<592, 256, 0, stream>>>(n, dH[i], L.act + (size_t)i * CW * Pp, gp);
     XRD_LAUNCH_CHECK();
     if (G) {
       dw_begin(P, Pp);
@@ -758,7 +757,7 @@ int color_backward(ColorP C, const PWs& L, char* ws, int P, const XrdPointColorD
 }  // namespace
 
 extern "C" size_t xrd_pointslam_workspace_bytes(int n_rays, int n_surface, int stage, int with_grads) {
-  return pws(n_rays, n_surface, stage, with_grads).total;
+  return PWs(nullptr, n_rays, n_surface, stage, with_grads).bytes();
 }
 
 extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* index,
@@ -794,26 +793,25 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   if (S < 2 || S > 16) return XRD_E_SHAPE;
   if (grads && !out->losses) return XRD_E_NULL;
   if (grads && !cfg->is_mapping && R > 8192) return XRD_E_SHAPE;
-  const PWs L = pws(R, S, stage, grads != nullptr);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const PWs L(workspace, R, S, stage, grads != nullptr);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   const int P = R * S;
-  float* z = out->z_vals ? out->z_vals : reinterpret_cast<float*>(ws + L.z);
+  float* z = out->z_vals ? out->z_vals : L.z;
 
   RayP Y;
   Y.R = R; Y.S = S; Y.rays_o = rays->rays_o; Y.rays_d = rays->rays_d;
   Y.target_s = rays->target_s; Y.target_d = rays->target_d; Y.t_surface = cfg->t_surface;
   Y.far = cfg->far; Y.near_s = cfg->near_end_surface; Y.far_s = cfg->far_end_surface;
   Y.near_end = cfg->near_end; Y.coef = cfg->sigmoid_coef; Y.z = z;
-  Y.occ = reinterpret_cast<float*>(ws + L.occ);
-  Y.has_nb = reinterpret_cast<unsigned char*>(ws + L.has);
+  Y.occ = L.occ;
+  Y.has_nb = L.has;
   Y.min_valid = S / 2 + 1;
   Y.o_rgb = out->rgb; Y.o_depth = out->depth; Y.o_var = out->uncertainty; Y.o_valid = out->valid_ray_mask;
   Y.is_mapping = cfg->is_mapping; Y.handle_dynamic = cfg->handle_dynamic;
   Y.gd = nullptr; Y.tmp = nullptr; Y.losses = out->losses; Y.d_occ = nullptr;
   Y.stage = stage; Y.Pp = L.Pp; Y.use_color_trk = cfg->use_color_in_tracking; Y.w_color = cfg->w_color;
-  Y.rgb3 = stage == 1 ? reinterpret_cast<float*>(ws + L.rgb3) : nullptr;
+  Y.rgb3 = L.rgb3;
   Y.grgb = nullptr; Y.d_raw3 = nullptr;
   k_sample_z<<<(R + 127) / 128, 128, 0, stream>>>(Y);
   XRD_LAUNCH_CHECK();
@@ -821,11 +819,11 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   InterpParams Q;
   Q.K.ix = *index; Q.K.q = nullptr; Q.K.rays_o = rays->rays_o; Q.K.rays_d = rays->rays_d; Q.K.z = z;
   Q.K.S = S; Q.K.radius = cfg->radius_query; Q.K.radius_div = S; Q.K.P = P;
-  Q.K.D = reinterpret_cast<float*>(ws + L.D); Q.K.I = reinterpret_cast<int*>(ws + L.I);
-  Q.K.nn = reinterpret_cast<int*>(ws + L.nn);
+  Q.K.D = L.D; Q.K.I = L.I;
+  Q.K.nn = L.nn;
   Q.feats = feats->geo_feats; Q.fmask = feats->frustum_mask; Q.rand_feat = cfg->rand_feat;
-  Q.min_nn = cfg->min_nn_num; Q.c = reinterpret_cast<float*>(ws + L.c);
-  Q.has_nb = reinterpret_cast<unsigned char*>(ws + L.has);
+  Q.min_nn = cfg->min_nn_num; Q.c = L.c;
+  Q.has_nb = L.has;
   Q.dc = nullptr; Q.d_feats = nullptr; Q.dp = nullptr; Q.need_dp = 0;
   {
     KernelTimer kt(stream);
@@ -842,12 +840,12 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   D.gb = D.ga;
   D.dec = *dec;
   for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
-  D.out[0] = reinterpret_cast<float*>(ws + L.occ);
-  D.masks = grads ? reinterpret_cast<uint32_t*>(ws + L.masks) : nullptr;
+  D.out[0] = L.occ;
+  D.masks = L.masks;
   D.acts = nullptr; D.Pp = P;
-  D.dp = grads ? reinterpret_cast<float*>(ws + L.dp) : nullptr;
+  D.dp = L.dp;
   D.need_dp = grads && (grads->d_rays_o || grads->d_rays_d);
-  D.ext_c = Q.c; D.ext_dc = grads ? reinterpret_cast<float*>(ws + L.dc) : nullptr;
+  D.ext_c = Q.c; D.ext_dc = L.dc;
   D.embed_scale = 6.283185307179586f;  // 2 * math.pi, float32
   const size_t smem = sizeof(float) * ((size_t)xrd::nice::woff(CD).total +
                                        (size_t)(xrd::nice::E + xrd::nice::CMAX) * xrd::nice::T);
@@ -861,25 +859,25 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   if (stage == 1) {
     C.K = Q.K; C.Pp = L.Pp; C.min_nn = cfg->min_nn_num; C.col_feats = feats->col_feats;
     C.rand_feat = cfg->rand_feat_color; C.dec = *cdec;
-    C.wn = reinterpret_cast<float*>(ws + L.wn); C.Xn = reinterpret_cast<float*>(ws + L.Xn);
-    C.Fn = reinterpret_cast<float*>(ws + L.Fn); C.cc = reinterpret_cast<float*>(ws + L.cc);
-    C.X3 = reinterpret_cast<float*>(ws + L.X3); C.has_nb = Q.has_nb;
-    const int st = color_forward(C, L, ws, P, stream);
+    C.wn = L.wn; C.Xn = L.Xn;
+    C.Fn = L.Fn; C.cc = L.cc;
+    C.X3 = L.X3; C.has_nb = Q.has_nb;
+    const int st = color_forward(C, L, P, stream);
     if (st != XRD_OK) return st;
   }
   k_composite_fwd<<<(R + 127) / 128, 128, 0, stream>>>(Y);
   XRD_LAUNCH_CHECK();
   if (!grads) return XRD_OK;
 
-  Y.gd = reinterpret_cast<float*>(ws + L.gd); Y.tmp = reinterpret_cast<float*>(ws + L.tmp);
-  Y.d_occ = reinterpret_cast<float*>(ws + L.d_occ);
-  Y.grgb = reinterpret_cast<float*>(ws + L.grgb);
-  Y.d_raw3 = stage == 1 ? reinterpret_cast<float*>(ws + L.d_raw3) : nullptr;
+  Y.gd = L.gd; Y.tmp = L.tmp;
+  Y.d_occ = L.d_occ;
+  Y.grgb = L.grgb;
+  Y.d_raw3 = L.d_raw3;
   point::k_loss<<<1, 1024, 0, stream>>>(Y);
   XRD_LAUNCH_CHECK();
   k_composite_bwd<<<(R + 127) / 128, 128, 0, stream>>>(Y);
   XRD_LAUNCH_CHECK();
-  XRD_CUDA_TRY(cudaMemsetAsync(ws + L.dp, 0, 3 * (size_t)P * 4, stream));
+  XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   D.dout[0] = Y.d_occ;
   XRD_CUDA_TRY(cudaFuncSetAttribute(xrd::nice::k_decoder_bwd,
                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -890,7 +888,7 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   XRD_LAUNCH_CHECK();
   if (stage == 1) {
     C.dp = D.dp; C.need_dp = D.need_dp; C.d_col_feats = grads->d_col_feats;
-    const int st = color_backward(C, L, ws, P, grads->color, stream);
+    const int st = color_backward(C, L, P, grads->color, stream);
     if (st != XRD_OK) return st;
   }
   if (D.need_dp) {

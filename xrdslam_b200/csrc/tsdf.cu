@@ -93,10 +93,6 @@ __global__ void k_alloc_heads(const unsigned long long* __restrict__ key, long l
   head[i] = i < n && key[i] != kNone && (i == 0 || key[i] != key[i - 1]);
 }
 
-__global__ void k_alloc_total(const int* rank, long long n, int32_t* n_blocks) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) n_blocks[0] = rank[n];
-}
-
 __global__ void k_alloc_emit(const unsigned long long* __restrict__ key,
                              const int* __restrict__ frame, const int* __restrict__ head,
                              const int* __restrict__ rank, long long n, int words,
@@ -263,10 +259,6 @@ __global__ void k_vcount(const uint32_t* __restrict__ flags, long long n, int* _
   if (g < n) vcnt[g] = __popc(flags[g]);
 }
 
-__global__ void k_totals(const int* vbase, const int* tbase, long long n, int32_t* counts) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) { counts[0] = vbase[n]; counts[1] = tbase[n]; }
-}
-
 __global__ void __launch_bounds__(256) k_verts(const unsigned long long* __restrict__ keys,
                                                const float* __restrict__ tsdf,
                                                const float* __restrict__ rgb,
@@ -371,31 +363,24 @@ __global__ void k_cc_compress(int* parent, int V) {
 }
 
 // ---- workspaces ---------------------------------------------------------------------------------
-struct AllocWs {
-  long long n;  // candidates
-  size_t key_in, key_out, frame_in, frame_out, head, rank, temp, temp_bytes, total;
+struct AllocWs : Carver {
+  AllocWs(void* base, int K, int H, int W, int stride)
+      : Carver(base), n((long long)K * ((H + stride - 1) / stride) * ((W + stride - 1) / stride) * 8) {}
+  const long long n;  // candidates
+  unsigned long long *key_in = take<unsigned long long>(n), *key_out = take<unsigned long long>(n);
+  int *frame_in = take<int>(n), *frame_out = take<int>(n);
+  int *head = take<int>(n + 1), *rank = take<int>(n + 1);
+  CubTemp temp = cub(
+      [&](size_t& b) {
+        return cub::DeviceRadixSort::SortPairs(nullptr, b, (const unsigned long long*)nullptr,
+                                               (unsigned long long*)nullptr, (const int*)nullptr,
+                                               (int*)nullptr, (int)n);
+      },
+      [&](size_t& b) {
+        return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr,
+                                             (int)(n + 1));
+      });
 };
-
-AllocWs alloc_ws(int K, int H, int W, int stride) {
-  AllocWs L;
-  const long long Hs = (H + stride - 1) / stride, Ws = (W + stride - 1) / stride;
-  L.n = (long long)K * Hs * Ws * 8;
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.key_in = take((size_t)L.n * 8); L.key_out = take((size_t)L.n * 8);
-  L.frame_in = take((size_t)L.n * 4); L.frame_out = take((size_t)L.n * 4);
-  L.head = take((size_t)(L.n + 1) * 4); L.rank = take((size_t)(L.n + 1) * 4);
-  size_t sort_b = 0, scan_b = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const unsigned long long*)nullptr,
-                                  (unsigned long long*)nullptr, (const int*)nullptr,
-                                  (int*)nullptr, (int)L.n);
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const int*)nullptr, (int*)nullptr,
-                                (int)(L.n + 1));
-  L.temp_bytes = sort_b > scan_b ? sort_b : scan_b;
-  L.temp = take(L.temp_bytes);
-  L.total = q;
-  return L;
-}
 
 bool alloc_shape_ok(int K, int H, int W, int stride) {
   if (K < 1 || H < 1 || W < 1 || stride < 1) return false;
@@ -409,33 +394,23 @@ bool params_ok(const XrdTsdfParams& P) {
          P.stride >= 1 && 2.f * P.sdf_trunc < P.voxel_length * (float)kRes;
 }
 
-struct McWs {
-  size_t nbr, cases, flags, vcnt, tcnt, vbase, tbase, scan, scan_bytes, total;
+struct McWs : Carver {
+  McWs(void* base, int n_blocks) : Carver(base), n_blocks(n_blocks) {}
+  const int n_blocks;
+  const long long n = (long long)n_blocks * kVox;  // voxels
+  int* nbr = take<int>((size_t)n_blocks * 7);
+  uint8_t* cases = take<uint8_t>(n);
+  uint32_t* flags = take<uint32_t>(n);
+  int *vcnt = take<int>(n + 1), *tcnt = take<int>(n + 1);
+  int *vbase = take<int>(n + 1), *tbase = take<int>(n + 1);
+  CubTemp scan = cub([&](size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, (int)(n + 1));
+  });
 };
-
-McWs mc_ws(int n_blocks) {
-  const long long n = (long long)n_blocks * kVox;
-  McWs L;
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.nbr = take((size_t)n_blocks * 7 * 4);
-  L.cases = take((size_t)n);
-  L.flags = take((size_t)n * 4);
-  L.vcnt = take((size_t)(n + 1) * 4); L.tcnt = take((size_t)(n + 1) * 4);
-  L.vbase = take((size_t)(n + 1) * 4); L.tbase = take((size_t)(n + 1) * 4);
-  L.scan_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, L.scan_bytes, (const int*)nullptr, (int*)nullptr,
-                                (int)(n + 1));
-  L.scan = take(L.scan_bytes);
-  L.total = q;
-  return L;
-}
 
 bool blocks_ok(int n_blocks) {
   return n_blocks >= 1 && (long long)n_blocks * kVox < 0x7fffffffLL;
 }
-
-unsigned grid(long long n) { return (unsigned)((n + 255) / 256); }
 
 }  // namespace tsdf
 }  // namespace xrd
@@ -445,7 +420,7 @@ using namespace xrd::tsdf;
 
 extern "C" size_t xrd_tsdf_alloc_workspace_bytes(int K, int H, int W, int stride) {
   if (!alloc_shape_ok(K, H, W, stride)) return 0;
-  return alloc_ws(K, H, W, stride).total;
+  return AllocWs(nullptr, K, H, W, stride).bytes();
 }
 
 extern "C" int xrd_tsdf_alloc_count(const float* depth, const float* c2w, int K, int H, int W,
@@ -454,30 +429,20 @@ extern "C" int xrd_tsdf_alloc_count(const float* depth, const float* c2w, int K,
   if (!depth || !c2w || !params || !n_blocks || !workspace) return XRD_E_NULL;
   const XrdTsdfParams P = *params;
   if (!params_ok(P) || !alloc_shape_ok(K, H, W, P.stride)) return XRD_E_SHAPE;
-  const AllocWs L = alloc_ws(K, H, W, P.stride);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  AllocWs L(workspace, K, H, W, P.stride);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  auto* key_in = reinterpret_cast<unsigned long long*>(ws + L.key_in);
-  auto* key_out = reinterpret_cast<unsigned long long*>(ws + L.key_out);
-  int* frame_in = reinterpret_cast<int*>(ws + L.frame_in);
-  int* frame_out = reinterpret_cast<int*>(ws + L.frame_out);
-  int* head = reinterpret_cast<int*>(ws + L.head);
-  int* rank = reinterpret_cast<int*>(ws + L.rank);
   const int Hs = (H + P.stride - 1) / P.stride, Ws = (W + P.stride - 1) / P.stride;
-  k_alloc_points<<<grid(L.n / 8), 256, 0, stream>>>(depth, c2w, K, H, W, Hs, Ws, P, key_in,
-                                                    frame_in);
+  k_alloc_points<<<blocks(L.n / 8), 256, 0, stream>>>(depth, c2w, K, H, W, Hs, Ws, P, L.key_in,
+                                                      L.frame_in);
   XRD_LAUNCH_CHECK();
-  size_t tb = L.temp_bytes;
-  XRD_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.temp, tb, key_in, key_out, frame_in,
-                                               frame_out, (int)L.n, 0, 64, stream));
-  k_alloc_heads<<<grid(L.n + 1), 256, 0, stream>>>(key_out, L.n, head);
+  XRD_CUDA_TRY(cub::DeviceRadixSort::SortPairs(L.temp.ptr, L.temp.bytes, L.key_in, L.key_out,
+                                               L.frame_in, L.frame_out, (int)L.n, 0, 64, stream));
+  k_alloc_heads<<<blocks(L.n + 1), 256, 0, stream>>>(L.key_out, L.n, L.head);
   XRD_LAUNCH_CHECK();
-  tb = L.temp_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.temp, tb, head, rank, (int)(L.n + 1), stream));
-  k_alloc_total<<<1, 32, 0, stream>>>(rank, L.n, n_blocks);
-  XRD_LAUNCH_CHECK();
-  return XRD_OK;
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.temp.ptr, L.temp.bytes, L.head, L.rank,
+                                             (int)(L.n + 1), stream));
+  return copy_totals(n_blocks, L.rank + L.n, nullptr, stream);
 }
 
 extern "C" int xrd_tsdf_alloc_emit(int K, int H, int W, const XrdTsdfParams* params,
@@ -486,17 +451,14 @@ extern "C" int xrd_tsdf_alloc_emit(int K, int H, int W, const XrdTsdfParams* par
   if (!params || !keys || !masks || !workspace) return XRD_E_NULL;
   const XrdTsdfParams P = *params;
   if (!params_ok(P) || !alloc_shape_ok(K, H, W, P.stride) || n_blocks < 1) return XRD_E_SHAPE;
-  const AllocWs L = alloc_ws(K, H, W, P.stride);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const AllocWs L(workspace, K, H, W, P.stride);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   const int words = (K + 31) / 32;
   XRD_CUDA_TRY(cudaMemsetAsync(masks, 0, (size_t)n_blocks * words * 4, stream));
-  k_alloc_emit<<<grid(L.n), 256, 0, stream>>>(
-      reinterpret_cast<const unsigned long long*>(ws + L.key_out),
-      reinterpret_cast<const int*>(ws + L.frame_out), reinterpret_cast<const int*>(ws + L.head),
-      reinterpret_cast<const int*>(ws + L.rank), L.n, words,
-      reinterpret_cast<unsigned long long*>(keys), masks);
+  k_alloc_emit<<<blocks(L.n), 256, 0, stream>>>(L.key_out, L.frame_out, L.head, L.rank, L.n,
+                                                words, reinterpret_cast<unsigned long long*>(keys),
+                                                masks);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
@@ -511,16 +473,16 @@ extern "C" int xrd_tsdf_integrate(const int64_t* keys, const uint32_t* masks, in
   if (!params_ok(P) || !blocks_ok(n_blocks) || K < 1 || H < 1 || W < 1) return XRD_E_SHAPE;
   cudaStream_t stream = (cudaStream_t)stream_;
   const long long n = (long long)n_blocks * kVox;
-  k_integrate<<<grid(n), 256, 0, stream>>>(reinterpret_cast<const unsigned long long*>(keys),
-                                           masks, (K + 31) / 32, depth, color, w2c, H, W, P,
-                                           tsdf, weight, color_acc);
+  k_integrate<<<blocks(n), 256, 0, stream>>>(reinterpret_cast<const unsigned long long*>(keys),
+                                             masks, (K + 31) / 32, depth, color, w2c, H, W, P,
+                                             tsdf, weight, color_acc);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
 
 extern "C" size_t xrd_tsdf_mc_workspace_bytes(int n_blocks) {
   if (!blocks_ok(n_blocks)) return 0;
-  return mc_ws(n_blocks).total;
+  return McWs(nullptr, n_blocks).bytes();
 }
 
 extern "C" int xrd_tsdf_mc_count(const int64_t* keys, int n_blocks, const float* tsdf,
@@ -528,34 +490,25 @@ extern "C" int xrd_tsdf_mc_count(const int64_t* keys, int n_blocks, const float*
                                  size_t workspace_bytes, void* stream_) {
   if (!keys || !tsdf || !weight || !counts || !workspace) return XRD_E_NULL;
   if (!blocks_ok(n_blocks)) return XRD_E_SHAPE;
-  const McWs L = mc_ws(n_blocks);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  McWs L(workspace, n_blocks);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  const long long n = (long long)n_blocks * kVox;
-  int* nbr = reinterpret_cast<int*>(ws + L.nbr);
-  uint8_t* cases = reinterpret_cast<uint8_t*>(ws + L.cases);
-  uint32_t* flags = reinterpret_cast<uint32_t*>(ws + L.flags);
-  int* vcnt = reinterpret_cast<int*>(ws + L.vcnt);
-  int* tcnt = reinterpret_cast<int*>(ws + L.tcnt);
-  int* vbase = reinterpret_cast<int*>(ws + L.vbase);
-  int* tbase = reinterpret_cast<int*>(ws + L.tbase);
+  const long long n = L.n;
   const auto* k = reinterpret_cast<const unsigned long long*>(keys);
-  k_neighbours<<<grid((long long)n_blocks * 7), 256, 0, stream>>>(k, n_blocks, nbr);
+  k_neighbours<<<blocks((long long)n_blocks * 7), 256, 0, stream>>>(k, n_blocks, L.nbr);
   XRD_LAUNCH_CHECK();
-  k_classify<<<grid(n + 1), 256, 0, stream>>>(tsdf, weight, nbr, n, cases, flags, vcnt, tcnt);
+  k_classify<<<blocks(n + 1), 256, 0, stream>>>(tsdf, weight, L.nbr, n, L.cases, L.flags, L.vcnt,
+                                                L.tcnt);
   XRD_LAUNCH_CHECK();
-  k_mark<<<grid(n), 256, 0, stream>>>(nbr, n, cases, tcnt, flags);
+  k_mark<<<blocks(n), 256, 0, stream>>>(L.nbr, n, L.cases, L.tcnt, L.flags);
   XRD_LAUNCH_CHECK();
-  k_vcount<<<grid(n), 256, 0, stream>>>(flags, n, vcnt);
+  k_vcount<<<blocks(n), 256, 0, stream>>>(L.flags, n, L.vcnt);
   XRD_LAUNCH_CHECK();
-  size_t sb = L.scan_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.scan, sb, vcnt, vbase, (int)(n + 1), stream));
-  sb = L.scan_bytes;
-  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(ws + L.scan, sb, tcnt, tbase, (int)(n + 1), stream));
-  k_totals<<<1, 32, 0, stream>>>(vbase, tbase, n, counts);
-  XRD_LAUNCH_CHECK();
-  return XRD_OK;
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.scan.ptr, L.scan.bytes, L.vcnt, L.vbase,
+                                             (int)(n + 1), stream));
+  XRD_CUDA_TRY(cub::DeviceScan::ExclusiveSum(L.scan.ptr, L.scan.bytes, L.tcnt, L.tbase,
+                                             (int)(n + 1), stream));
+  return copy_totals(counts, L.vbase + n, L.tbase + n, stream);
 }
 
 extern "C" int xrd_tsdf_mc_emit(const int64_t* keys, int n_blocks, const float* tsdf,
@@ -564,25 +517,19 @@ extern "C" int xrd_tsdf_mc_emit(const int64_t* keys, int n_blocks, const float* 
                                 size_t workspace_bytes, void* stream_) {
   if (!keys || !tsdf || !color_acc || !params || !workspace) return XRD_E_NULL;
   if (!blocks_ok(n_blocks) || !params_ok(*params)) return XRD_E_SHAPE;
-  const McWs L = mc_ws(n_blocks);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const McWs L(workspace, n_blocks);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
-  const long long n = (long long)n_blocks * kVox;
-  const int* nbr = reinterpret_cast<const int*>(ws + L.nbr);
-  const uint8_t* cases = reinterpret_cast<const uint8_t*>(ws + L.cases);
-  const uint32_t* flags = reinterpret_cast<const uint32_t*>(ws + L.flags);
-  const int* tcnt = reinterpret_cast<const int*>(ws + L.tcnt);
-  const int* vbase = reinterpret_cast<const int*>(ws + L.vbase);
-  const int* tbase = reinterpret_cast<const int*>(ws + L.tbase);
+  const long long n = L.n;
   if (verts && colors) {
-    k_verts<<<grid(n), 256, 0, stream>>>(reinterpret_cast<const unsigned long long*>(keys), tsdf,
-                                         color_acc, nbr, n, params->voxel_length, flags, vbase,
-                                         verts, colors);
+    k_verts<<<blocks(n), 256, 0, stream>>>(reinterpret_cast<const unsigned long long*>(keys), tsdf,
+                                           color_acc, L.nbr, n, params->voxel_length, L.flags,
+                                           L.vbase, verts, colors);
     XRD_LAUNCH_CHECK();
   }
   if (faces) {
-    k_faces<<<grid(n), 256, 0, stream>>>(nbr, n, cases, tcnt, flags, vbase, tbase, faces);
+    k_faces<<<blocks(n), 256, 0, stream>>>(L.nbr, n, L.cases, L.tcnt, L.flags, L.vbase, L.tbase,
+                                           faces);
     XRD_LAUNCH_CHECK();
   }
   return XRD_OK;
@@ -594,14 +541,14 @@ extern "C" int xrd_tsdf_components(const int32_t* faces, int n_faces, int n_vert
   if (n_faces < 0 || n_verts < 0) return XRD_E_SHAPE;
   if (n_verts == 0) return XRD_OK;
   cudaStream_t stream = (cudaStream_t)stream_;
-  k_cc_init<<<grid(n_verts), 256, 0, stream>>>(labels, n_verts);
+  k_cc_init<<<blocks(n_verts), 256, 0, stream>>>(labels, n_verts);
   XRD_LAUNCH_CHECK();
   if (n_faces > 0) {
     const long long ne = (long long)n_faces * 3;
-    k_cc_hook<<<grid(ne), 256, 0, stream>>>(faces, ne, labels);
+    k_cc_hook<<<blocks(ne), 256, 0, stream>>>(faces, ne, labels);
     XRD_LAUNCH_CHECK();
   }
-  k_cc_compress<<<grid(n_verts), 256, 0, stream>>>(labels, n_verts);
+  k_cc_compress<<<blocks(n_verts), 256, 0, stream>>>(labels, n_verts);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }

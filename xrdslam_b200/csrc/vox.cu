@@ -759,27 +759,18 @@ extern "C" int xrd_voxfusion_march(const XrdRays* rays, const XrdVoxMap* map,
 }
 
 namespace {
-struct VWs {
-  size_t hdr, pt_ray, pt_k, sdf, rgb, d_sdf, d_rgb, dp, acts, grads, total;
+struct VWs : Carver {
+  VWs(void* base, int Pn, int with_grads)
+      : Carver(base), P((size_t)(Pn > 0 ? Pn : 1)), g(with_grads != 0) {}
+  const size_t P, Pp = align_up(P, 64);
+  const bool g;
+  char* hdr = take<char>(256);  // counts int[4] at +0 and loss_acc double[4] at +64, one memset
+  int *pt_ray = take<int>(P), *pt_k = take<int>(P);
+  float *sdf = take<float>(P), *rgb = take<float>(3 * P);
+  float* acts = take<float>((size_t)ra_rows() * Pp);  // the GEMM decoder path keeps activations in HBM
+  float *d_sdf = g ? take<float>(P) : nullptr, *d_rgb = g ? take<float>(3 * P) : nullptr;
+  float *dp = g ? take<float>(3 * P) : nullptr, *grads = g ? take<float>((size_t)rg_rows() * Pp) : nullptr;
 };
-VWs vws(int R, int Pn, int with_grads) {
-  VWs L;
-  const size_t P = (size_t)(Pn > 0 ? Pn : 1), Pp = align_up(P, 64);
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.hdr = take(256);
-  L.pt_ray = take(P * 4); L.pt_k = take(P * 4);
-  L.sdf = take(P * 4); L.rgb = take(3 * P * 4);
-  L.d_sdf = L.d_rgb = L.dp = L.grads = 0;
-  L.acts = take((size_t)ra_rows() * Pp * 4);  // the GEMM decoder path keeps activations in HBM
-  if (with_grads) {
-    L.d_sdf = take(P * 4); L.d_rgb = take(3 * P * 4); L.dp = take(3 * P * 4);
-    L.grads = take((size_t)rg_rows() * Pp * 4);
-  }
-  (void)R;
-  L.total = q;
-  return L;
-}
 
 // Decoder.get_values (decoder_voxfusion.py:122-149) as GEMMs over [feature][point] rows of
 // `acts` (x already gathered into rows ra_x).  rgb == nullptr: the sdf head only.
@@ -806,22 +797,16 @@ int decoder_forward(const XrdVoxDecoder* dec, float* acts, int Pp, int Pn, float
 }
 
 // query workspace: activation rows + colour rows [3][P]
-struct QWs {
-  size_t acts, rgb, total;
+struct QWs : Carver {
+  QWs(void* base, int Pn) : Carver(base), P((size_t)(Pn > 0 ? Pn : 1)) {}
+  const size_t P;
+  float *acts = take<float>((size_t)ra_rows() * align_up(P, 64)), *rgb = take<float>(3 * P);
 };
-QWs qws(int Pn) {
-  QWs L;
-  const size_t P = (size_t)(Pn > 0 ? Pn : 1), Pp = align_up(P, 64);
-  size_t q = 0;
-  auto take = [&](size_t b) { size_t o = q; q += align_up(b, 256); return o; };
-  L.acts = take((size_t)ra_rows() * Pp * 4);
-  L.rgb = take(3 * P * 4);
-  L.total = q;
-  return L;
-}
 }  // namespace
 
-extern "C" size_t xrd_voxfusion_query_workspace_bytes(int n_points) { return qws(n_points).total; }
+extern "C" size_t xrd_voxfusion_query_workspace_bytes(int n_points) {
+  return QWs(nullptr, n_points).bytes();
+}
 
 extern "C" int xrd_voxfusion_query(const XrdVoxMap* map, const XrdVoxDecoder* dec, float voxel_size,
                                    int n, const int32_t* vox, int res, const float* lin,
@@ -839,19 +824,18 @@ extern "C" int xrd_voxfusion_query(const XrdVoxMap* map, const XrdVoxDecoder* de
   }
   const int Pn = res > 0 ? n * res * res * res : n;
   if (Pn == 0) return XRD_OK;
-  const QWs L = qws(Pn);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const QWs L(workspace, Pn);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   QueryParams Q;
   Q.P = Pn; Q.Pp = (int)align_up((size_t)Pn, 64); Q.res = res;
   Q.vox = vox; Q.lin = lin; Q.xyz = xyz;
   Q.centres = map->centres; Q.vertex_idx = map->vertex_idx; Q.emb = map->embeddings;
   Q.voxel_size = voxel_size;
-  Q.acts = reinterpret_cast<float*>(ws + L.acts);
+  Q.acts = L.acts;
   k_vox_query_gather<<<(Pn + T - 1) / T, T, 0, stream>>>(Q);
   XRD_LAUNCH_CHECK();
-  float* rgb_rows = rgb ? reinterpret_cast<float*>(ws + L.rgb) : nullptr;
+  float* rgb_rows = rgb ? L.rgb : nullptr;
   const int st = decoder_forward(dec, Q.acts, Q.Pp, Pn, sdf, rgb_rows, stream);
   if (st != XRD_OK) return st;
   if (rgb) {
@@ -862,7 +846,8 @@ extern "C" int xrd_voxfusion_query(const XrdVoxMap* map, const XrdVoxDecoder* de
 }
 
 extern "C" size_t xrd_voxfusion_render_workspace_bytes(int n_rays, int n_points, int with_grads) {
-  return vws(n_rays, n_points, with_grads).total;
+  (void)n_rays;
+  return VWs(nullptr, n_points, with_grads).bytes();
 }
 
 extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
@@ -877,26 +862,24 @@ extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
   const int R = rays->n_rays, Pn = cfg->n_points;
   if (R <= 0) return XRD_OK;
   if (cfg->n_hit_rays <= 0 || Pn <= 0) return XRD_E_NOHIT;  // reference: render_rays -> None
-  const VWs L = vws(R, Pn, grads != nullptr);
-  if (workspace_bytes < L.total) return XRD_E_WORKSPACE;
+  const VWs L(workspace, Pn, grads != nullptr);
+  if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  char* ws = reinterpret_cast<char*>(workspace);
   const int Pp = (int)align_up((size_t)Pn, 64);
-  int* counts = reinterpret_cast<int*>(ws + L.hdr);
-  double* loss_acc = reinterpret_cast<double*>(ws + L.hdr + 64);
-  int* pt_ray = reinterpret_cast<int*>(ws + L.pt_ray);
-  int* pt_k = reinterpret_cast<int*>(ws + L.pt_k);
-  XRD_CUDA_TRY(cudaMemsetAsync(ws + L.hdr, 0, 256, stream));
-  k_points<<<(R + 127) / 128, 128, 0, stream>>>(R, march->smp_count, march->smp_base, pt_ray, pt_k);
+  int* counts = reinterpret_cast<int*>(L.hdr);
+  double* loss_acc = reinterpret_cast<double*>(L.hdr + 64);
+  XRD_CUDA_TRY(cudaMemsetAsync(L.hdr, 0, 256, stream));
+  k_points<<<(R + 127) / 128, 128, 0, stream>>>(R, march->smp_count, march->smp_base, L.pt_ray,
+                                                L.pt_k);
   XRD_LAUNCH_CHECK();
   PointParams Q;
-  Q.P = Pn; Q.Pp = Pp; Q.R = R; Q.pt_ray = pt_ray; Q.pt_k = pt_k;
+  Q.P = Pn; Q.Pp = Pp; Q.R = R; Q.pt_ray = L.pt_ray; Q.pt_k = L.pt_k;
   Q.rays_o = rays->rays_o; Q.rays_d = rays->rays_d;
   Q.smp_depth = march->smp_depth; Q.smp_idx = march->smp_idx; Q.scap = mcfg->max_samples;
   Q.centres = map->centres; Q.vertex_idx = map->vertex_idx; Q.emb = map->embeddings;
   Q.voxel_size = cfg->voxel_size; Q.dec = *dec;
-  Q.acts = reinterpret_cast<float*>(ws + L.acts);
-  Q.sdf = reinterpret_cast<float*>(ws + L.sdf); Q.rgb = reinterpret_cast<float*>(ws + L.rgb);
+  Q.acts = L.acts;
+  Q.sdf = L.sdf; Q.rgb = L.rgb;
   Q.d_sdf = nullptr; Q.d_rgb = nullptr; Q.grads = nullptr; Q.d_emb = nullptr; Q.dp = nullptr;
   Q.need_dp = 0;
   // decoder (decoder_voxfusion.py:122-149) as GEMMs over [feature][point] rows
@@ -921,8 +904,8 @@ extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
   if (grads) {
     k_counts<<<(R + 127) / 128, 128, 0, stream>>>(Y);
     XRD_LAUNCH_CHECK();
-    Y.d_sdf = reinterpret_cast<float*>(ws + L.d_sdf);
-    Y.d_rgb = reinterpret_cast<float*>(ws + L.d_rgb);
+    Y.d_sdf = L.d_sdf;
+    Y.d_rgb = L.d_rgb;
     Y.bwd = 1;
   }
   k_composite<<<(R + 3) / 4, 128, 0, stream>>>(Y);
@@ -933,9 +916,9 @@ extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
   XRD_LAUNCH_CHECK();
 
   Q.d_sdf = Y.d_sdf; Q.d_rgb = Y.d_rgb;
-  Q.grads = reinterpret_cast<float*>(ws + L.grads);
+  Q.grads = L.grads;
   Q.d_emb = grads->d_embeddings;
-  Q.dp = reinterpret_cast<float*>(ws + L.dp);
+  Q.dp = L.dp;
   Q.need_dp = (grads->d_rays_o || grads->d_rays_d) ? 1 : 0;
   auto gr_ = [&](int row) { return Q.grads + (size_t)row * Pp; };
   k_vox_dout<<<(Pn + 255) / 256, 256, 0, stream>>>(Q);
