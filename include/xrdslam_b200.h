@@ -875,6 +875,79 @@ int xrd_eval_icp_stats(const float* src, const float* tgt, const int32_t* ids, c
                        int n, double* out, void* workspace, size_t workspace_bytes, void* stream);
 int xrd_eval_transform(const float* points, int n, const double* T, float* out, void* stream);
 
+/* ---- Depth L1 (ds-eval calc_2d_metric) -----------------------------------------
+ *
+ *   xrd_eval_render_depth  eval_recon.py:234-265: open3d Visualizer depth captures of a mesh
+ *                          (mesh_show_back_face, constant z_far 20, capture_depth_float_buffer)
+ *   xrd_eval_points_seen   eval_recon.py:66-90 check_proj, for many candidate views at once
+ *   xrd_eval_depth_l1      eval_recon.py:267-274: per view |gt - rec| over rec > 0
+ *
+ * Depth rasteriser.  verts DEVICE f32 [V][3], faces DEVICE i32 [F][3], w2c DEVICE f64
+ * [n_views][3][4] (rows 0..2 of world-to-camera, OpenCV: +z forward, +y down),
+ * 1 <= n_views <= XRD_EVAL_RENDER_MAX_VIEWS, F * n_views < 2^31.  depth DEVICE f32
+ * [n_views][H][W] is written whole: the nearest fragment's z, 0 where nothing is drawn.
+ * Per view and face (no culling; open3d's behaviour restated from memory, unverified):
+ *   1. camera space in f64: p = ((r0 x + r1 y) + r2 z) + t per row, x y z the fp32 vertex.
+ *   2. a face whose three z are all < z_near draws nothing.  Otherwise the triangle is clipped
+ *      (Sutherland-Hodgman, vertex order kept) against z >= z_near, then against the guard band
+ *      |fx x| <= G z and |fy y| <= G z, G = XRD_EVAL_RENDER_GUARD pixels, in that order.  A
+ *      crossing on segment (a, b) is computed from its lexicographically (x, y, z) smaller end:
+ *      t = d_a / (d_a - d_b), p = a + t (b - a), so faces sharing an edge share the point even
+ *      when their vertices are duplicates.  The polygon is fanned as (0, k, k + 1).
+ *   3. each vertex projects to u = (fx x) / z + cx, v = (fy y) / z + cy (f64) and snaps to
+ *      X = rint(256 u), Y = rint(256 v) (int64, 1/XRD_EVAL_RENDER_SUBPIXEL pixel).  Pixel (i, j)
+ *      samples (256 i, 256 j), i.e. u = i, v = j (GL's pixel centre when cx = W / 2 - 0.5).
+ *      A triangle with zero snapped area draws nothing; otherwise pixel (i, j) is covered when
+ *      its three int64 edge functions are all >= 0 (area > 0) or all <= 0 (area < 0), so a
+ *      pixel on a shared edge is drawn by both faces and a closed surface has no cracks.
+ *   4. depth is perspective-correct from the unclipped face's plane: n = (p1 - p0) x (p2 - p0),
+ *      k = (n_x p0_x + n_y p0_y) + n_z p0_z (f64), ax = n_x / fx, ay = n_y / fy,
+ *      c0 = n_z - (ax cx + ay cy), z = fp32(k / ((ax i + ay j) + c0)).  k = 0 draws nothing; a
+ *      fragment is kept when 0 < z <= fp32(z_far) and z is finite.  The image keeps the
+ *      smallest z (an integer max on the complemented bits), so it does not depend on the order
+ *      of faces or on the launch split.
+ * Faces whose pixel box has more than XRD_EVAL_RENDER_INLINE_PX pixels, or that need clipping,
+ * are queued in the workspace and drawn by one warp each; the result is the same either way.
+ * status DEVICE i32 [1] becomes XRD_E_SHAPE when a face index lies outside [0, V) (depth is
+ * then undefined), 0 otherwise.  H, W <= XRD_EVAL_RENDER_MAX_SIDE, fx, fy > 0,
+ * 0 < z_near < z_far, |cx|, |cy| <= 2 XRD_EVAL_RENDER_MAX_SIDE, else XRD_E_SHAPE at once.
+ * Workspace >= xrd_eval_render_workspace_bytes(F, n_views) (4 bytes per (face, view) + 256).
+ * xrd_debug_eval_render_queued: *count (DEVICE u32) = the faces the last render with this
+ * workspace queued, summed over its views.
+ *
+ * Unseen check.  xrd_eval_points_seen: points DEVICE f32 [N][3], w2c DEVICE f32 [K][3][4] =
+ * fp32(inv(c2w with columns 1 and 2 negated)) as check_proj builds it; seen DEVICE u8 [K].
+ * In fp32, per point and view: c = ((w0 x + w1 y) + w2 z) + w3 per row; x' = -c_x;
+ * u' = fx x' + cx c_z, v' = fy c_y + cy c_z; z' = c_z + fp32(1e-5); u = u' / z', v = v' / z';
+ * seen[k] = 1 when some point has 0 <= -z', 0 < u < W and 0 < v < H (fx..cy, W, H as fp32).
+ * The reference multiplies with torch matmuls whose summation order is unspecified.
+ *
+ * Per-view sums.  xrd_eval_depth_l1: gt, rec DEVICE f32 [n_views][n_pixels]; out DEVICE f64
+ * [n_views][2] = (sum |gt - rec|, count) over the pixels with rec > 0.  The fp32 difference is
+ * widened exactly; thread t of 256 sums pixels t, t + 256, ... in order, then a fixed tree, so
+ * the sums are bit-identical run to run.  The reference takes the mean in fp32 numpy. */
+#define XRD_EVAL_RENDER_MAX_VIEWS 32
+#define XRD_EVAL_RENDER_SUBPIXEL 256
+#define XRD_EVAL_RENDER_INLINE_PX 64
+#define XRD_EVAL_RENDER_GUARD 2097152.0
+#define XRD_EVAL_RENDER_MAX_SIDE 16384
+typedef struct {
+  int H, W;
+  double fx, fy, cx, cy;
+  double z_near, z_far;
+} XrdEvalCamera;
+
+size_t xrd_eval_render_workspace_bytes(int n_faces, int n_views);
+int xrd_eval_render_depth(const float* verts, int n_verts, const int32_t* faces, int n_faces,
+                          const double* w2c, int n_views, const XrdEvalCamera* camera,
+                          float* depth, int32_t* status, void* workspace, size_t workspace_bytes,
+                          void* stream);
+int xrd_debug_eval_render_queued(const void* workspace, unsigned* count, void* stream);
+int xrd_eval_points_seen(const float* points, int n_points, const float* w2c, int n_views,
+                         const XrdEvalCamera* camera, uint8_t* seen, void* stream);
+int xrd_eval_depth_l1(const float* gt, const float* rec, int n_views, int n_pixels, double* out,
+                      void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -197,6 +197,15 @@ class XrdNnIndex(C.Structure):
                 ('sorted', vp)]
 
 
+XRD_EVAL_RENDER_MAX_VIEWS = 32
+
+
+class XrdEvalCamera(C.Structure):
+    _fields_ = [('H', C.c_int), ('W', C.c_int), ('fx', C.c_double), ('fy', C.c_double),
+                ('cx', C.c_double), ('cy', C.c_double), ('z_near', C.c_double),
+                ('z_far', C.c_double)]
+
+
 class XrdPointIndex(C.Structure):
     _fields_ = [('pos', vp), ('n_points', C.c_int), ('cell', C.c_float),
                 ('table_size', C.c_int), ('cell_start', vp), ('cell_end', vp),
@@ -347,6 +356,13 @@ SYMBOLS = {
     'xrd_eval_dist_stats': (C.c_int, [vp, C.c_int, C.c_float, vp, vp, C.c_size_t, vp]),
     'xrd_eval_icp_stats': (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_size_t, vp]),
     'xrd_eval_transform': (C.c_int, [vp, C.c_int, C.POINTER(C.c_double), vp, vp]),
+    'xrd_eval_render_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int]),
+    'xrd_eval_render_depth': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, C.c_int,
+                                        C.POINTER(XrdEvalCamera), vp, vp, vp, C.c_size_t, vp]),
+    'xrd_debug_eval_render_queued': (C.c_int, [vp, vp, vp]),
+    'xrd_eval_points_seen': (C.c_int, [vp, C.c_int, vp, C.c_int, C.POINTER(XrdEvalCamera), vp,
+                                       vp]),
+    'xrd_eval_depth_l1': (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

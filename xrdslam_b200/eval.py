@@ -1,10 +1,11 @@
-"""ds-eval (scripts/eval.py, reference @ f0366f20): the trajectory's ATE from eval.tar and the
-3D reconstruction metrics of final_mesh_rec.ply against a ground-truth mesh.
+"""ds-eval (scripts/eval.py, reference @ f0366f20): the trajectory's ATE from eval.tar, the
+3D reconstruction metrics of final_mesh_rec.ply against a ground-truth mesh and, with
+eval_2d_metric, the 2D depth L1 (calc_2d_metric), which reads <gt>_pc_unseen.npy beside the mesh.
 
-    python -m xrdslam_b200.eval --output_dir <run dir> --gt_mesh <gt.ply>
+    python -m xrdslam_b200.eval --output_dir <run dir> --gt_mesh <gt.ply> [--eval_2d_metric true]
 
-The 2D depth-L1 metric is not available (it needs a mesh rasteriser with open3d's visualiser
-semantics and per-scene data): eval_2d_metric defaults to False and True raises."""
+eval_2d_metric defaults to False here; the reference's default is True.  A run that asks for
+it fails before any other work when the unseen point cloud is missing."""
 from __future__ import annotations
 
 import argparse
@@ -16,6 +17,11 @@ from typing import Optional
 import numpy as np
 
 from .io_formats import ate_rmse, load_eval_tar
+
+
+class MissingUnseenPointCloud(FileNotFoundError, NotImplementedError):
+    """The depth-L1 metric's <gt>_pc_unseen.npy does not exist.  A FileNotFoundError, as the
+    reference's np.load raises, and a NotImplementedError: without it the metric cannot run."""
 
 
 @dataclass
@@ -49,11 +55,14 @@ class EvalMatrics:
 
     def main(self):
         """-> the merged metric dict (also printed), or None when an input is missing."""
-        if self.eval_2d_metric:
-            raise NotImplementedError(
-                'eval_2d_metric: the 2D depth-L1 metric needs a mesh depth renderer with '
-                "open3d's visualiser semantics, trimesh's oriented_bounds and the scene's "
-                '_pc_unseen.npy; none of them is available here')
+        if self.eval_2d_metric and self.eval_recon and self.gt_mesh is not None and \
+                os.path.exists(str(self.gt_mesh)):
+            from .eval_recon import unseen_file
+            unseen = unseen_file(self.gt_mesh)
+            if not os.path.exists(unseen):
+                raise MissingUnseenPointCloud(
+                    2, f'eval_2d_metric: the depth renderer draws only views that do not see '
+                    f'the unseen region, and its point cloud {unseen} does not exist', unseen)
         eval_mesh = f'{self.output_dir}/final_mesh_rec.ply'
         transform_matrix = None
         self.traj_result = None
@@ -76,6 +85,12 @@ class EvalMatrics:
                                             transform_matrix=transform_matrix,
                                             seed=self.seed + 2, device=self.device)
         result = result_3d | result_3d_more
+        if self.eval_2d_metric:
+            from .eval_recon import calc_2d_metric
+            result_2d = calc_2d_metric(eval_mesh, str(self.gt_mesh),
+                                       transform_matrix=transform_matrix, n_imgs=1000,
+                                       seed=self.seed, device=self.device)
+            result = result_2d | result
         print(result)
         return result
 

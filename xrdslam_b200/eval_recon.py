@@ -401,3 +401,296 @@ def calc_3d_metric_New(rec_meshfile, gt_meshfile, align=True, distance_thresh=0.
                           transform_matrix=transform_matrix, icp_align=align,
                           full_path_to_gt_ply=gt_meshfile, seed=seed, uniforms=uniforms,
                           device=device)
+
+
+# ---------------------------------------------------------------- calc_2d_metric ---
+RENDER_W = RENDER_H = 500   # calc_2d_metric's camera: 500 x 500, focal 300, centre 249.5
+RENDER_FOCAL = 300.0
+Z_FAR = 20.0                # set_constant_z_far(20)
+NEAR_FRACTION = 0.01        # open3d's z_near: 0.01 x the drawn geometry's largest AABB extent
+
+
+def _norm(x):
+    x = np.asarray(x, np.float64)
+    return np.sqrt((x[..., 0] * x[..., 0] + x[..., 1] * x[..., 1]) + x[..., 2] * x[..., 2])
+
+
+def _cross(a, b):
+    return np.stack([a[..., 1] * b[..., 2] - a[..., 2] * b[..., 1],
+                     a[..., 2] * b[..., 0] - a[..., 0] * b[..., 2],
+                     a[..., 0] * b[..., 1] - a[..., 1] * b[..., 0]], -1)
+
+
+def normalize(x):
+    """eval_recon.py:16-17, over the last axis of [..., 3] with an explicit sum order, so one
+    vector and a batch of them round alike."""
+    x = np.asarray(x, np.float64)
+    return x / _norm(x)[..., None]
+
+
+def viewmatrix(z, up, pos):
+    """eval_recon.py:20-26: [..., 3, 4] camera-to-world columns (x, y, z, position) with z along
+    `z`, built from `up`."""
+    vec2 = normalize(z)
+    up = np.broadcast_to(np.asarray(up, np.float64), vec2.shape)
+    vec0 = normalize(_cross(up, vec2))
+    vec1 = normalize(_cross(vec2, vec0))
+    pos = np.broadcast_to(np.asarray(pos, np.float64), vec2.shape)
+    return np.stack([vec0, vec1, vec2, pos], -1)
+
+
+def volume_rectangular(extents, count, transform=None, rng=None):
+    """trimesh.sample.volume_rectangular (from memory, unverified): (random((count, 3)) - 0.5) *
+    extents, then transform (4x4) applied as ((T0 x + T1 y) + T2 z) + T3 per row.  `rng` is a
+    numpy RandomState (the global one when None); count rows are the same draws as count
+    one-row calls."""
+    rng = np.random if rng is None else rng
+    p = (rng.random((count, 3)) - 0.5) * np.asarray(extents, np.float64)
+    if transform is None:
+        return p
+    T = np.asarray(transform, np.float64)
+    return np.stack([((T[a, 0] * p[:, 0] + T[a, 1] * p[:, 1]) + T[a, 2] * p[:, 2]) + T[a, 3]
+                     for a in range(3)], -1)
+
+
+def _min_area_rect(p2):
+    """Smallest-area rectangle around 2D points over their hull's edge directions ->
+    (area, unit edge direction)."""
+    from scipy.spatial import ConvexHull
+    h = p2[ConvexHull(p2).vertices]
+    e = np.roll(h, -1, 0) - h
+    e = e / np.linalg.norm(e, axis=1, keepdims=True)
+    best = (np.inf, None)
+    for d in e:
+        r = h @ np.array([d, [-d[1], d[0]]]).T
+        area = np.ptp(r[:, 0]) * np.ptp(r[:, 1])
+        if area < best[0]:
+            best = (area, d)
+    return best
+
+
+def oriented_bounds(obj, angle_digits=1, ordered=True):
+    """trimesh.bounds.oriented_bounds, restated from memory (unverified): the minimum-volume box
+    over the convex hull's face normals, each with the minimum-area rectangle of the points
+    projected on the normal's plane.  obj: a mesh, vertices or a PLY path.  -> (to_origin 4x4
+    mapping the box's centre to the origin and its axes to x, y, z; extents), extents ascending
+    when `ordered`.  angle_digits is accepted for the reference's signature; normals are merged
+    to 1e-8."""
+    from scipy.spatial import ConvexHull
+    v, _ = load_mesh(obj) if not isinstance(obj, np.ndarray) else (obj, None)
+    pts = np.asarray(v.cpu().numpy() if torch.is_tensor(v) else v, np.float64).reshape(-1, 3)
+    hull = ConvexHull(pts)
+    hv = pts[hull.vertices]
+    normals = np.unique(np.round(hull.equations[:, :3], 8), axis=0)
+    best = (np.inf, None)
+    for n in normals:
+        n = n / np.linalg.norm(n)
+        a = np.cross(n, [1.0, 0.0, 0.0] if abs(n[0]) < 0.9 else [0.0, 1.0, 0.0])
+        a /= np.linalg.norm(a)
+        b = np.cross(n, a)
+        area, d = _min_area_rect(hv @ np.stack([a, b]).T)
+        vol = area * np.ptp(hv @ n)
+        if vol < best[0]:
+            u = d[0] * a + d[1] * b
+            best = (vol, np.stack([n, u, np.cross(n, u)]))
+    R = best[1]
+    proj = hv @ R.T
+    lo, hi = proj.min(0), proj.max(0)
+    extents = hi - lo
+    centre = R.T @ ((lo + hi) / 2)
+    if ordered:
+        order = np.argsort(extents, kind='stable')
+        R, extents = R[order], extents[order]
+    if np.linalg.det(R) < 0:
+        R[2] *= -1
+    to_origin = np.eye(4)
+    to_origin[:3, :3] = R
+    to_origin[:3, 3] = -R @ centre
+    return to_origin, extents
+
+
+def get_cam_position(gt_meshfile):
+    """eval_recon.py:158-166: the box camera origins are drawn from, inside the ground truth's
+    oriented bounds (extents scaled by 0.3, 0.7, 0.7, centre raised 0.4 m in world z)."""
+    to_origin, extents = oriented_bounds(gt_meshfile)
+    extents = extents.copy()
+    extents[2] *= 0.7
+    extents[1] *= 0.7
+    extents[0] *= 0.3
+    transform = np.linalg.inv(to_origin)
+    transform[2, 3] += 0.4
+    return extents, transform
+
+
+def _camera(near, H=RENDER_H, W=RENDER_W, fx=RENDER_FOCAL, fy=RENDER_FOCAL, cx=None, cy=None,
+            far=Z_FAR):
+    cx = H / 2.0 - 0.5 if cx is None else cx
+    cy = W / 2.0 - 0.5 if cy is None else cy
+    return _cabi.XrdEvalCamera(H, W, fx, fy, cx, cy, near, far)
+
+
+def points_seen(points, c2w, W=RENDER_W, H=RENDER_H, fx=RENDER_FOCAL, fy=RENDER_FOCAL, cx=None,
+                cy=None, device=None):
+    """check_proj for K views at once: DEVICE or host points [N,3], c2w [K,4,4] -> bool [K]
+    (host), True where some point projects into the view (xrd_eval_points_seen)."""
+    dev = _device(device) if not torch.is_tensor(points) or not points.is_cuda else points.device
+    p = _pts(points, dev)
+    c = np.array(c2w, np.float64, copy=True).reshape(-1, 4, 4)
+    c[:, :3, 1] *= -1.0
+    c[:, :3, 2] *= -1.0
+    w2c = torch.from_numpy(np.ascontiguousarray(np.linalg.inv(c).astype(np.float32)[:, :3, :4]))
+    w2c = w2c.to(dev)
+    seen = torch.empty(len(c), dtype=torch.uint8, device=dev)
+    cam = _camera(0.0, H, W, fx, fy, cx, cy, 1.0)
+    with torch.cuda.device(dev):
+        check('xrd_eval_points_seen', _cabi.lib().xrd_eval_points_seen(
+            ptr(p), p.shape[0], ptr(w2c), len(c), C.byref(cam), ptr(seen), _stream(dev)))
+    return seen.cpu().numpy().astype(bool)
+
+
+def check_proj(points, W, H, fx, fy, cx, cy, c2w):
+    """eval_recon.py:66-90: whether any point projects into the view c2w [4,4]."""
+    return bool(points_seen(points, np.asarray(c2w)[None], W, H, fx, fy, cx, cy)[0])
+
+
+def sample_views(pc_unseen, extents, transform, n_imgs, seed=0, batch=1024, max_candidates=None,
+                 device=None, seen_fn=None):
+    """calc_2d_metric's view sampler (eval_recon.py:212-232): origin in the camera box (numpy
+    RandomState(seed)), target = three round(uniform(-1e4, 1e4), 2) (random.Random(seed)) minus
+    the origin, up (0, 0, -1); a view that sees the unseen cloud is drawn again.  Candidates are
+    drawn and checked `batch` at a time and taken in order; the two streams are independent, so
+    the accepted views are those of the one-at-a-time loop.  -> c2w f64 [n_imgs,4,4].  Raises
+    RuntimeError after max_candidates (default 1000 n_imgs) candidates.  seen_fn(c2w [K,4,4]) ->
+    bool [K] replaces the device check (xrd_eval_points_seen on pc_unseen) when given."""
+    import random
+    pyr, npr = random.Random(seed), np.random.RandomState(seed)
+    if seen_fn is None:
+        dev = _device(device)
+        pts = _pts(pc_unseen, dev)
+        seen_fn = (lambda c: points_seen(pts, c, device=dev)) if pts.shape[0] else \
+            (lambda c: np.zeros(len(c), bool))
+    limit = 1000 * n_imgs if max_candidates is None else max_candidates
+    views, tried = [], 0
+    while len(views) < n_imgs:
+        k = min(batch, limit - tried)
+        if k <= 0:
+            raise RuntimeError(f'calc_2d_metric: {tried} candidate views all see the unseen '
+                               f'region; {len(views)} of {n_imgs} accepted')
+        origin = volume_rectangular(extents, k, transform, npr)
+        target = np.array([[round(pyr.uniform(-10000, +10000), 2) for _ in range(3)]
+                           for _ in range(k)]) - origin
+        c2w = np.tile(np.eye(4), (k, 1, 1))
+        c2w[:, :3, :] = viewmatrix(target, [0, 0, -1], origin)
+        seen = np.asarray(seen_fn(c2w), bool)
+        tried += k
+        for i in np.nonzero(~seen)[0][:n_imgs - len(views)]:
+            views.append(c2w[i])
+    return np.array(views).reshape(-1, 4, 4)
+
+
+class DepthRenderer:
+    """xrd_eval_render_depth over one mesh: DEVICE vertices / faces, near = 0.01 x the largest
+    AABB extent of the vertices (one host read), far 20; renders up to 32 views per launch."""
+
+    def __init__(self, verts, faces, device=None, H=RENDER_H, W=RENDER_W, fx=RENDER_FOCAL,
+                 fy=RENDER_FOCAL, cx=None, cy=None, near=None, far=Z_FAR):
+        dev = _device(device) if not torch.is_tensor(verts) or not verts.is_cuda else verts.device
+        self.device = dev
+        self.verts = _pts(verts, dev)
+        f = faces if torch.is_tensor(faces) else torch.from_numpy(np.asarray(faces, np.int32))
+        self.faces = f.to(dev, torch.int32).reshape(-1, 3).contiguous()
+        if near is None:
+            lo, hi = torch.aminmax(self.verts, dim=0)
+            near = NEAR_FRACTION * float((hi - lo).max())
+        self.camera = _camera(near, H, W, fx, fy, cx, cy, far)
+        self.B = _cabi.XRD_EVAL_RENDER_MAX_VIEWS
+        self.ws_bytes = _cabi.lib().xrd_eval_render_workspace_bytes(self.faces.shape[0], self.B)
+        if self.ws_bytes == 0:
+            raise ValueError('the depth renderer needs at least one face')
+        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=dev)
+
+    def render(self, w2c, out=None, status=None):
+        """w2c [n,3,4] or [n,4,4] (host f64 or DEVICE) -> DEVICE depth f32 [n,H,W].  status: a
+        DEVICE i32 [>= ceil(n / 32)] to collect the per-launch status words in (the caller
+        checks them); without it they are read at once."""
+        W = torch.as_tensor(np.asarray(w2c, np.float64) if not torch.is_tensor(w2c) else w2c)
+        W = W.to(self.device, torch.float64)[:, :3, :4].contiguous()
+        n = W.shape[0]
+        cam = self.camera
+        out = torch.empty(n, cam.H, cam.W, dtype=torch.float32, device=self.device) \
+            if out is None else out
+        own = status is None
+        if own:
+            status = torch.zeros(max(1, -(-n // self.B)), dtype=torch.int32, device=self.device)
+        lib = _cabi.lib()
+        with torch.cuda.device(self.device):
+            s = _stream(self.device)
+            for k, b0 in enumerate(range(0, n, self.B)):
+                nb = min(self.B, n - b0)
+                check('xrd_eval_render_depth', lib.xrd_eval_render_depth(
+                    ptr(self.verts), self.verts.shape[0], ptr(self.faces), self.faces.shape[0],
+                    ptr(W[b0:b0 + nb]), nb, C.byref(cam), ptr(out[b0:b0 + nb]),
+                    ptr(status[k:k + 1]), ptr(self.ws), self.ws_bytes, s))
+        if own:
+            _check_status(status)
+        return out
+
+
+def _check_status(status):
+    st = status.cpu().numpy()
+    if st.any():
+        check('xrd_eval_render_depth', int(st[st != 0][0]))
+
+
+def depth_l1_sums(gt, rec):
+    """DEVICE f64 [n,2] = (sum |gt - rec|, count) over rec > 0 per view, bit-identical run to
+    run (xrd_eval_depth_l1)."""
+    n = gt.shape[0]
+    out = torch.empty(n, 2, dtype=torch.float64, device=gt.device)
+    with torch.cuda.device(gt.device):
+        check('xrd_eval_depth_l1', _cabi.lib().xrd_eval_depth_l1(
+            ptr(gt), ptr(rec), n, gt[0].numel() if n else 0, ptr(out), _stream(gt.device)))
+    return out
+
+
+def unseen_file(gt_meshfile):
+    """The unseen point cloud calc_2d_metric reads beside the ground-truth mesh."""
+    return str(gt_meshfile).replace('.ply', '_pc_unseen.npy')
+
+
+def calc_2d_metric(rec_meshfile, gt_meshfile, transform_matrix=None, align=True, n_imgs=1000,
+                   seed=0, device=None):
+    """eval_recon.py:169-283, depth L1 in cm: align the reconstruction as calc_3d_metric does,
+    draw n_imgs views inside the ground truth's camera box that do not see
+    <gt>_pc_unseen.npy, render both meshes' depth at 500 x 500 (fx = fy = 300) and average, over
+    the views where the reconstruction draws anything, the mean |gt - rec| over its pixels.
+    -> {'depth l1': cm} (NaN when no view draws the reconstruction).  Renders run 32 views per
+    launch; the host reads the sums once.  The reference reads a quantised OpenGL depth buffer
+    and keeps whichever surface wins z-fighting; here z is exact and the nearest surface wins."""
+    dev = _device(device)
+    pc_unseen = np.load(unseen_file(gt_meshfile))
+    rv, rf = load_mesh(rec_meshfile)
+    gv, gf = load_mesh(gt_meshfile)
+    rv, gv = _pts(rv, dev), _pts(gv, dev)
+    rv, _ = _aligned_vertices(rv, gv, transform_matrix, align, 30)
+    extents, transform = get_cam_position(gv.cpu().numpy())
+    c2w = sample_views(pc_unseen, extents, transform, n_imgs, seed, device=dev)
+    if n_imgs == 0:
+        return {'depth l1': float('nan')}
+    w2c = np.linalg.inv(c2w)
+    gt_r, rec_r = DepthRenderer(gv, gf, dev), DepthRenderer(rv, rf, dev)
+    B = gt_r.B
+    nbatch = -(-n_imgs // B)
+    sums = torch.empty(n_imgs, 2, dtype=torch.float64, device=dev)
+    status = torch.zeros(2 * nbatch, dtype=torch.int32, device=dev)
+    for k in range(nbatch):
+        sl = slice(k * B, min(n_imgs, (k + 1) * B))
+        gd = gt_r.render(w2c[sl], status=status[2 * k:2 * k + 1])
+        rd = rec_r.render(w2c[sl], status=status[2 * k + 1:2 * k + 2])
+        sums[sl] = depth_l1_sums(gd, rd)
+    _check_status(status)
+    s = sums.cpu().numpy()
+    ok = s[:, 1] > 0
+    if not ok.any():
+        return {'depth l1': float('nan')}
+    return {'depth l1': float((s[ok, 0] / s[ok, 1]).mean() * 100)}
