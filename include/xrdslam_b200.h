@@ -948,6 +948,68 @@ int xrd_eval_points_seen(const float* points, int n_points, const float* w2c, in
 int xrd_eval_depth_l1(const float* gt, const float* rec, int n_views, int n_pixels, double* out,
                       void* stream);
 
+/* ---- Render-quality metrics of re-rendered frames ------------------------------
+ *
+ *   xrd_eval_image_metrics  slam/common/common.py:429-479 save_render_imgs: clip, the colour
+ *                           mask when no depth is rendered, F.mse_loss / PSNR, the masked
+ *                           rendered-depth L1 and pytorch_msssim.ms_ssim(data_range=1,
+ *                           size_average=True), for B frames per call; called once per
+ *                           re-rendered frame by slam/pipeline/tracker.py:343-409
+ *                           save_re_render_frames.  LPIPS is not computed here.
+ *
+ * gt_color, color DEVICE f32 [B][H][W][3]; gt_depth DEVICE f32 [B][H][W]; depth DEVICE f64
+ * [B][H][W] (render_img's depth is float64).  flags: XRD_EVAL_IMAGE_NO_DEPTH = no rendered
+ * depth (depth is ignored and may be NULL).  out DEVICE f64 [B][XRD_EVAL_IMAGE_OUT] = (psnr,
+ * ms_ssim, depth_l1, mse); levels DEVICE f64 [B][5][3][2] = (mean ssim, mean cs) per level and
+ * channel, or NULL.  Per frame, in this order:
+ *   1. colour: both images are clipped to [0, 1] (fminf(fmaxf(v, 0), 1)).  With NO_DEPTH both
+ *      are then multiplied by (gt_depth > 0) (common.py:447-450); otherwise they are not masked.
+ *   2. mse: the fp32 squared difference (a - r)^2 of every element, widened to f64 and summed;
+ *      mse = sum / (3 H W); psnr = -10 log10(mse) (+inf when mse = 0).
+ *   3. depth_l1 = 100 (sum |(f64) gt - r| / count) over the pixels with gt > 0, all f64; NaN
+ *      when there is none.  0 with NO_DEPTH (common.py:460).
+ *   4. ms_ssim, five levels l = 0..4 of an image pyramid, per channel, all in fp32 with every
+ *      operation rounded in the order written (no contraction):
+ *      - window w[11]: d = k - 5, g_k = fp32(exp(fp32(-(d d) / 4.5))), s = g_0 + ... + g_10 summed
+ *        in order, w_k = g_k / s.
+ *      - filter: valid (unpadded) 11-tap correlation along x (columns) first, then along y (rows),
+ *        each as ((w_0 v_0 + w_1 v_1) + ...) + w_10 v_10, of the five maps x, y, x x, y y, x y
+ *        (x = gt, y = render; the products are formed before filtering).  A level of H_l x W_l
+ *        gives (H_l - 10) x (W_l - 10) outputs.
+ *      - from mu1, mu2 and the filtered squares: s1 = E[x x] - mu1 mu1, s2 = E[y y] - mu2 mu2,
+ *        s12 = E[x y] - mu1 mu2, cs = (2 s12 + C2) / ((s1 + s2) + C2),
+ *        ssim = ((2 mu1 mu2 + C1) / ((mu1 mu1 + mu2 mu2) + C1)) cs, C1 = fp32(0.01^2),
+ *        C2 = fp32(0.03^2).  Their means over the valid outputs are f64: each 32 x 16 output
+ *        tile is summed by 256 threads (thread t = 32 r + q takes rows r and r + 8 of column q,
+ *        in that order), then a fixed tree over the threads; the tile sums of a level are summed
+ *        thread t taking tiles t, t + 256, ... in order, then the same tree; mean = sum / count.
+ *      - pooling to the next level: avg_pool2d(kernel 2, stride 2, padding s % 2 per axis,
+ *        count_include_pad): H_{l+1} = (H_l + 1) / 2, output (i, j) = (((v00 + v01) + v10) + v11)
+ *        * 0.25 over input rows 2i - H_l % 2 + {0, 1} and columns 2j - W_l % 2 + {0, 1}, zeros
+ *        outside.
+ *      - ms_ssim = mean over the 3 channels of prod_l p_l (left to right), p_l = pow(relu(cs_l),
+ *        w_l) for l < 4 and pow(relu(ssim_4), w_4), weights fp32(0.0448, 0.2856, 0.3001,
+ *        0.2363, 0.1333) widened to f64; the channel mean is ((c0 + c1) + c2) / 3, all f64.
+ *      The reference passes the image transposed, [1, 3, W, H]; its filter runs along W first
+ *      too, and the window and pooling are symmetric in the axes, so the transposition only
+ *      changes the order in which the 2x2 pooling windows and the means are summed.
+ * The frame sums of steps 2 and 3 are fixed-order: 256 threads per chunk of 4096 pixels, thread
+ * t summing pixels t, t + 256, ... (channels 0, 1, 2 of each) in order, a fixed tree, then the
+ * chunk sums as the tile sums above.  Everything is bit-identical run to run.
+ * min(H, W) >= XRD_EVAL_IMAGE_MIN_SIDE (pytorch_msssim asserts min(H, W) > (11 - 1) 2^4),
+ * max(H, W) <= XRD_EVAL_IMAGE_MAX_SIDE, 1 <= B <= 65535 and no unknown flag, else XRD_E_SHAPE;
+ * a required pointer NULL: XRD_E_NULL; workspace < xrd_eval_image_workspace_bytes(B, H, W):
+ * XRD_E_WORKSPACE. */
+#define XRD_EVAL_IMAGE_LEVELS 5
+#define XRD_EVAL_IMAGE_MIN_SIDE 161
+#define XRD_EVAL_IMAGE_MAX_SIDE 16384
+#define XRD_EVAL_IMAGE_NO_DEPTH 1
+#define XRD_EVAL_IMAGE_OUT 4
+size_t xrd_eval_image_workspace_bytes(int B, int H, int W);
+int xrd_eval_image_metrics(const float* gt_color, const float* color, const float* gt_depth,
+                           const double* depth, int B, int H, int W, int flags, double* out,
+                           double* levels, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -198,6 +198,8 @@ class XrdNnIndex(C.Structure):
 
 
 XRD_EVAL_RENDER_MAX_VIEWS = 32
+XRD_EVAL_IMAGE_LEVELS, XRD_EVAL_IMAGE_MIN_SIDE, XRD_EVAL_IMAGE_MAX_SIDE = 5, 161, 16384
+XRD_EVAL_IMAGE_NO_DEPTH, XRD_EVAL_IMAGE_OUT = 1, 4
 
 
 class XrdEvalCamera(C.Structure):
@@ -363,6 +365,9 @@ SYMBOLS = {
     'xrd_eval_points_seen': (C.c_int, [vp, C.c_int, vp, C.c_int, C.POINTER(XrdEvalCamera), vp,
                                        vp]),
     'xrd_eval_depth_l1': (C.c_int, [vp, vp, C.c_int, C.c_int, vp, vp]),
+    'xrd_eval_image_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    'xrd_eval_image_metrics': (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
+                                         vp, vp, C.c_size_t, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

@@ -67,7 +67,7 @@ class Algorithm():
     def post_processing(self, step, is_mapping, optimizer=None, coarse=False):
         pass
 
-    def render_img(self, c2w, gt_depth=None, idx=None):
+    def render_img(self, c2w, gt_depth=None, idx=None, to_host=True):
         return None, None
 
     def optimizer_config_update(self, max_iters, coarse=False):
@@ -100,8 +100,10 @@ class Algorithm():
                              [self._frame_tensor(f, 'rgb') for f in frames], poses, n, Hedge,
                              Wedge, return_index=return_index)
 
-    def _render_full(self, c2w, gt_depth, extra=None, per_pixel=None):
-        """render_img body shared by the algorithms: all H*W rays in ray_batch_size chunks."""
+    def _render_full(self, c2w, gt_depth, extra=None, per_pixel=None, to_host=True):
+        """render_img body shared by the algorithms: all H*W rays in ray_batch_size chunks.
+        -> colour f32 [H,W,3] and depth f64 [H,W]: host numpy arrays, or the DEVICE tensors
+        when not to_host."""
         import numpy as np
         from .common import get_rays
         dev = self.device
@@ -122,8 +124,10 @@ class Algorithm():
             depths.append(out['depth'].double())
             colors.append(out['rgb'])
         H, W = self.camera.height, self.camera.width
-        return (torch.cat(colors, 0).reshape(H, W, 3).cpu().numpy(),
-                torch.cat(depths, 0).reshape(H, W).cpu().numpy())
+        color, depth = torch.cat(colors, 0).reshape(H, W, 3), torch.cat(depths, 0).reshape(H, W)
+        if not to_host:
+            return color, depth
+        return color.cpu().numpy(), depth.cpu().numpy()
 
     # ---- bookkeeping ------------------------------------------------------
     def add_framepose(self, c2w, gt_c2w, gt_c2w_ori):
@@ -177,6 +181,60 @@ class Algorithm():
         culled = cull_mesh(dataset, mesh, estimate_c2w_list=self.get_estimate_c2w_list(),
                            eval_rec=True, device=self.device)
         return path, culled.export(os.path.join(out_dir, 'final_mesh_rec.ply'))
+
+    def eval_re_render(self, dataset, render_freq=50, estimate_c2w_list=None, lpips_fn=None):
+        """The render metrics of save_re_render_frames (tracker.py:343-409): frames i of
+        `dataset` (dataset[i] -> (idx, rgb, depth, c2w)) with i % render_freq == 0 are rendered
+        from estimate_c2w_list[idx] (default: this run's estimates) with render_img(c2w,
+        gt_depth, idx) and scored on the device (eval_image.image_metrics) into one device
+        buffer, which the host reads once at the end.  LPIPS is lpips_fn(gt, pred) of the
+        clipped DEVICE colours [H,W,3], once per frame, or NaN without the hook.  No figure is
+        written.  Prints the reference's per-frame and summary lines.  -> {'frames': [{'idx',
+        'psnr', 'ssim', 'lpips', 'depth_l1'}, ...], 'avg_psnr', 'avg_ssim', 'avg_lpips',
+        'avg_depth_l1'}, the averages None when no frame is scored."""
+        import numpy as np
+        from .eval_image import DEPTH_L1, PSNR, SSIM, image_metrics, lpips_inputs
+        if estimate_c2w_list is None:
+            estimate_c2w_list = self.get_estimate_c2w_list()
+        dev = self.device
+        picked = range(0, len(dataset), render_freq)
+        buf = torch.empty(len(picked), 4, dtype=torch.float64, device=dev)
+        ids, lpips = [], []
+        for i in picked:
+            idx, rgb, depth, _ = dataset[i]
+            idx = int(idx)
+            c2w = estimate_c2w_list[idx]
+            c2w = c2w.detach() if torch.is_tensor(c2w) else np.asarray(c2w)
+            color, rdepth = self.render_img(c2w, gt_depth=depth, idx=idx, to_host=False)
+            if color is None:
+                continue
+            gc = torch.as_tensor(np.asarray(rgb) if not torch.is_tensor(rgb) else rgb)
+            gd = torch.as_tensor(np.asarray(depth) if not torch.is_tensor(depth) else depth)
+            gc, gd = gc.to(dev, torch.float32)[None], gd.to(dev, torch.float32)[None]
+            k = len(ids)
+            image_metrics(gc, gd, color[None], rdepth[None], out=buf[k:k + 1])
+            if lpips_fn is not None:
+                lpips.append(lpips_fn(*lpips_inputs(gc[0], color, gd[0], False)))
+            ids.append(idx)
+        vals = buf[:len(ids)].cpu().numpy()
+        frames = []
+        for k, idx in enumerate(ids):
+            row = {'idx': idx, 'psnr': float(vals[k, PSNR]), 'ssim': float(vals[k, SSIM]),
+                   'lpips': float(lpips[k]) if lpips_fn is not None else float('nan'),
+                   'depth_l1': float(vals[k, DEPTH_L1])}
+            print(f"idx: {idx}, psnr[dB]: {row['psnr']}, ssim: {row['ssim']},"
+                  f"lpips: {row['lpips']}, depth_l1_render[cm]:{row['depth_l1']}")
+            frames.append(row)
+        res = {'frames': frames}
+        for key in ('psnr', 'ssim', 'lpips', 'depth_l1'):
+            s = 0
+            for row in frames:
+                s += row[key]
+            res['avg_' + key] = s / len(frames) if frames else None
+        if frames:
+            print(f"avg_psnr[dB]: {res['avg_psnr']}, avg_ms_ssim: {res['avg_ssim']},"
+                  f"avg_lpips: {res['avg_lpips']}, avg_depth_l1[cm]: {res['avg_depth_l1']}")
+        return res
 
     def is_separate_LR(self):
         with self.lock:

@@ -287,6 +287,18 @@ def clean_mesh(mesh, min_len=100):
     return TriMesh(v.cpu().numpy(), f.cpu().numpy(), vertex_colors=colors_to_u8(c).cpu().numpy())
 
 
+# ---- save_render_imgs (common.py:429-479): the render metrics on the device -------------------
+def save_render_imgs(idx, gt_color_np, gt_depth_np, color_np, depth_np, img_save_dir):
+    """The metrics of save_render_imgs on the device (eval_image.render_metrics): -> (psnr,
+    ssim, lpips, depth_l1_render) as floats, or None without a rendered colour.  LPIPS is NaN
+    (its network weights are not shipped) and no figure is written, so img_save_dir is unused."""
+    from .eval_image import render_metrics
+    r = render_metrics(gt_color_np, gt_depth_np, color_np, depth_np)
+    if r is None:
+        return None
+    return r['psnr'], r['ssim'], r['lpips'], r['depth_l1']
+
+
 # ---- cull_mesh (common.py:714-789): the frames' visibility test on the device -----------------
 CULL_CHUNK = 16  # frames per depth upload and visibility launch
 

@@ -319,7 +319,7 @@ class CoSLAM(Algorithm):
         return functools.reduce(torch.add, loss_dict.values())
 
     # coslam.py:245-289
-    def render_img(self, c2w, gt_depth=None, idx=None):
+    def render_img(self, c2w, gt_depth=None, idx=None, to_host=True):
         with self.lock, torch.no_grad():
             dev = self.device
             rays_o, rays_d = get_rays(self.camera, c2w, device=dev)
@@ -341,6 +341,8 @@ class CoSLAM(Algorithm):
                                                  self.camera.width)
             color = torch.cat(colors, 0).reshape(self.camera.height,
                                                  self.camera.width, 3)
+            if not to_host:
+                return color, depth
             return color.cpu().numpy(), depth.cpu().numpy()
 
     # coslam.py:291-298

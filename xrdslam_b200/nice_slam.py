@@ -172,9 +172,9 @@ class NiceSLAM(Algorithm):
         loss_dict = self.model.get_loss_dict(model_outputs, model_input, is_mapping, self.stage)
         return functools.reduce(torch.add, loss_dict.values())
 
-    def render_img(self, c2w, gt_depth=None, idx=None):
+    def render_img(self, c2w, gt_depth=None, idx=None, to_host=True):
         with self.lock, torch.no_grad():
-            return self._render_full(c2w, gt_depth, extra={'stage': 'color'})
+            return self._render_full(c2w, gt_depth, extra={'stage': 'color'}, to_host=to_host)
 
     # nice_slam.py:281-288
     def get_mesh(self):

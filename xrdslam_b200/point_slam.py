@@ -214,13 +214,14 @@ class PointSLAM(Algorithm):
         loss_dict = self.model.get_loss_dict(model_outputs, model_input, is_mapping, self.stage)
         return functools.reduce(torch.add, loss_dict.values())
 
-    def render_img(self, c2w, gt_depth=None, idx=None):
+    def render_img(self, c2w, gt_depth=None, idx=None, to_host=True):
         with self.lock, torch.no_grad():
             per_pixel = None
             if self.config.use_dynamic_radius:
                 per_pixel = {'batch_dynamic_r':
                              self.dynamic_r_query_allkeyframe[str(int(idx))].reshape(-1).float()}
-            return self._render_full(c2w, gt_depth, extra={'stage': 'color'}, per_pixel=per_pixel)
+            return self._render_full(c2w, gt_depth, extra={'stage': 'color'}, per_pixel=per_pixel,
+                                     to_host=to_host)
 
     # point_slam.py:426-435
     def get_mesh(self):

@@ -83,9 +83,9 @@ class VoxFusion(Algorithm):
         loss_dict = self.model.get_loss_dict(model_outputs, model_input, is_mapping, step)
         return functools.reduce(torch.add, loss_dict.values())
 
-    def render_img(self, c2w, gt_depth=None, idx=None):
+    def render_img(self, c2w, gt_depth=None, idx=None, to_host=True):
         with self.lock, torch.no_grad():
-            return self._render_full(c2w, gt_depth)
+            return self._render_full(c2w, gt_depth, to_host=to_host)
 
     # voxfusion.py:171-176
     def get_mesh(self):
