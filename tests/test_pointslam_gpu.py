@@ -167,7 +167,9 @@ def test_pointslam_step_vs_oracle(cuda_dev, is_mapping):
 @pytest.mark.parametrize('tag,is_mapping', [('cmap', True), ('ctrk', False)])
 def test_pointslam_color_golden(cuda_dev, tag, is_mapping):
     """Stage 'color' against the reference ConvOnet2's outputs, losses and every gradient
-    (geo/col features, rays, all colour-decoder tensors).  fp32 SIMT GEMMs; the softplus
+    (geo/col features, rays, all colour-decoder tensors).  The GEMMs run in the default
+    3xTF32 mode (the trunk on mma.sync: P = 400 columns is below the wgmma kernel's 512; the
+    neighbour MLP at 8 P = 3200 columns on the wgmma kernel); the softplus
     (beta = 100) trunk amplifies rounding differences ~10x relative to the geometry stage."""
     g = load_golden_pointslam()
     model = pointslam_from_golden(g, 'b200', cuda_dev)
