@@ -1010,6 +1010,55 @@ int xrd_eval_image_metrics(const float* gt_color, const float* color, const floa
                            const double* depth, int B, int H, int W, int flags, double* out,
                            double* levels, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Frame ingest -----------------------------------------------------------
+ *
+ *   xrd_frame_ingest  slam/common/datasets.py:95-134 BaseDataset.__getitem__ after decoding:
+ *                     B decoded frames -> the float32 colour and depth frames of the dataset
+ *
+ * color DEVICE uint8 [B][H0][W0][3] in BGR order (cv2.imread's), depth DEVICE uint16
+ * [B][Hd][Wd]; rgb DEVICE f32 [B][h][w][3], depth_out DEVICE f32 [B][h][w] with
+ * (h, w) = (Hd - 2 crop_edge, Wd - 2 crop_edge), each divided (floor) by downsample_factor when it
+ * is > 1.  Stage by stage, in cv2's own arithmetic (cv2 without Intel IPP; with IPP, cv2 hands
+ * the INTER_LINEAR resize of f64 colour in step 4 to IPP, which differs by up to ~2e-6):
+ *   1. n_dist > 0: cv::undistort(color, K, dist) with K = [fx 0 cx; 0 fy cy; 0 0 1]: per stripe of
+ *      max(1, 4096 / W0) rows, initUndistortRectifyMap with new camera matrix K (cy shifted to the
+ *      stripe), its inverse by the 3x3 cofactor formula, the k1 k2 p1 p2 k3 k4 k5 k6 s1 s2 s3 s4
+ *      model (missing ones 0) in f64, maps cvRound(u 32) / cvRound(v 32) (CV_16SC2 + 1/32-pixel
+ *      fractions), remap INTER_LINEAR with 15-bit weights ((sum + 2^14) >> 15) and
+ *      BORDER_CONSTANT 0.  The column coordinate is ir2 + x ir0 per pixel where cv2 sums
+ *      ir0 along the row; the two agree to ~1e-15 pixel before the 1/32-pixel rounding.
+ *   2. BGR -> RGB, value / 255. in f64.
+ *   3. depth = f32(d) / f32(png_depth_scale), f32 division.
+ *   4. colour cv2.resize to (Hd, Wd) INTER_LINEAR on f64: scale = 1 / (dst / src), f32 weights
+ *      t = f32((d + 0.5) scale - 0.5) - floor, x clamped with weights (1, 0) at the borders, rows
+ *      clamped when fetched, h = s0 a0 + s1 a1 along x then h0 b0 + h1 b1; exactly 2x on both
+ *      axes is cv2's 2x2 area average (((0 + s00) + s01) + s10) + s11) * 0.25; equal sizes copy.
+ *   5. crop crop_edge pixels on every side; 6. downsample_factor > 1: colour as in 4, depth
+ *      INTER_NEAREST (min(floor(d scale), src - 1)); 7. colour rounded to f32.
+ * No operation is contracted into an FMA.  Asynchronous on `stream`, no allocation.  With
+ * n_dist > 0 the undistorted colour frames live in the workspace (B H0 W0 3 bytes); without, the
+ * workspace is 0 bytes and may be NULL.
+ * B in [1, 65535], every side in [1, 32767], n_dist in {0, 4, 5, 8, 12}, crop_edge >= 0,
+ * downsample_factor >= 1, png_depth_scale != 0 and h, w >= 1, else XRD_E_SHAPE (and
+ * xrd_frame_ingest_workspace_bytes returns 0); cfg or a data pointer NULL, or a NULL workspace
+ * where one is needed: XRD_E_NULL; workspace_bytes < xrd_frame_ingest_workspace_bytes(cfg):
+ * XRD_E_WORKSPACE. */
+typedef struct {
+  int B, H0, W0;            /* colour frames                                                */
+  int Hd, Wd;               /* depth frames                                                 */
+  double fx, fy, cx, cy;    /* the camera of the colour frames (cam: in devices.yaml)       */
+  double dist[12];          /* distortion coefficients, the first n_dist used               */
+  int n_dist;               /* 0 = no undistortion                                          */
+  double png_depth_scale;
+  int crop_edge;
+  int downsample_factor;
+} XrdIngestCfg;
+
+size_t xrd_frame_ingest_workspace_bytes(const XrdIngestCfg* cfg);
+int xrd_frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color, const uint16_t* depth,
+                     float* rgb, float* depth_out, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -249,6 +249,14 @@ class XrdPointGrads(C.Structure):
                 ('color', C.POINTER(XrdPointColorDecoderGrads))]
 
 
+class XrdIngestCfg(C.Structure):
+    _fields_ = [('B', C.c_int), ('H0', C.c_int), ('W0', C.c_int), ('Hd', C.c_int),
+                ('Wd', C.c_int), ('fx', C.c_double), ('fy', C.c_double), ('cx', C.c_double),
+                ('cy', C.c_double), ('dist', C.c_double * 12), ('n_dist', C.c_int),
+                ('png_depth_scale', C.c_double), ('crop_edge', C.c_int),
+                ('downsample_factor', C.c_int)]
+
+
 _lib = None
 
 # name -> (restype, argtypes); every symbol include/xrdslam_b200.h declares
@@ -368,6 +376,8 @@ SYMBOLS = {
     'xrd_eval_image_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     'xrd_eval_image_metrics': (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp,
                                          vp, vp, C.c_size_t, vp]),
+    'xrd_frame_ingest_workspace_bytes': (C.c_size_t, [C.POINTER(XrdIngestCfg)]),
+    'xrd_frame_ingest': (C.c_int, [C.POINTER(XrdIngestCfg), vp, vp, vp, vp, vp, C.c_size_t, vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

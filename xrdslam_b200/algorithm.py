@@ -89,6 +89,14 @@ class Algorithm():
             frame.__dict__[key] = t
         return t
 
+    def seed_frame_tensors(self, frame, rgb=None, depth=None):
+        """Give `frame` the device copies of its images that _frame_tensor would upload, from
+        tensors already on the device (the dataset's ingest output): rgb f32 [H,W,3], depth f32
+        [H,W].  Tensors on another device or dtype are converted."""
+        for which, t in (('rgb', rgb), ('depth', depth)):
+            if t is not None:
+                frame.__dict__['_dev_' + which] = t.to(self.device, torch.float32).contiguous()
+
     def _sample_window(self, frames, n, Hedge=0, Wedge=0, return_index=False):
         """All frames of the window at once: one batched pose evaluation, one H2D, three
         launches (csrc/rays.cu) -- instead of ~150 ATen launches and a host Rodrigues /
@@ -110,8 +118,9 @@ class Algorithm():
         rays_o, rays_d = get_rays(self.camera, torch.as_tensor(c2w), device=dev)
         rays_o, rays_d = rays_o.reshape(-1, 3), rays_d.reshape(-1, 3)
         if gt_depth is not None:
-            gt_depth = torch.as_tensor(np.asarray(gt_depth), dtype=torch.float32).to(dev
-                                                                                     ).reshape(-1, 1)
+            if not torch.is_tensor(gt_depth):  # a dataset's device frame is used as it is
+                gt_depth = np.asarray(gt_depth)
+            gt_depth = torch.as_tensor(gt_depth, dtype=torch.float32).to(dev).reshape(-1, 1)
         depths, colors = [], []
         bs = self.config.ray_batch_size
         for i in range(0, rays_d.shape[0], bs):

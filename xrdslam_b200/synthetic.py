@@ -30,10 +30,11 @@ def look_at(eye, target, up=np.array([0.0, 0.0, 1.0])):
     return c2w.astype(np.float32)
 
 
-def trajectory(n_frames, radius=0.8, offset=(0.0, 0.0, 0.0)):
+def trajectory(n_frames, radius=0.8, offset=(0.0, 0.0, 0.0), turn=0.25):
+    """c2w of n_frames cameras on a circle: `turn` of a full revolution over the run."""
     poses = []
     for k in range(n_frames):
-        a = 2 * np.pi * k / max(n_frames, 1) * 0.25  # quarter turn over the run
+        a = 2 * np.pi * k / max(n_frames, 1) * turn
         eye = CENTRE + np.array([radius * np.cos(a), radius * np.sin(a), 0.1])
         tgt = CENTRE + np.array([-1.5 * np.cos(a + 0.6), -1.5 * np.sin(a + 0.6), -0.3])
         c2w = look_at(eye, tgt)
@@ -77,12 +78,54 @@ def render_frame(camera: Camera, c2w, offset=(0.0, 0.0, 0.0), invalid_frac=0.02,
     return rgb.astype(np.float32), depth.astype(np.float32)
 
 
-def make_sequence(n_frames, width=640, height=480, offset=(0.0, 0.0, 0.0)):
+def make_sequence(n_frames, width=640, height=480, offset=(0.0, 0.0, 0.0), turn=0.25):
     cam = make_camera(width, height)
-    poses = trajectory(n_frames, offset=offset)
+    poses = trajectory(n_frames, offset=offset, turn=turn)
     frames = [render_frame(cam, p, offset=offset, seed=k)
               for k, p in enumerate(poses)]
     return cam, poses, frames
+
+
+REPLICA_DEPTH_SCALE = 6553.5
+
+
+def write_replica(folder, n_frames, width=640, height=480, offset=(0.0, 0.0, 0.0), turn=0.25):
+    """The sequence of make_sequence as a Replica folder: results/frame%06d.jpg (colour, JPEG
+    quality 95), results/depth%06d.png (uint16 depth x 6553.5), traj.txt (one row-major c2w per
+    line in the dataset's camera axes: columns 1 and 2 negated, the inverse of the reader's flip)
+    and devices.yaml.  -> (camera, poses)."""
+    import os
+    cam, poses, frames = make_sequence(n_frames, width=width, height=height, offset=offset,
+                                       turn=turn)
+    res = os.path.join(folder, 'results')
+    os.makedirs(res, exist_ok=True)
+    try:
+        import cv2
+    except ImportError:
+        cv2 = None
+    for k, (rgb, depth) in enumerate(frames):
+        rgb8 = np.clip(np.rint(rgb * 255.0), 0, 255).astype(np.uint8)
+        d16 = np.clip(np.rint(depth.astype(np.float64) * REPLICA_DEPTH_SCALE), 0,
+                      65535).astype(np.uint16)
+        cpath = os.path.join(res, f'frame{k:06d}.jpg')
+        dpath = os.path.join(res, f'depth{k:06d}.png')
+        if cv2 is not None:
+            cv2.imwrite(cpath, rgb8[..., ::-1], [cv2.IMWRITE_JPEG_QUALITY, 95])
+            cv2.imwrite(dpath, d16)
+        else:
+            from PIL import Image
+            Image.fromarray(rgb8).save(cpath, quality=95)
+            Image.fromarray(d16).save(dpath)
+    with open(os.path.join(folder, 'traj.txt'), 'w') as f:
+        for p in poses:
+            q = np.asarray(p, np.float64).copy()
+            q[:3, 1] *= -1
+            q[:3, 2] *= -1
+            f.write(' '.join(repr(float(v)) for v in q.reshape(-1)) + '\n')
+    with open(os.path.join(folder, 'devices.yaml'), 'w') as f:
+        f.write(f'cam:\n  H: {height}\n  W: {width}\n  fx: {cam.fx!r}\n  fy: {cam.fy!r}\n'
+                f'  cx: {cam.cx!r}\n  cy: {cam.cy!r}\n  png_depth_scale: {REPLICA_DEPTH_SCALE}\n')
+    return cam, poses
 
 
 def _grid_rect(origin, u, v, nu, nv):
