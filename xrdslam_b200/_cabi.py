@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'lib', 'libxrdslam_b200.so')
 
@@ -438,6 +440,41 @@ def lib():
 def check(fn_name, status):
     if status != 0:
         raise XrdError(fn_name, status, lib().xrd_last_cuda_error())
+
+
+def call(name, *args):
+    """lib().<name>(*args) for an entry point that returns an XrdStatus; raises XrdError naming
+    it on a non-zero status."""
+    check(name, getattr(lib(), name)(*args))
+
+
+def launch(name, *args, stream):
+    """call() with the cudaStream_t handle `stream` appended as the last argument.  Switches no
+    device, allocates nothing and does not synchronise, so it may run under stream capture."""
+    call(name, *args, stream)
+
+
+def launch_on(dev, name, *args):
+    """launch() with `dev` as the current device, on that device's current stream."""
+    with torch.cuda.device(dev):
+        launch(name, *args, stream=torch.cuda.current_stream(dev).cuda_stream)
+
+
+def workspace(dev, name, *size_args, error=None):
+    """-> (buffer, nbytes): nbytes = xrd_<name>_workspace_bytes(*size_args) as the library
+    reports it (pass it on), buffer a uint8 tensor on `dev` of at least one byte, so the entry
+    point never sees a null workspace and reports a rejected size itself.  With `error`, a
+    reported size of 0 raises ValueError(error) instead."""
+    nb = getattr(lib(), f'xrd_{name}_workspace_bytes')(*size_args)
+    if nb == 0 and error is not None:
+        raise ValueError(error)
+    return torch.empty(max(nb, 1), dtype=torch.uint8, device=dev), nb
+
+
+def require_cuda(dev, what):
+    """There is no CPU path: raise unless `dev` is a CUDA device."""
+    if torch.device(dev).type != 'cuda':
+        raise RuntimeError(f'xrdslam_b200 has no CPU path: {what} must be on a CUDA device')
 
 
 def ptr(t):

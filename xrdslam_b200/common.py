@@ -24,11 +24,8 @@ class _PosedRays(torch.autograd.Function):
         R = dirs.shape[0]
         rays_o = torch.empty(R, 3, device=dirs.device)
         rays_d = torch.empty(R, 3, device=dirs.device)
-        with torch.cuda.device(dirs.device):
-            st = _cabi.lib().xrd_rays_from_poses(
-                R, _cabi.ptr(dirs), _cabi.ptr(ids), _cabi.ptr(P), P.shape[0], _cabi.ptr(rays_o),
-                _cabi.ptr(rays_d), torch.cuda.current_stream(dirs.device).cuda_stream)
-        _cabi.check('xrd_rays_from_poses', st)
+        _cabi.launch_on(dirs.device, 'xrd_rays_from_poses', R, _cabi.ptr(dirs), _cabi.ptr(ids),
+                        _cabi.ptr(P), P.shape[0], _cabi.ptr(rays_o), _cabi.ptr(rays_d))
         ctx.save_for_backward(dirs, ids)
         ctx.n_poses = P.shape[0]
         return rays_o, rays_d
@@ -39,12 +36,9 @@ class _PosedRays(torch.autograd.Function):
         dirs, ids = ctx.saved_tensors
         d_poses = torch.empty(ctx.n_poses, 4, 4, device=dirs.device)
         g_o, g_d = g_o.contiguous(), g_d.contiguous()
-        with torch.cuda.device(dirs.device):
-            st = _cabi.lib().xrd_rays_pose_grads(
-                dirs.shape[0], _cabi.ptr(dirs), _cabi.ptr(ids), ctx.n_poses, _cabi.ptr(g_o),
-                _cabi.ptr(g_d), _cabi.ptr(d_poses),
-                torch.cuda.current_stream(dirs.device).cuda_stream)
-        _cabi.check('xrd_rays_pose_grads', st)
+        _cabi.launch_on(dirs.device, 'xrd_rays_pose_grads', dirs.shape[0], _cabi.ptr(dirs),
+                        _cabi.ptr(ids), ctx.n_poses, _cabi.ptr(g_o), _cabi.ptr(g_d),
+                        _cabi.ptr(d_poses))
         return None, None, d_poses
 
 
@@ -72,8 +66,7 @@ def sample_window(camera, depth_imgs, rgb_imgs, poses, n, Hedge=0, Wedge=0, indi
     import ctypes as C
     from . import _cabi
     dev = poses.device
-    if dev.type != 'cuda':
-        raise RuntimeError('xrdslam_b200 has no CPU path')
+    _cabi.require_cuda(dev, 'poses')
     F = len(depth_imgs)
     H, W = camera.height, camera.width
     H0, H1, W0, W1 = Hedge, H - Hedge, Wedge, W - Wedge
@@ -90,12 +83,8 @@ def sample_window(camera, depth_imgs, rgb_imgs, poses, n, Hedge=0, Wedge=0, indi
                                   camera.cy)
     dp = (C.c_void_p * F)(*[_cabi.ptr(t) for t in depth_imgs])
     cp = (C.c_void_p * F)(*[_cabi.ptr(t) for t in rgb_imgs])
-    with torch.cuda.device(dev):
-        st = _cabi.lib().xrd_sample_pixels(
-            C.byref(cfg), dp, cp, _cabi.ptr(indices), _cabi.ptr(dirs), _cabi.ptr(depth),
-            _cabi.ptr(rgb), _cabi.ptr(ids), _cabi.ptr(ij),
-            torch.cuda.current_stream(dev).cuda_stream)
-    _cabi.check('xrd_sample_pixels', st)
+    _cabi.launch_on(dev, 'xrd_sample_pixels', C.byref(cfg), dp, cp, _cabi.ptr(indices),
+                    _cabi.ptr(dirs), _cabi.ptr(depth), _cabi.ptr(rgb), _cabi.ptr(ids), _cabi.ptr(ij))
     rays_o, rays_d = _PosedRays.apply(dirs, ids, poses)
     if return_index:
         return rays_o, rays_d, depth, rgb, ij[:, 0], ij[:, 1]
@@ -330,8 +319,7 @@ def cull_visibility(dataset, vertices, estimate_c2w_list=None, eval_rec=False, t
     from . import _cabi
     from ._cabi import XRD_CULL_MAX_FRAMES, XrdCullParams
     dev = torch.device(device)
-    if dev.type != 'cuda':
-        raise RuntimeError('xrdslam_b200 has no CPU path: cull_mesh runs on a CUDA device')
+    _cabi.require_cuda(dev, 'cull_mesh')
     n_imgs = len(estimate_c2w_list) if estimate_c2w_list is not None else len(dataset)
     cam = dataset.get_camera()
     H, W = int(cam.height), int(cam.width)
@@ -343,7 +331,6 @@ def cull_visibility(dataset, vertices, estimate_c2w_list=None, eval_rec=False, t
     if V == 0 or n_imgs == 0:
         return seen
     chunk = max(1, min(int(chunk), XRD_CULL_MAX_FRAMES, n_imgs))
-    lib = _cabi.lib()
     with torch.cuda.device(dev):
         main = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
@@ -391,9 +378,9 @@ def cull_visibility(dataset, vertices, estimate_c2w_list=None, eval_rec=False, t
                 dst.copy_(t)
             for j in range(n):
                 w2c[j].copy_(cull_w2c(pose_d[b][j]))
-            _cabi.check('xrd_cull_visible', lib.xrd_cull_visible(
-                _cabi.ptr(verts), V, _cabi.ptr(w2c), _cabi.ptr(depth_d[b]), n,
-                C.byref(P), _cabi.ptr(seen), main.cuda_stream))
+            _cabi.launch('xrd_cull_visible', _cabi.ptr(verts), V, _cabi.ptr(w2c),
+                         _cabi.ptr(depth_d[b]), n, C.byref(P), _cabi.ptr(seen),
+                         stream=main.cuda_stream)
             consumed[b] = torch.cuda.Event()
             consumed[b].record(main)
     return seen
@@ -419,25 +406,21 @@ def cull_compact(seen, vertices, faces, colors=None):
         row = int(np.prod(colors.shape[1:], dtype=np.int64))
         cb = row * colors.element_size()
         cbytes = colors.reshape(V, row).view(torch.uint8)   # [V, cb]: any element type
-    lib = _cabi.lib()
-    nb = lib.xrd_cull_workspace_bytes(V, nF)
-    if nb == 0:
-        raise ValueError(f'cull_mesh: unsupported mesh size V={V}, F={nF}')
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    ws, nb = _cabi.workspace(dev, 'cull', V, nF,
+                             error=f'cull_mesh: unsupported mesh size V={V}, F={nF}')
     counts = torch.empty(3, dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
-        s = torch.cuda.current_stream(dev).cuda_stream
-        _cabi.check('xrd_cull_count', lib.xrd_cull_count(
-            _cabi.ptr(seen), V, _cabi.ptr(faces), nF, _cabi.ptr(counts), _cabi.ptr(ws), nb, s))
+        _cabi.launch_on(dev, 'xrd_cull_count', _cabi.ptr(seen), V, _cabi.ptr(faces), nF,
+                        _cabi.ptr(counts), _cabi.ptr(ws), nb)
         V2, F2, bad = counts.tolist()
         if bad:
             raise ValueError(f'cull_mesh: {bad} faces index outside [0, {V})')
         out_v = torch.empty(V2, 3, dtype=torch.float32, device=dev)
         out_f = torch.empty(F2, 3, dtype=torch.int32, device=dev)
         out_c = torch.empty(V2, cb, dtype=torch.uint8, device=dev) if colors is not None else None
-        _cabi.check('xrd_cull_emit', lib.xrd_cull_emit(
-            _cabi.ptr(verts), _cabi.ptr(cbytes), cb, V, _cabi.ptr(faces), nF, _cabi.ptr(out_v),
-            _cabi.ptr(out_c), _cabi.ptr(out_f), _cabi.ptr(ws), nb, s))
+        _cabi.launch_on(dev, 'xrd_cull_emit', _cabi.ptr(verts), _cabi.ptr(cbytes), cb, V,
+                        _cabi.ptr(faces), nF, _cabi.ptr(out_v), _cabi.ptr(out_c), _cabi.ptr(out_f),
+                        _cabi.ptr(ws), nb)
     if colors is not None:
         out_c = out_c.view(colors.dtype).reshape((V2, ) + tuple(colors.shape[1:]))
     return out_v, out_f, out_c

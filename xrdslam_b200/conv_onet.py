@@ -24,7 +24,7 @@ from torch.nn import Parameter
 
 from . import _cabi
 from ._cabi import (XrdNiceCfg, XrdNiceCoarseCfg, XrdNiceCoarseDecoder, XrdNiceDecoder,
-                    XrdNiceDecoderGrads, XrdNiceGrads, XrdNiceGrid, XrdNiceOut, XrdRays, check, ptr)
+                    XrdNiceDecoderGrads, XrdNiceGrads, XrdNiceGrid, XrdNiceOut, XrdRays, ptr)
 from .base_model import Model, ModelConfig, scale_grads, upstream_scale
 
 STAGES = {'middle': 0, 'fine': 1, 'color': 2}  # 'coarse' has its own entry (xrd_nice_coarse_step)
@@ -295,9 +295,7 @@ class ConvOnet(Model):
                 need_rays=False, need_grid=(False, False, False), need_col=False):
         cfg = self.config
         dev = self.grids['grid_middle'].device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on a CUDA device')
-        lib = _cabi.lib()
+        _cabi.require_cuda(dev, 'model')
         f32 = dict(dtype=torch.float32, device=dev)
         f64 = dict(dtype=torch.float64, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()
@@ -359,13 +357,9 @@ class ConvOnet(Model):
                 keep.append(dg)
                 gs.d_color = C.pointer(dg)
             gs.d_rays_o, gs.d_rays_d = ptr(g['d_rays_o']), ptr(g['d_rays_d'])
-        nb = lib.xrd_nice_workspace_bytes(R, S, int(with_grads))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_nice_step(C.byref(rays), grids, decs, C.byref(c), C.byref(out),
-                                   C.byref(gs) if gs is not None else None, ptr(ws), nb,
-                                   torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_nice_step', st)
+        ws, nb = _cabi.workspace(dev, 'nice', R, S, int(with_grads))
+        _cabi.launch_on(dev, 'xrd_nice_step', C.byref(rays), grids, decs, C.byref(c), C.byref(out),
+                        C.byref(gs) if gs is not None else None, ptr(ws), nb)
         return o, g
 
     def _launch_coarse(self, rays_o, rays_d, target_d, with_grads, need_rays=False,
@@ -376,9 +370,7 @@ class ConvOnet(Model):
             raise RuntimeError("stage 'coarse' needs ConvOnetConfig(coarse=True)")
         grid = self.grids['grid_coarse']
         dev = grid.device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on a CUDA device')
-        lib = _cabi.lib()
+        _cabi.require_cuda(dev, 'model')
         f32 = dict(dtype=torch.float32, device=dev)
         f64 = dict(dtype=torch.float64, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()
@@ -416,15 +408,11 @@ class ConvOnet(Model):
             gr = dict(d_grid=torch.zeros_like(grid) if need_grid else None,
                       d_rays_o=torch.empty(R, 3, **f32) if need_rays else None,
                       d_rays_d=torch.empty(R, 3, **f32) if need_rays else None)
-        nb = lib.xrd_nice_coarse_workspace_bytes(R, S, int(with_grads))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_nice_coarse_step(
-                C.byref(rays), C.byref(gs), C.byref(dec), C.byref(c), C.byref(out),
-                ptr(gr['d_grid']) if gr else None, ptr(gr['d_rays_o']) if gr else None,
-                ptr(gr['d_rays_d']) if gr else None, int(with_grads), ptr(ws), nb,
-                torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_nice_coarse_step', st)
+        ws, nb = _cabi.workspace(dev, 'nice_coarse', R, S, int(with_grads))
+        _cabi.launch_on(dev, 'xrd_nice_coarse_step', C.byref(rays), C.byref(gs), C.byref(dec),
+                        C.byref(c), C.byref(out), ptr(gr['d_grid']) if gr else None,
+                        ptr(gr['d_rays_o']) if gr else None, ptr(gr['d_rays_d']) if gr else None,
+                        int(with_grads), ptr(ws), nb)
         return o, gr
 
     # --------------------------------------------------------- Model API ---
@@ -465,9 +453,7 @@ class ConvOnet(Model):
     # ---- mesher-facing queries (conv_onet.py:213-240) -----------------------------------
     def _query(self, pi, stage):
         dev = self.grids['grid_middle'].device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on a CUDA device')
-        lib = _cabi.lib()
+        _cabi.require_cuda(dev, 'model')
         pts = pi.detach().reshape(-1, 3).to(device=dev, dtype=torch.float32).contiguous()
         P = pts.shape[0]
         keys = ('grid_middle', 'grid_fine', 'grid_color')
@@ -485,12 +471,9 @@ class ConvOnet(Model):
         bmin = (C.c_double * 3)(*[float(self.bounding_box[d, 0]) for d in range(3)])
         bmax = (C.c_double * 3)(*[float(self.bounding_box[d, 1]) for d in range(3)])
         raw = torch.empty(P, 4, dtype=torch.float32, device=dev)
-        nb = lib.xrd_nice_query_workspace_bytes(P)
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_nice_query(ptr(pts), P, grids, decs, bmin, bmax, STAGES[stage], ptr(raw),
-                                    ptr(ws), nb, torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_nice_query', st)
+        ws, nb = _cabi.workspace(dev, 'nice_query', P)
+        _cabi.launch_on(dev, 'xrd_nice_query', ptr(pts), P, grids, decs, bmin, bmax, STAGES[stage],
+                        ptr(raw), ptr(ws), nb)
         return raw
 
     def query_fn(self, pi):

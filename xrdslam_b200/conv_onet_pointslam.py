@@ -20,7 +20,7 @@ from torch.nn import Parameter
 from . import _cabi
 from ._cabi import (XrdNiceDecoder, XrdPointCfg, XrdPointColorDecoder,
                     XrdPointColorDecoderGrads, XrdPointFeats, XrdPointGrads, XrdPointOut,
-                    XrdRays, check, ptr)
+                    XrdRays, ptr)
 from .base_model import Model, ModelConfig, scale_grads, upstream_scale
 from .conv_onet import MLP as _GeoMLP
 from .conv_onet import _dec_struct
@@ -235,9 +235,7 @@ class ConvOnet2(Model):
         color = stage == 'color'
         npc = self.neural_point_cloud
         dev = npc.device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path')
-        lib = _cabi.lib()
+        _cabi.require_cuda(dev, 'the neural point cloud')
         f32 = dict(dtype=torch.float32, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()
         rays_d = rays_d.detach().to(**f32).contiguous()
@@ -284,15 +282,10 @@ class ConvOnet2(Model):
             cg = _color_struct(XrdPointColorDecoderGrads, g['d_cdec']) if need_cdec else None
             gs = XrdPointGrads(ptr(g['d_geo_feats']), ptr(g['d_rays_o']), ptr(g['d_rays_d']),
                                ptr(g['d_col_feats']), C.pointer(cg) if cg is not None else None)
-        nb = lib.xrd_pointslam_workspace_bytes(R, S, int(color), int(with_grads))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_pointslam_step(C.byref(rays), C.byref(ix), C.byref(feats), C.byref(dec),
-                                        C.byref(cdec) if cdec is not None else None,
-                                        C.byref(c), C.byref(out),
-                                        C.byref(gs) if gs is not None else None, ptr(ws), nb,
-                                        torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_pointslam_step', st)
+        ws, nb = _cabi.workspace(dev, 'pointslam', R, S, int(color), int(with_grads))
+        _cabi.launch_on(dev, 'xrd_pointslam_step', C.byref(rays), C.byref(ix), C.byref(feats),
+                        C.byref(dec), C.byref(cdec) if cdec is not None else None, C.byref(c),
+                        C.byref(out), C.byref(gs) if gs is not None else None, ptr(ws), nb)
         o['valid_ray_mask'] = o['valid_ray_mask'].bool()
         return o, g
 

@@ -24,7 +24,7 @@ import torch
 
 from . import _cabi
 from ._cabi import (XrdAdamTensor, XrdCoslamCfg, XrdCoslamGrads, XrdCoslamMlp, XrdCoslamOut,
-                    XrdRays, check, ptr)
+                    XrdRays, launch, ptr)
 from .optimizers import FusedAdam
 
 
@@ -49,10 +49,9 @@ class MappingGraphSession:
         self.d_rays_o, self.d_rays_d = z(R, 3), z(R, 3)
         self.out = dict(rgb=z(R, 3), depth=z(R), disp=z(R), acc=z(R), var=z(R), z_vals=z(R, S),
                         raw=z(R, S, 4))
-        lib = _cabi.lib()
-        self.ws = torch.empty(lib.xrd_coslam_workspace_bytes(R, S), dtype=torch.uint8, device=dev)
-        self.ws_s = torch.empty(lib.xrd_coslam_smoothness_workspace_bytes(cfg.trainging_smooth_pts),
-                                dtype=torch.uint8, device=dev)
+        self.ws, self.ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
+        self.ws_s, self.ws_s_bytes = _cabi.workspace(dev, 'coslam_smoothness',
+                                                     cfg.trainging_smooth_pts)
         # per-iteration scalars: [seed u64 | smooth_rand f32 x6 | (lr, bc1, bc2) per group]
         self.dyn = torch.zeros(128, dtype=torch.uint8, device=dev)
         self._dyn_ring = [torch.zeros(128, dtype=torch.uint8).pin_memory() for _ in range(8)]
@@ -149,34 +148,30 @@ class MappingGraphSession:
     def _part_a(self, stream):
         """zero the bucket, unpack the rows, poses -> c2w -> rays (+ the sample phase when the
         batch is sharded: z_vals and this rank's loss-normaliser counts)."""
-        lib, R, n = _cabi.lib(), self.R, self.n_poses
+        R, n = self.R, self.n_poses
         self.flat.zero_()
         self.dirs = self.rows[:, :3].contiguous()
         self.ts = self.rows[:, 3:6].contiguous()
         self.td = self.rows[:, 6].contiguous()
-        check('xrd_pose_matrices',
-              lib.xrd_pose_matrices(n, ptr(self.rot), ptr(self.trans), ptr(self.poses), stream))
-        check('xrd_rays_from_poses',
-              lib.xrd_rays_from_poses(R, ptr(self.dirs), ptr(self.ids), ptr(self.poses), n,
-                                      ptr(self.rays_o), ptr(self.rays_d), stream))
+        launch('xrd_pose_matrices', n, ptr(self.rot), ptr(self.trans), ptr(self.poses),
+               stream=stream)
+        launch('xrd_rays_from_poses', R, ptr(self.dirs), ptr(self.ids), ptr(self.poses), n,
+               ptr(self.rays_o), ptr(self.rays_d), stream=stream)
         if self.world > 1:
             rays, grid, mlp, c, out = self._step_structs(1)
-            check('xrd_coslam_step[sample]',
-                  lib.xrd_coslam_step(C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
-                                      C.byref(out), None, ptr(self.ws), self.ws.numel(), stream))
+            launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
+                   C.byref(out), None, ptr(self.ws), self.ws_bytes, stream=stream)
 
     def _part_b(self, stream, smooth=True, pose=True):
         """fused forward / loss / backward (+ smoothness, pose-gradient reduction)."""
-        model, cfg, lib = self.model, self.model.config, _cabi.lib()
         rays, grid, mlp, c, out = self._step_structs(2 if self.world > 1 else 0)
         G = self.grads
         gs = XrdCoslamGrads(ptr(G[self.table]), *(ptr(G[t]) for t in self.weights),
                             ptr(self.d_rays_o) if self.ba else None,
                             ptr(self.d_rays_d) if self.ba else None,
                             (C.c_float * 4)(1.0, 1.0, 1.0, 1.0))
-        check('xrd_coslam_step',
-              lib.xrd_coslam_step(C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
-                                  C.byref(out), C.byref(gs), ptr(self.ws), self.ws.numel(), stream))
+        launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
+               C.byref(out), C.byref(gs), ptr(self.ws), self.ws_bytes, stream=stream)
         if smooth:
             self._part_smooth(stream)
         if pose:
@@ -188,24 +183,22 @@ class MappingGraphSession:
         the all-reduced sum is the single-GPU term."""
         if self.first:
             return
-        model, cfg, lib = self.model, self.model.config, _cabi.lib()
+        model, cfg = self.model, self.model.config
         grid = model._grid_struct(self.table.detach())
-        check('xrd_coslam_smoothness_dev', lib.xrd_coslam_smoothness_dev(
-            C.byref(grid), cfg.trainging_smooth_pts, cfg.trainging_smooth_vox,
-            cfg.trainging_smooth_margin, cfg.trainging_smooth_weight / self.world,
-            self.dyn.data_ptr() + 8, ptr(self.smooth_loss), ptr(self.grads[self.table]), 1.0,
-            ptr(self.ws_s), self.ws_s.numel(), stream))
+        launch('xrd_coslam_smoothness_dev', C.byref(grid), cfg.trainging_smooth_pts,
+               cfg.trainging_smooth_vox, cfg.trainging_smooth_margin,
+               cfg.trainging_smooth_weight / self.world, self.dyn.data_ptr() + 8,
+               ptr(self.smooth_loss), ptr(self.grads[self.table]), 1.0, ptr(self.ws_s),
+               self.ws_s_bytes, stream=stream)
 
     def _part_pose(self, stream):
         if not self.ba:
             return
-        lib, R, n = _cabi.lib(), self.R, self.n_poses
-        check('xrd_rays_pose_grads', lib.xrd_rays_pose_grads(
-            R, ptr(self.dirs), ptr(self.ids), n, ptr(self.d_rays_o), ptr(self.d_rays_d),
-            ptr(self.d_poses), stream))
-        check('xrd_pose_matrices_grads', lib.xrd_pose_matrices_grads(
-            n, ptr(self.rot), ptr(self.d_poses), ptr(self.fixed), ptr(self.d_rot_it),
-            ptr(self.d_trans_it), stream))
+        R, n = self.R, self.n_poses
+        launch('xrd_rays_pose_grads', R, ptr(self.dirs), ptr(self.ids), n, ptr(self.d_rays_o),
+               ptr(self.d_rays_d), ptr(self.d_poses), stream=stream)
+        launch('xrd_pose_matrices_grads', n, ptr(self.rot), ptr(self.d_poses), ptr(self.fixed),
+               ptr(self.d_rot_it), ptr(self.d_trans_it), stream=stream)
 
     def _part_pose_acc(self):
         if self.ba:
@@ -214,7 +207,6 @@ class MappingGraphSession:
 
     def _part_c(self, stream, with_adam, pose_acc=True):
         """Adam on table + decoder, pose-gradient accumulation (accum_step), total loss."""
-        lib = _cabi.lib()
         if with_adam:
             descs = self._adam_descs()
         else:  # warm-up: load the kernel on scratch tensors, leave the model untouched
@@ -226,7 +218,7 @@ class MappingGraphSession:
             a.bias_correction1 = a.bias_correction2 = 1.0
             descs = [a]
         arr = (XrdAdamTensor * len(descs))(*descs)
-        check('xrd_adam_step', lib.xrd_adam_step(arr, len(descs), 0, stream))
+        launch('xrd_adam_step', arr, len(descs), 0, stream=stream)
         if pose_acc:
             self._part_pose_acc()
         self.loss_total = self.flat[-8:-3].sum()
@@ -440,10 +432,8 @@ class MappingGraphSession:
             a.n, a.lr, a.beta1, a.beta2, a.eps = p.numel(), o.lr, o.betas[0], o.betas[1], o.eps
             a.weight_decay = getattr(o, 'weight_decay', 0)
             a.bias_correction1, a.bias_correction2 = 1.0 - o.betas[0]**t, 1.0 - o.betas[1]**t
-        with torch.cuda.device(self.dev):
-            # zero_grad = 1: the accumulated pose gradients restart after the step
-            check('xrd_adam_step', _cabi.lib().xrd_adam_step(
-                arr, 2, 1, torch.cuda.current_stream(self.dev).cuda_stream))
+        # zero_grad = 1: the accumulated pose gradients restart after the step
+        _cabi.launch_on(self.dev, 'xrd_adam_step', arr, 2, 1)
 
     def end(self, optimize_frames):
         """Write the optimised poses back into the Frame parameters (host)."""
@@ -492,8 +482,7 @@ class TrackingGraphSession:
         self.out = dict(rgb=z(R, 3), depth=z(R), disp=z(R), acc=z(R), var=z(R), z_vals=z(R, S),
                         raw=z(R, S, 4))
         self.losses = z(4)
-        self.ws = torch.empty(_cabi.lib().xrd_coslam_workspace_bytes(R, S), dtype=torch.uint8,
-                              device=dev)
+        self.ws, self.ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
         # per-iteration scalars: [seed u64 | pad | (lr, bc1, bc2) rot | (lr, bc1, bc2) trans]
         self.dyn = torch.zeros(64, dtype=torch.uint8, device=dev)
         self._dyn_ring = [torch.zeros(64, dtype=torch.uint8).pin_memory() for _ in range(8)]
@@ -508,7 +497,7 @@ class TrackingGraphSession:
                 self._sequence(torch.cuda.current_stream(dev).cuda_stream, warm=False)
 
     def _sequence(self, stream, warm):
-        a, model, cfg, lib = self.algo, self.model, self.model.config, _cabi.lib()
+        a, model, cfg = self.algo, self.model, self.model.config
         cam, R = a.camera, self.R
         He, We = a.config.tracking_Hedge, a.config.tracking_Wedge
         S = cfg.training_n_sample_d + cfg.training_n_range_d
@@ -519,14 +508,12 @@ class TrackingGraphSession:
                                      cam.width - We, cam.fx, cam.fy, cam.cx, cam.cy)
         dp = (C.c_void_p * 1)(ptr(self.depth_img))
         cp = (C.c_void_p * 1)(ptr(self.rgb_img))
-        check('xrd_sample_pixels', lib.xrd_sample_pixels(
-            C.byref(pc), dp, cp, ptr(self.idx), ptr(self.dirs), ptr(self.td2), ptr(self.ts),
-            ptr(self.ids), None, stream))
-        check('xrd_pose_matrices',
-              lib.xrd_pose_matrices(1, ptr(self.rot), ptr(self.trans), ptr(self.poses), stream))
-        check('xrd_rays_from_poses',
-              lib.xrd_rays_from_poses(R, ptr(self.dirs), None, ptr(self.poses), 1,
-                                      ptr(self.rays_o), ptr(self.rays_d), stream))
+        launch('xrd_sample_pixels', C.byref(pc), dp, cp, ptr(self.idx), ptr(self.dirs),
+               ptr(self.td2), ptr(self.ts), ptr(self.ids), None, stream=stream)
+        launch('xrd_pose_matrices', 1, ptr(self.rot), ptr(self.trans), ptr(self.poses),
+               stream=stream)
+        launch('xrd_rays_from_poses', R, ptr(self.dirs), None, ptr(self.poses), 1,
+               ptr(self.rays_o), ptr(self.rays_d), stream=stream)
         rays = XrdRays(R, ptr(self.rays_o), ptr(self.rays_d), ptr(self.ts), ptr(self.td2))
         grid = model._grid_struct(model.embed_fn.params.detach())
         mlp = XrdCoslamMlp(*(ptr(t.detach()) for t in model._weights()))
@@ -542,16 +529,14 @@ class TrackingGraphSession:
                            ptr(o['var']), ptr(o['z_vals']), ptr(o['raw']), ptr(self.losses))
         gs = XrdCoslamGrads(None, None, None, None, None, ptr(self.d_rays_o), ptr(self.d_rays_d),
                             (C.c_float * 4)(1.0, 1.0, 1.0, 1.0))  # pose-only pass
-        check('xrd_coslam_step',
-              lib.xrd_coslam_step(C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
-                                  C.byref(out), C.byref(gs), ptr(self.ws), self.ws.numel(), stream))
-        check('xrd_rays_pose_grads', lib.xrd_rays_pose_grads(
-            R, ptr(self.dirs), None, 1, ptr(self.d_rays_o), ptr(self.d_rays_d), ptr(self.d_poses),
-            stream))
+        launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
+               C.byref(out), C.byref(gs), ptr(self.ws), self.ws_bytes, stream=stream)
+        launch('xrd_rays_pose_grads', R, ptr(self.dirs), None, 1, ptr(self.d_rays_o),
+               ptr(self.d_rays_d), ptr(self.d_poses), stream=stream)
         self.d_rot.zero_()
         self.d_trans.zero_()
-        check('xrd_pose_matrices_grads', lib.xrd_pose_matrices_grads(
-            1, ptr(self.rot), ptr(self.d_poses), None, ptr(self.d_rot), ptr(self.d_trans), stream))
+        launch('xrd_pose_matrices_grads', 1, ptr(self.rot), ptr(self.d_poses), None,
+               ptr(self.d_rot), ptr(self.d_trans), stream=stream)
         self.loss_total = self.losses.sum()
         # candidate pose = the pose this loss was evaluated at (before the update)
         better = self.loss_total < self.best_loss
@@ -569,7 +554,7 @@ class TrackingGraphSession:
             x.weight_decay = getattr(oo, 'weight_decay', 0)
             x.bias_correction1 = x.bias_correction2 = 1.0
             x.dyn = None if warm else self.dyn.data_ptr() + 16 + 12 * k
-        check('xrd_adam_step', lib.xrd_adam_step(arr, 2, 0, stream))
+        launch('xrd_adam_step', arr, 2, 0, stream=stream)
 
     def begin(self, frame):
         self.depth_img.copy_(self.algo._frame_tensor(frame, 'depth'))

@@ -118,14 +118,9 @@ def frame_ingest(color, depth, fx, fy, cx, cy, distortion=None, png_depth_scale=
         dep = torch.empty(B, h, w, dtype=torch.float32, device=dev)
     else:
         rgb, dep = out
-    L = _cabi.lib()
-    nbytes = L.xrd_frame_ingest_workspace_bytes(cfg)
-    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream(dev).cuda_stream
-    _cabi.check('xrd_frame_ingest',
-                L.xrd_frame_ingest(cfg, _cabi.ptr(color), _cabi.ptr(depth), _cabi.ptr(rgb),
-                                   _cabi.ptr(dep), _cabi.ptr(ws), nbytes, stream))
+    ws, nbytes = _cabi.workspace(dev, 'frame_ingest', cfg)
+    _cabi.launch_on(dev, 'xrd_frame_ingest', cfg, _cabi.ptr(color), _cabi.ptr(depth),
+                    _cabi.ptr(rgb), _cabi.ptr(dep), _cabi.ptr(ws), nbytes)
     return rgb, dep
 
 

@@ -13,15 +13,14 @@ import torch
 
 from . import _cabi
 from ._cabi import (XRD_EVAL_IMAGE_MAX_SIDE, XRD_EVAL_IMAGE_MIN_SIDE, XRD_EVAL_IMAGE_NO_DEPTH,
-                    XRD_EVAL_IMAGE_OUT, check, ptr)
+                    XRD_EVAL_IMAGE_OUT, ptr)
 
 PSNR, SSIM, DEPTH_L1, MSE = range(XRD_EVAL_IMAGE_OUT)
 
 
 def _device(device=None):
     dev = torch.device(device if device is not None else 'cuda:0')
-    if dev.type != 'cuda':
-        raise RuntimeError('xrdslam_b200 has no CPU path: the render metrics run on a CUDA device')
+    _cabi.require_cuda(dev, 'the render metrics')
     return dev
 
 
@@ -55,16 +54,12 @@ def image_metrics(gt_color, gt_depth, color, depth=None, out=None, levels=None):
                          f'{XRD_EVAL_IMAGE_MAX_SIDE}), got {H} x {W}')
     if out is None:
         out = torch.empty(B, XRD_EVAL_IMAGE_OUT, dtype=torch.float64, device=dev)
-    lib = _cabi.lib()
-    nb = lib.xrd_eval_image_workspace_bytes(B, H, W)
-    if nb == 0:
-        raise ValueError(f'render metrics: unsupported batch of {B} frames of {H} x {W}')
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    ws, nb = _cabi.workspace(
+        dev, 'eval_image', B, H, W,
+        error=f'render metrics: unsupported batch of {B} frames of {H} x {W}')
     flags = XRD_EVAL_IMAGE_NO_DEPTH if depth is None else 0
-    with torch.cuda.device(dev):
-        check('xrd_eval_image_metrics', lib.xrd_eval_image_metrics(
-            ptr(gt_color), ptr(color), ptr(gt_depth), ptr(depth), B, H, W, flags, ptr(out),
-            ptr(levels), ptr(ws), nb, torch.cuda.current_stream(dev).cuda_stream))
+    _cabi.launch_on(dev, 'xrd_eval_image_metrics', ptr(gt_color), ptr(color), ptr(gt_depth),
+                    ptr(depth), B, H, W, flags, ptr(out), ptr(levels), ptr(ws), nb)
     return out
 
 

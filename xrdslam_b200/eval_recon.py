@@ -27,9 +27,7 @@ PLOT_STRETCH = 5
 
 def _device(device=None):
     dev = torch.device(device if device is not None else 'cuda:0')
-    if dev.type != 'cuda':
-        raise RuntimeError('xrdslam_b200 has no CPU path: the reconstruction metrics run on a '
-                           'CUDA device')
+    _cabi.require_cuda(dev, 'the reconstruction metrics')
     return dev
 
 
@@ -53,10 +51,6 @@ def load_mesh(mesh):
 
 
 # ---------------------------------------------------------------- kernels ---
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
-
-
 def sample_surface(verts, faces, n, mode, uniforms=None, seed=0, device=None):
     """Area-weighted samples on a triangle mesh: mode XRD_EVAL_TRIMESH (trimesh sample_surface)
     or XRD_EVAL_OPEN3D (open3d sample_points_uniformly).  uniforms DEVICE f32 [n,3] / [n,2] or
@@ -68,10 +62,8 @@ def sample_surface(verts, faces, n, mode, uniforms=None, seed=0, device=None):
         faces = np.zeros((0, 3), np.int32)
     f = (faces if torch.is_tensor(faces) else torch.from_numpy(np.asarray(faces, np.int32))
          ).to(dev, torch.int32).reshape(-1, 3).contiguous()
-    lib = _cabi.lib()
     nF = f.shape[0]
-    nb = lib.xrd_eval_surface_workspace_bytes(nF)
-    ws = torch.empty(max(nb, 1), dtype=torch.uint8, device=dev)
+    ws, nb = _cabi.workspace(dev, 'eval_surface', nF)
     cum = torch.empty(max(nF, 1), dtype=torch.float64, device=dev)
     total = torch.empty(1, dtype=torch.float64, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -82,12 +74,10 @@ def sample_surface(verts, faces, n, mode, uniforms=None, seed=0, device=None):
         if uniforms.shape != (n, 3 if mode == XRD_EVAL_TRIMESH else 2):
             raise ValueError(f'uniforms must be [{n}, {3 if mode == XRD_EVAL_TRIMESH else 2}]')
     with torch.cuda.device(dev):
-        s = _stream(dev)
-        check('xrd_eval_surface_prepare', lib.xrd_eval_surface_prepare(
-            ptr(v), v.shape[0], ptr(f), nF, ptr(cum), ptr(total), ptr(status), ptr(ws), nb, s))
-        check('xrd_eval_sample_surface', lib.xrd_eval_sample_surface(
-            ptr(v), ptr(f), nF, ptr(cum), ptr(total), ptr(status), mode, n, ptr(uniforms),
-            seed, ptr(out), ptr(fid), s))
+        _cabi.launch_on(dev, 'xrd_eval_surface_prepare', ptr(v), v.shape[0], ptr(f), nF, ptr(cum),
+                        ptr(total), ptr(status), ptr(ws), nb)
+        _cabi.launch_on(dev, 'xrd_eval_sample_surface', ptr(v), ptr(f), nF, ptr(cum), ptr(total),
+                        ptr(status), mode, n, ptr(uniforms), seed, ptr(out), ptr(fid))
         check('xrd_eval_surface_prepare', int(status.item()))
     return out, fid
 
@@ -106,20 +96,16 @@ class NNIndex:
             raise ValueError('the nearest-neighbour index needs at least one target point')
         lo, hi = torch.aminmax(self.points, dim=0)
         box = torch.stack([lo, hi]).double().cpu().numpy()
-        lib = _cabi.lib()
         I = XrdNnIndex()
-        check('xrd_nn_layout', lib.xrd_nn_layout(
-            n, (C.c_double * 3)(*box[0]), (C.c_double * 3)(*box[1]), C.byref(I)))
+        _cabi.call('xrd_nn_layout', n, (C.c_double * 3)(*box[0]), (C.c_double * 3)(*box[1]),
+                   C.byref(I))
         self.cell_ptr = torch.empty(I.n_cells + 1, dtype=torch.int32, device=dev)
         self.occ = torch.empty(max(I.occ_bytes, 1), dtype=torch.uint8, device=dev)
         self.sorted = torch.empty(n, 4, dtype=torch.float32, device=dev)
         I.cell_ptr, I.occ, I.sorted = ptr(self.cell_ptr), ptr(self.occ), ptr(self.sorted)
         self.index = I
-        nb = lib.xrd_nn_build_workspace_bytes(C.byref(I))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            check('xrd_nn_build', lib.xrd_nn_build(ptr(self.points), C.byref(I), ptr(ws), nb,
-                                                   _stream(dev)))
+        ws, nb = _cabi.workspace(dev, 'nn_build', C.byref(I))
+        _cabi.launch_on(dev, 'xrd_nn_build', ptr(self.points), C.byref(I), ptr(ws), nb)
 
     def query(self, queries, radius=None):
         """-> (dist f32 [Q], ids i32 [Q]) on the device; with a radius, targets further than it
@@ -127,36 +113,26 @@ class NNIndex:
         q = _pts(queries, self.device)
         dist = torch.empty(q.shape[0], dtype=torch.float32, device=self.device)
         ids = torch.empty(q.shape[0], dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            check('xrd_nn_query', _cabi.lib().xrd_nn_query(
-                C.byref(self.index), ptr(q), q.shape[0], float(radius or 0.0), ptr(dist),
-                ptr(ids), _stream(self.device)))
+        _cabi.launch_on(self.device, 'xrd_nn_query', C.byref(self.index), ptr(q), q.shape[0],
+                        float(radius or 0.0), ptr(dist), ptr(ids))
         return dist, ids
-
-
-def _reduce_ws(n, dev):
-    nb = _cabi.lib().xrd_eval_reduce_workspace_bytes(n)
-    return torch.empty(nb, dtype=torch.uint8, device=dev), nb
 
 
 def dist_stats(d, tau):
     """DEVICE f64 [3]: (sum d, sum d*d, count of d < tau), bit-identical run to run."""
-    ws, nb = _reduce_ws(d.shape[0], d.device)
+    ws, nb = _cabi.workspace(d.device, 'eval_reduce', d.shape[0])
     out = torch.empty(3, dtype=torch.float64, device=d.device)
-    with torch.cuda.device(d.device):
-        check('xrd_eval_dist_stats', _cabi.lib().xrd_eval_dist_stats(
-            ptr(d), d.shape[0], float(tau), ptr(out), ptr(ws), nb, _stream(d.device)))
+    _cabi.launch_on(d.device, 'xrd_eval_dist_stats', ptr(d), d.shape[0], float(tau), ptr(out),
+                    ptr(ws), nb)
     return out
 
 
 def icp_stats(src, tgt, ids, dist):
     """DEVICE f64 [17]: (count, sum s, sum t, sum s t^T, sum d*d) over the correspondences."""
-    ws, nb = _reduce_ws(src.shape[0], src.device)
+    ws, nb = _cabi.workspace(src.device, 'eval_reduce', src.shape[0])
     out = torch.empty(17, dtype=torch.float64, device=src.device)
-    with torch.cuda.device(src.device):
-        check('xrd_eval_icp_stats', _cabi.lib().xrd_eval_icp_stats(
-            ptr(src), ptr(tgt), ptr(ids), ptr(dist), src.shape[0], ptr(out), ptr(ws), nb,
-            _stream(src.device)))
+    _cabi.launch_on(src.device, 'xrd_eval_icp_stats', ptr(src), ptr(tgt), ptr(ids), ptr(dist),
+                    src.shape[0], ptr(out), ptr(ws), nb)
     return out
 
 
@@ -164,10 +140,8 @@ def transform(points, T):
     """fp32(T applied in f64) to DEVICE points [n,3]; T a 4x4 (rows 0..2 used)."""
     T = np.ascontiguousarray(np.asarray(T, np.float64)[:3, :4]).reshape(-1)
     out = torch.empty_like(points)
-    with torch.cuda.device(points.device):
-        check('xrd_eval_transform', _cabi.lib().xrd_eval_transform(
-            ptr(points), points.shape[0], (C.c_double * 12)(*T), ptr(out),
-            _stream(points.device)))
+    _cabi.launch_on(points.device, 'xrd_eval_transform', ptr(points), points.shape[0],
+                    (C.c_double * 12)(*T), ptr(out))
     return out
 
 
@@ -542,9 +516,8 @@ def points_seen(points, c2w, W=RENDER_W, H=RENDER_H, fx=RENDER_FOCAL, fy=RENDER_
     w2c = w2c.to(dev)
     seen = torch.empty(len(c), dtype=torch.uint8, device=dev)
     cam = _camera(0.0, H, W, fx, fy, cx, cy, 1.0)
-    with torch.cuda.device(dev):
-        check('xrd_eval_points_seen', _cabi.lib().xrd_eval_points_seen(
-            ptr(p), p.shape[0], ptr(w2c), len(c), C.byref(cam), ptr(seen), _stream(dev)))
+    _cabi.launch_on(dev, 'xrd_eval_points_seen', ptr(p), p.shape[0], ptr(w2c), len(c),
+                    C.byref(cam), ptr(seen))
     return seen.cpu().numpy().astype(bool)
 
 
@@ -604,10 +577,8 @@ class DepthRenderer:
             near = NEAR_FRACTION * float((hi - lo).max())
         self.camera = _camera(near, H, W, fx, fy, cx, cy, far)
         self.B = _cabi.XRD_EVAL_RENDER_MAX_VIEWS
-        self.ws_bytes = _cabi.lib().xrd_eval_render_workspace_bytes(self.faces.shape[0], self.B)
-        if self.ws_bytes == 0:
-            raise ValueError('the depth renderer needs at least one face')
-        self.ws = torch.empty(self.ws_bytes, dtype=torch.uint8, device=dev)
+        self.ws, self.ws_bytes = _cabi.workspace(dev, 'eval_render', self.faces.shape[0], self.B,
+                                                 error='the depth renderer needs at least one face')
 
     def render(self, w2c, out=None, status=None):
         """w2c [n,3,4] or [n,4,4] (host f64 or DEVICE) -> DEVICE depth f32 [n,H,W].  status: a
@@ -622,15 +593,12 @@ class DepthRenderer:
         own = status is None
         if own:
             status = torch.zeros(max(1, -(-n // self.B)), dtype=torch.int32, device=self.device)
-        lib = _cabi.lib()
-        with torch.cuda.device(self.device):
-            s = _stream(self.device)
-            for k, b0 in enumerate(range(0, n, self.B)):
-                nb = min(self.B, n - b0)
-                check('xrd_eval_render_depth', lib.xrd_eval_render_depth(
-                    ptr(self.verts), self.verts.shape[0], ptr(self.faces), self.faces.shape[0],
-                    ptr(W[b0:b0 + nb]), nb, C.byref(cam), ptr(out[b0:b0 + nb]),
-                    ptr(status[k:k + 1]), ptr(self.ws), self.ws_bytes, s))
+        for k, b0 in enumerate(range(0, n, self.B)):
+            nb = min(self.B, n - b0)
+            _cabi.launch_on(self.device, 'xrd_eval_render_depth', ptr(self.verts),
+                            self.verts.shape[0], ptr(self.faces), self.faces.shape[0],
+                            ptr(W[b0:b0 + nb]), nb, C.byref(cam), ptr(out[b0:b0 + nb]),
+                            ptr(status[k:k + 1]), ptr(self.ws), self.ws_bytes)
         if own:
             _check_status(status)
         return out
@@ -647,9 +615,8 @@ def depth_l1_sums(gt, rec):
     run (xrd_eval_depth_l1)."""
     n = gt.shape[0]
     out = torch.empty(n, 2, dtype=torch.float64, device=gt.device)
-    with torch.cuda.device(gt.device):
-        check('xrd_eval_depth_l1', _cabi.lib().xrd_eval_depth_l1(
-            ptr(gt), ptr(rec), n, gt[0].numel() if n else 0, ptr(out), _stream(gt.device)))
+    _cabi.launch_on(gt.device, 'xrd_eval_depth_l1', ptr(gt), ptr(rec), n,
+                    gt[0].numel() if n else 0, ptr(out))
     return out
 
 

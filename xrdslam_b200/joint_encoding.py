@@ -28,7 +28,7 @@ from torch.nn import Parameter
 
 from . import _cabi
 from ._cabi import (XrdCoslamCfg, XrdCoslamGrads, XrdCoslamMlp, XrdCoslamOut,
-                    XrdHashGrid, XrdRays, check, ptr)
+                    XrdHashGrid, XrdRays, ptr)
 from .base_model import Model, ModelConfig, scale_grads, upstream_scale
 
 
@@ -89,11 +89,8 @@ class HashGridParams(nn.Module):
                  per_level_scale, seed=1337):
         super().__init__()
         g = XrdHashGrid()
-        check('xrd_hashgrid_layout',
-              _cabi.lib().xrd_hashgrid_layout(C.byref(g), n_levels,
-                                              log2_hashmap_size,
-                                              base_resolution,
-                                              float(np.float32(per_level_scale))))
+        _cabi.call('xrd_hashgrid_layout', C.byref(g), n_levels, log2_hashmap_size,
+                   base_resolution, float(np.float32(per_level_scale)))
         self.layout = g
         self.n_levels = n_levels
         self.n_output_dims = 2 * n_levels
@@ -274,10 +271,7 @@ class JointEncoding(Model):
                 loss_scale=None, seed=None, map_grads=True):
         cfg = self.config
         dev = table.device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on '
-                               'a CUDA (sm_90) device')
-        lib = _cabi.lib()
+        _cabi.require_cuda(dev, 'model')
         f32 = dict(dtype=torch.float32, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()
         rays_d = rays_d.detach().to(**f32).contiguous()
@@ -340,47 +334,35 @@ class JointEncoding(Model):
                                 ptr(g['d_w_sdf1']), ptr(g['d_w_col0']),
                                 ptr(g['d_w_col1']), ptr(g['d_rays_o']),
                                 ptr(g['d_rays_d']), (C.c_float * 4)(*sc))
-        ws_bytes = lib.xrd_coslam_workspace_bytes(R, S)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            if dp is not None:
-                # sharded mapping: the loss normalisers are batch-global (SURVEY Q9):
-                # sample -> all-reduce the three counters -> render with the global counts
-                counts = torch.zeros(4, dtype=torch.int32, device=dev)
-                c.phase, c.counts_out = 1, ptr(counts)
-                st = lib.xrd_coslam_step(C.byref(rays), C.byref(grid), C.byref(mlp),
-                                         C.byref(c), ptr(noise), C.byref(out), None,
-                                         ptr(ws), ws_bytes, stream)
-                check('xrd_coslam_step[sample]', st)
-                dp.all_reduce_sum(counts)
-                c.phase, c.counts_global = 2, ptr(counts)
-                c.n_rays_global = R * dp.world  # equal shards
-            st = lib.xrd_coslam_step(C.byref(rays), C.byref(grid), C.byref(mlp),
-                                     C.byref(c), ptr(noise), C.byref(out),
-                                     C.byref(gs) if gs is not None else None,
-                                     ptr(ws), ws_bytes, stream)
-        check('xrd_coslam_step', st)
+        ws, ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
+
+        def step(grads):
+            _cabi.launch_on(dev, 'xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp),
+                            C.byref(c), ptr(noise), C.byref(out), grads, ptr(ws), ws_bytes)
+        if dp is not None:
+            # sharded mapping: the loss normalisers are batch-global (SURVEY Q9):
+            # sample -> all-reduce the three counters -> render with the global counts
+            counts = torch.zeros(4, dtype=torch.int32, device=dev)
+            c.phase, c.counts_out = 1, ptr(counts)
+            step(None)
+            dp.all_reduce_sum(counts)
+            c.phase, c.counts_global = 2, ptr(counts)
+            c.n_rays_global = R * dp.world  # equal shards
+        step(C.byref(gs) if gs is not None else None)
         self._last_seed = seed
         return o, g
 
     def _launch_smooth(self, table, rand6, need_grad, weight=1.0):
         cfg = self.config
-        lib = _cabi.lib()
         dev = table.device
         grid = self._grid_struct(table.detach())
         loss = torch.zeros(1, dtype=torch.float32, device=dev)
         d_table = torch.zeros_like(table) if need_grad else None
         r = (C.c_float * 6)(*[float(v) for v in rand6])
-        nb = lib.xrd_coslam_smoothness_workspace_bytes(cfg.trainging_smooth_pts)
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_coslam_smoothness(
-                C.byref(grid), cfg.trainging_smooth_pts,
-                cfg.trainging_smooth_vox, cfg.trainging_smooth_margin, weight,
-                r, ptr(loss), ptr(d_table), 1.0, ptr(ws), nb,
-                torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_coslam_smoothness', st)
+        ws, nb = _cabi.workspace(dev, 'coslam_smoothness', cfg.trainging_smooth_pts)
+        _cabi.launch_on(dev, 'xrd_coslam_smoothness', C.byref(grid), cfg.trainging_smooth_pts,
+                        cfg.trainging_smooth_vox, cfg.trainging_smooth_margin, weight, r,
+                        ptr(loss), ptr(d_table), 1.0, ptr(ws), nb)
         return loss[0], d_table
 
     # --------------------------------------------------------- Model API ---
@@ -460,8 +442,7 @@ class JointEncoding(Model):
         """xrd_coslam_query on [..., 3] points -> dict of flat [P, k] tensors (inference)."""
         table = self.embed_fn.params
         dev = table.device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on a CUDA device')
+        _cabi.require_cuda(dev, 'model')
         flat = pts.detach().reshape(-1, 3).to(device=dev, dtype=torch.float32).contiguous()
         P = flat.shape[0]
         f32 = dict(dtype=torch.float32, device=dev)
@@ -470,11 +451,8 @@ class JointEncoding(Model):
         feat = torch.empty(P, 32, **f32) if want_feat else None
         grid = self._grid_struct(table.detach())
         mlp = XrdCoslamMlp(*(ptr(w.detach()) for w in self._weights()))
-        with torch.cuda.device(dev):
-            st = _cabi.lib().xrd_coslam_query(C.byref(grid), C.byref(mlp), ptr(flat), P,
-                                              int(normalised), ptr(raw), ptr(geo), ptr(feat),
-                                              torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_coslam_query', st)
+        _cabi.launch_on(dev, 'xrd_coslam_query', C.byref(grid), C.byref(mlp), ptr(flat), P,
+                        int(normalised), ptr(raw), ptr(geo), ptr(feat))
         return dict(raw=raw, geo=geo, feat=feat)
 
     def query_fn(self, pi):

@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from ._cabi import XrdMeshAffine, check, ptr
+from ._cabi import XrdMeshAffine, ptr
 from .base_model import InstantiateConfig
 
 
@@ -52,16 +52,13 @@ def marching_cubes(values, level, spacing, shift=(0.0, 0.0, 0.0), scale=(1.0, 1.
     """csrc/mesh.cu on DEVICE values f32 [B,nx,ny,nz] -> DEVICE verts f32 [V,3], faces i32 [F,3].
     World coordinates ((p * spacing + shift) * scale) + origin[b] (fp32), origin [B,3] or None;
     semantics in include/xrdslam_b200.h.  One host read: the two totals."""
-    if values.device.type != 'cuda':
-        raise RuntimeError('xrdslam_b200 has no CPU path: values must be on a CUDA device')
-    lib = _cabi.lib()
+    _cabi.require_cuda(values.device, 'values')
     dev = values.device
     vals = values.detach().to(torch.float32).contiguous()
     B, nx, ny, nz = vals.shape
-    nb = lib.xrd_mesh_mc_workspace_bytes(B, nx, ny, nz)
-    if nb == 0:
-        raise ValueError(f'marching cubes needs B >= 1 and nx, ny, nz >= 2, got {tuple(vals.shape)}')
-    ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    ws, nb = _cabi.workspace(
+        dev, 'mesh_mc', B, nx, ny, nz,
+        error=f'marching cubes needs B >= 1 and nx, ny, nz >= 2, got {tuple(vals.shape)}')
     counts = torch.empty(2, dtype=torch.int32, device=dev)
     org = None if origin is None else origin.detach().to(dev, torch.float32).contiguous()
     if org is not None and tuple(org.shape) != (B, 3):
@@ -69,15 +66,13 @@ def marching_cubes(values, level, spacing, shift=(0.0, 0.0, 0.0), scale=(1.0, 1.
     f3 = lambda a: (C.c_float * 3)(*[float(x) for x in a])
     aff = XrdMeshAffine(f3(spacing), f3(shift), f3(scale), ptr(org))
     with torch.cuda.device(dev):
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        check('xrd_mesh_mc_count', lib.xrd_mesh_mc_count(ptr(vals), B, nx, ny, nz, float(level),
-                                                         ptr(counts), ptr(ws), nb, stream))
+        _cabi.launch_on(dev, 'xrd_mesh_mc_count', ptr(vals), B, nx, ny, nz, float(level),
+                        ptr(counts), ptr(ws), nb)
         V, F = counts.tolist()
         verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
         faces = torch.empty(F, 3, dtype=torch.int32, device=dev)
-        check('xrd_mesh_mc_emit', lib.xrd_mesh_mc_emit(ptr(vals), B, nx, ny, nz, float(level),
-                                                       C.byref(aff), ptr(verts), ptr(faces),
-                                                       ptr(ws), nb, stream))
+        _cabi.launch_on(dev, 'xrd_mesh_mc_emit', ptr(vals), B, nx, ny, nz, float(level),
+                        C.byref(aff), ptr(verts), ptr(faces), ptr(ws), nb)
     return verts, faces
 
 

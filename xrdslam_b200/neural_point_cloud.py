@@ -13,7 +13,7 @@ import torch
 import torch.nn as nn
 
 from . import _cabi
-from ._cabi import XrdPointIndex, check, ptr
+from ._cabi import XrdPointIndex, ptr
 
 
 class NeuralPointCloud(nn.Module):
@@ -64,17 +64,12 @@ class NeuralPointCloud(nn.Module):
         by xrd_pointslam_knn_build (histogram, scan, scatter, per-bucket id sort)."""
         N = self._pos.shape[0]
         dev = self.device
-        lib = _cabi.lib()
         i32 = dict(dtype=torch.int32, device=dev)
         start, end = torch.empty(self.table_size, **i32), torch.empty(self.table_size, **i32)
         ids = torch.empty(max(N, 1), **i32)
-        nb = lib.xrd_pointslam_knn_build_workspace_bytes(self.table_size)
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_pointslam_knn_build(ptr(self._pos), N, self.cell, self.table_size, ptr(start),
-                                             ptr(end), ptr(ids), ptr(ws), nb,
-                                             torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_pointslam_knn_build', st)
+        ws, nb = _cabi.workspace(dev, 'pointslam_knn_build', self.table_size)
+        _cabi.launch_on(dev, 'xrd_pointslam_knn_build', ptr(self._pos), N, self.cell,
+                        self.table_size, ptr(start), ptr(end), ptr(ids), ptr(ws), nb)
         self._index = dict(sorted_ids=ids, cell_start=start, cell_end=end, n=N)
 
     def rebuild_index_torch(self):
@@ -119,11 +114,8 @@ class NeuralPointCloud(nn.Module):
             D.fill_(torch.finfo(torch.float32).max); I.fill_(-1); n.zero_()
             return D, I, n
         ix = self.index_struct()
-        with torch.cuda.device(self.device):
-            st = _cabi.lib().xrd_pointslam_knn_query(
-                C.byref(ix), ptr(pos), ptr(radius), stride, P, ptr(D), ptr(I), ptr(n),
-                torch.cuda.current_stream(self.device).cuda_stream)
-        check('xrd_pointslam_knn_query', st)
+        _cabi.launch_on(self.device, 'xrd_pointslam_knn_query', C.byref(ix), ptr(pos), ptr(radius),
+                        stride, P, ptr(D), ptr(I), ptr(n))
         return D, I, n
 
     # ---- map update (neural_point_cloud.py:109-221) -----------------------------

@@ -56,10 +56,7 @@ class FusedAdam(torch.optim.Optimizer):
                 assert mask.is_cuda and mask.dtype == torch.uint8 and mask.is_contiguous() and \
                     p.numel() % mask.numel() == 0
                 a.row_mask, a.row_len = mask.data_ptr(), p.numel() // mask.numel()
-        with torch.cuda.device(dev):
-            rc = _cabi.lib().xrd_adam_step(arr, len(descs), 0,
-                                           torch.cuda.current_stream(dev).cuda_stream)
-        _cabi.check('xrd_adam_step', rc)
+        _cabi.launch_on(dev, 'xrd_adam_step', arr, len(descs), 0)
         return loss
 
 

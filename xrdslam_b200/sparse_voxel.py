@@ -222,7 +222,6 @@ class SparseVoxel(Model):
         """Intersections + samples (device tensors) and the host copy of the 5 stats."""
         cfg = self.config
         dev = self.embeddings.device
-        lib = _cabi.lib()
         R = rays_o.shape[0]
         i32 = dict(dtype=torch.int32, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -241,10 +240,8 @@ class SparseVoxel(Model):
                                                'ray_mask', 'stats')])
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), None, None)
         mp = self._map_struct(self.embeddings.detach())
-        with torch.cuda.device(dev):
-            st = lib.xrd_voxfusion_march(C.byref(rays), C.byref(mp), C.byref(mc), ptr(noise),
-                                         C.byref(ms), torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_voxfusion_march', st)
+        _cabi.launch_on(dev, 'xrd_voxfusion_march', C.byref(rays), C.byref(mp), C.byref(mc),
+                        ptr(noise), C.byref(ms))
         stats = m['stats'][:8].cpu().tolist()  # the one host read (reference: hits.sum() == 0)
         m['_cfg'], m['_struct'] = mc, ms
         m['n_hit_rays'], m['n_points'], m['s_max'], m['p_max'], m['overflow'] = stats[:5]
@@ -254,11 +251,9 @@ class SparseVoxel(Model):
                 need_map=False):
         cfg = self.config
         dev = self.embeddings.device
-        if dev.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: model must be on a CUDA device')
+        _cabi.require_cuda(dev, 'model')
         if self.map_states is None:
             raise RuntimeError('empty map: call insert_points first')
-        lib = _cabi.lib()
         f32 = dict(dtype=torch.float32, device=dev)
         rays_o = rays_o.detach().to(**f32).contiguous()
         rays_d = rays_d.detach().to(**f32).contiguous()
@@ -298,31 +293,23 @@ class SparseVoxel(Model):
                 keep.append(dg)
                 gs.d_decoder = C.pointer(dg)
             gs.d_rays_o, gs.d_rays_d = ptr(g['d_rays_o']), ptr(g['d_rays_d'])
-        nb = lib.xrd_voxfusion_render_workspace_bytes(R, m['n_points'], int(with_grads))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            st = lib.xrd_voxfusion_render(C.byref(rays), C.byref(mp), C.byref(m['_struct']),
-                                          C.byref(m['_cfg']), C.byref(dec), C.byref(rc),
-                                          C.byref(out), C.byref(gs) if gs is not None else None,
-                                          ptr(ws), nb, torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_voxfusion_render', st)
+        ws, nb = _cabi.workspace(dev, 'voxfusion_render', R, m['n_points'], int(with_grads))
+        _cabi.launch_on(dev, 'xrd_voxfusion_render', C.byref(rays), C.byref(mp),
+                        C.byref(m['_struct']), C.byref(m['_cfg']), C.byref(dec), C.byref(rc),
+                        C.byref(out), C.byref(gs) if gs is not None else None, ptr(ws), nb)
         return o, g
 
     # ------------------------------------------------ mesh-extraction queries ---
     QUERY_POINTS = 1 << 18  # points per xrd_voxfusion_query call (~0.55 GB of activations)
 
     def _query(self, n, vox, res=0, lin=None, xyz=None, sdf=None, rgb=None, ws=None):
-        lib = _cabi.lib()
         dev = self.embeddings.device
         dts = [t.detach() for t in self.decoder.tensors()]
         dec = _dec_struct(dts, XrdVoxDecoder)
         mp = self._map_struct(self.embeddings.detach())
-        with torch.cuda.device(dev):
-            st = lib.xrd_voxfusion_query(C.byref(mp), C.byref(dec), self.config.voxel_size, n,
-                                         ptr(vox), res, ptr(lin), ptr(xyz), ptr(sdf), ptr(rgb),
-                                         ptr(ws), ws.numel(),
-                                         torch.cuda.current_stream(dev).cuda_stream)
-        check('xrd_voxfusion_query', st)
+        _cabi.launch_on(dev, 'xrd_voxfusion_query', C.byref(mp), C.byref(dec),
+                        self.config.voxel_size, n, ptr(vox), res, ptr(lin), ptr(xyz), ptr(sdf),
+                        ptr(rgb), ptr(ws), ws.numel())
 
     def get_scores(self, vox_ids, res=8):
         """voxel_helpers_voxfusion.py:15-59: sdf f32 [B,res,res,res] on the lattice
@@ -334,8 +321,7 @@ class SparseVoxel(Model):
         lin = torch.linspace(-.5, .5, res).to(dev)  # torch's symmetric fp32 linspace, on the host
         sdf = torch.empty(B, res, res, res, dtype=torch.float32, device=dev)
         per = max(1, self.QUERY_POINTS // res ** 3)
-        nb = _cabi.lib().xrd_voxfusion_query_workspace_bytes(min(B, per) * res ** 3)
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        ws, _ = _cabi.workspace(dev, 'voxfusion_query', min(B, per) * res ** 3)
         for s in range(0, B, per):
             c = min(per, B - s)
             self._query(c, ids[s:s + c], res, lin, sdf=sdf[s:s + c], ws=ws)
@@ -350,8 +336,7 @@ class SparseVoxel(Model):
         P = pts.shape[0]
         rgb = torch.empty(P, 3, dtype=torch.float32, device=dev)
         per = self.QUERY_POINTS
-        nb = _cabi.lib().xrd_voxfusion_query_workspace_bytes(min(P, per))
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        ws, _ = _cabi.workspace(dev, 'voxfusion_query', min(P, per))
         for s in range(0, P, per):
             c = min(per, P - s)
             self._query(c, ids[s:s + c], xyz=pts[s:s + c], rgb=rgb[s:s + c], ws=ws)

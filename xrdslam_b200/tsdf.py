@@ -16,14 +16,10 @@ import numpy as np
 import torch
 
 from . import _cabi
-from ._cabi import XrdTsdfParams, check, ptr
+from ._cabi import XrdTsdfParams, ptr
 
 BLOCK_RES = 16
 BLOCK_VOXELS = BLOCK_RES ** 3
-
-
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
 
 
 class TSDFVolume:
@@ -39,8 +35,7 @@ class TSDFVolume:
         self.depth_trunc = float(depth_trunc)
         self.stride = int(stride)
         self.device = torch.device(device)
-        if self.device.type != 'cuda':
-            raise RuntimeError('xrdslam_b200 has no CPU path: the TSDF volume lives on a CUDA device')
+        _cabi.require_cuda(self.device, 'the TSDF volume')
         self.keys = torch.empty(0, dtype=torch.int64, device=self.device)
         self.tsdf = torch.empty(0, dtype=torch.float32, device=self.device)
         self.weight = torch.empty(0, dtype=torch.float32, device=self.device)
@@ -59,26 +54,23 @@ class TSDFVolume:
     def allocate(self, depth, c2w, intrinsic):
         """The blocks a batch touches: keys i64 [n] (sorted) and touched-frame masks i32
         [n, ceil(K/32)] (u32 bit patterns), on the device."""
-        lib = _cabi.lib()
         dev = self.device
         K, H, W = depth.shape
         P = self._params(intrinsic)
-        nb = lib.xrd_tsdf_alloc_workspace_bytes(K, H, W, self.stride)
-        if nb == 0:
-            raise ValueError(f'TSDF allocation: unsupported batch shape {tuple(depth.shape)}')
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        ws, nb = _cabi.workspace(
+            dev, 'tsdf_alloc', K, H, W, self.stride,
+            error=f'TSDF allocation: unsupported batch shape {tuple(depth.shape)}')
         cnt = torch.empty(1, dtype=torch.int32, device=dev)
         words = (K + 31) // 32
         with torch.cuda.device(dev):
-            s = _stream(dev)
-            check('xrd_tsdf_alloc_count', lib.xrd_tsdf_alloc_count(
-                ptr(depth), ptr(c2w), K, H, W, C.byref(P), ptr(cnt), ptr(ws), nb, s))
+            _cabi.launch_on(dev, 'xrd_tsdf_alloc_count', ptr(depth), ptr(c2w), K, H, W,
+                            C.byref(P), ptr(cnt), ptr(ws), nb)
             n = int(cnt.item())
             keys = torch.empty(n, dtype=torch.int64, device=dev)
             masks = torch.empty(n, words, dtype=torch.int32, device=dev)
             if n:
-                check('xrd_tsdf_alloc_emit', lib.xrd_tsdf_alloc_emit(
-                    K, H, W, C.byref(P), n, ptr(keys), ptr(masks), ptr(ws), nb, s))
+                _cabi.launch_on(dev, 'xrd_tsdf_alloc_emit', K, H, W, C.byref(P), n, ptr(keys),
+                                ptr(masks), ptr(ws), nb)
         return keys, masks
 
     def _grow(self, keys):
@@ -126,38 +118,32 @@ class TSDFVolume:
         all_masks = torch.zeros(self.n_blocks, masks.shape[1], dtype=torch.int32, device=dev)
         all_masks[rows] = masks
         P = self._params(intrinsic)
-        with torch.cuda.device(dev):
-            check('xrd_tsdf_integrate', _cabi.lib().xrd_tsdf_integrate(
-                ptr(self.keys), ptr(all_masks), self.n_blocks, ptr(depth), ptr(color), ptr(w2c_d),
-                K, H, W, C.byref(P), ptr(self.tsdf), ptr(self.weight), ptr(self.color),
-                _stream(dev)))
+        _cabi.launch_on(dev, 'xrd_tsdf_integrate', ptr(self.keys), ptr(all_masks), self.n_blocks,
+                        ptr(depth), ptr(color), ptr(w2c_d), K, H, W, C.byref(P), ptr(self.tsdf),
+                        ptr(self.weight), ptr(self.color))
 
     def extract_triangle_mesh(self):
         """-> DEVICE verts f32 [V,3], faces i32 [F,3], colors f32 [V,3] in [0,1] (nominally).
         One host read: the two totals."""
         dev = self.device
-        lib = _cabi.lib()
         if self.n_blocks == 0:
             return (torch.empty(0, 3, device=dev), torch.empty(0, 3, dtype=torch.int32, device=dev),
                     torch.empty(0, 3, device=dev))
-        nb = lib.xrd_tsdf_mc_workspace_bytes(self.n_blocks)
-        if nb == 0:
-            raise ValueError(f'TSDF volume of {self.n_blocks} blocks is too large to mesh')
-        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        ws, nb = _cabi.workspace(
+            dev, 'tsdf_mc', self.n_blocks,
+            error=f'TSDF volume of {self.n_blocks} blocks is too large to mesh')
         counts = torch.empty(2, dtype=torch.int32, device=dev)
         P = self._params(self._intrinsic)
         with torch.cuda.device(dev):
-            s = _stream(dev)
-            check('xrd_tsdf_mc_count', lib.xrd_tsdf_mc_count(
-                ptr(self.keys), self.n_blocks, ptr(self.tsdf), ptr(self.weight), ptr(counts),
-                ptr(ws), nb, s))
+            _cabi.launch_on(dev, 'xrd_tsdf_mc_count', ptr(self.keys), self.n_blocks, ptr(self.tsdf),
+                            ptr(self.weight), ptr(counts), ptr(ws), nb)
             V, F = counts.tolist()
             verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
             colors = torch.empty(V, 3, dtype=torch.float32, device=dev)
             faces = torch.empty(F, 3, dtype=torch.int32, device=dev)
-            check('xrd_tsdf_mc_emit', lib.xrd_tsdf_mc_emit(
-                ptr(self.keys), self.n_blocks, ptr(self.tsdf), ptr(self.color), C.byref(P),
-                ptr(verts), ptr(colors), ptr(faces), ptr(ws), nb, s))
+            _cabi.launch_on(dev, 'xrd_tsdf_mc_emit', ptr(self.keys), self.n_blocks, ptr(self.tsdf),
+                            ptr(self.color), C.byref(P), ptr(verts), ptr(colors), ptr(faces),
+                            ptr(ws), nb)
         return verts, faces, colors
 
 
@@ -174,9 +160,8 @@ def components(faces, n_verts):
     dev = faces.device
     faces = faces.to(torch.int32).contiguous()
     labels = torch.empty(n_verts, dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        check('xrd_tsdf_components', _cabi.lib().xrd_tsdf_components(
-            ptr(faces), int(faces.shape[0]), int(n_verts), ptr(labels), _stream(dev)))
+    _cabi.launch_on(dev, 'xrd_tsdf_components', ptr(faces), int(faces.shape[0]), int(n_verts),
+                    ptr(labels))
     return labels
 
 
