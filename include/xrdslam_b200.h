@@ -1059,6 +1059,21 @@ int xrd_frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color, const uint16
                      float* rgb, float* depth_out, void* workspace, size_t workspace_bytes,
                      void* stream);
 
+/*   xrd_frame_ingest_f32  the same for float32 depth (CoFusion's OpenEXR depth_noise frames):
+ *                         slam/common/datasets.py:20-52 readEXR_onlydepth's 'Y' channel through
+ *                         :98-101 and the rest of __getitem__.
+ *
+ * depth DEVICE float32 [B][Hd][Wd]; every other argument, the workspace
+ * (xrd_frame_ingest_workspace_bytes), the status codes and stages 1, 2 and 4-7 are those of
+ * xrd_frame_ingest.  Stage 3 is depth = d / f32(png_depth_scale) in f32, numpy's
+ * `depth.astype(np.float32) / png_depth_scale`: infinities, signed zeros, negative and subnormal
+ * values follow IEEE division (no flush to zero), a NaN comes back quietened with its payload
+ * (the depth's first, then the scale's) and an invalid division (inf / inf) gives 0xffc00000, as
+ * x86 division returns them; INTER_NEAREST then copies the values' bits. */
+int xrd_frame_ingest_f32(const XrdIngestCfg* cfg, const uint8_t* color, const float* depth,
+                         float* rgb, float* depth_out, void* workspace, size_t workspace_bytes,
+                         void* stream);
+
 /* ---- Point-SLAM -------------------------------------------------------------
  *
  *   xrd_pointslam_knn_query  slam/model_components/neural_point_cloud.py:223-282

@@ -380,6 +380,8 @@ SYMBOLS = {
                                          vp, vp, C.c_size_t, vp]),
     'xrd_frame_ingest_workspace_bytes': (C.c_size_t, [C.POINTER(XrdIngestCfg)]),
     'xrd_frame_ingest': (C.c_int, [C.POINTER(XrdIngestCfg), vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    'xrd_frame_ingest_f32': (C.c_int, [C.POINTER(XrdIngestCfg), vp, vp, vp, vp, vp, C.c_size_t,
+                                       vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,

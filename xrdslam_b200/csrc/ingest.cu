@@ -1,8 +1,8 @@
-// Frame ingest (sm_90a): decoded uint8 BGR colour and uint16 depth -> the float32 frames the
-// reference's BaseDataset.__getitem__ (slam/common/datasets.py:95-134) produces, stage by stage in
-// the same arithmetic:
+// Frame ingest (sm_90a): decoded uint8 BGR colour and uint16 (PNG) or float32 (EXR) depth -> the
+// float32 frames the reference's BaseDataset.__getitem__ (slam/common/datasets.py:95-134)
+// produces, stage by stage in the same arithmetic:
 //   undistort (colour, uint8; cv::undistort's map and fixed-point remap) -> BGR->RGB, / 255. in
-//   f64 -> depth f32(u16) / f32(scale) -> colour resized to the depth's size (cv2.resize
+//   f64 -> depth f32(d) / f32(scale) -> colour resized to the depth's size (cv2.resize
 //   INTER_LINEAR on f64) -> crop -> downsample (colour INTER_LINEAR, depth INTER_NEAREST) -> f32.
 // Every floating-point operation is an explicit round-to-nearest intrinsic, so nothing is
 // contracted into an FMA: cv2's own C++ code has none.  oracle/ingest.py restates this file.
@@ -176,9 +176,28 @@ struct Stage1 {
   }
 };
 
-// One thread per output pixel: colour (3 channels) and depth.
+// Stage 3 on one depth value: f32(d) / f32(png_depth_scale).  uint16 depth converts exactly.
+__device__ __forceinline__ float depth_div(uint16_t d, float scale) {
+  return __fdiv_rn((float)d, scale);
+}
+
+// float32 depth as numpy divides it on x86 (SSE divss): a NaN operand comes back quietened with
+// its payload (the dividend's first), and an invalid division (inf / inf, 0 / 0) gives x86's
+// default NaN 0xffc00000, where the device's division would return 0x7fffffff in both cases.
+// Infinities, signed zeros and subnormals follow IEEE division, as __fdiv_rn does.
+__device__ __forceinline__ float depth_div(float d, float scale) {
+  constexpr unsigned kQuiet = 0x00400000u, kDefaultNaN = 0xffc00000u;
+  if (isnan(d)) return __uint_as_float(__float_as_uint(d) | kQuiet);
+  if (isnan(scale)) return __uint_as_float(__float_as_uint(scale) | kQuiet);
+  const float q = __fdiv_rn(d, scale);
+  return isnan(q) ? __uint_as_float(kDefaultNaN) : q;
+}
+
+// One thread per output pixel: colour (3 channels) and depth.  DepthT is uint16_t (PNG depth) or
+// float (EXR depth); only stage 3 reads it.
+template <class DepthT>
 __global__ void __launch_bounds__(kThreads)
-k_ingest(const uint8_t* __restrict__ color, const uint16_t* __restrict__ depth, Params P,
+k_ingest(const uint8_t* __restrict__ color, const DepthT* __restrict__ depth, Params P,
          float* __restrict__ rgb, float* __restrict__ depth_out) {
   const long long n = (long long)P.B * P.h * P.w;
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -195,8 +214,8 @@ k_ingest(const uint8_t* __restrict__ color, const uint16_t* __restrict__ depth, 
     dx = min((int)floor(dmul((double)x, P.nn_scale_x)), P.wc - 1);
     dy = min((int)floor(dmul((double)y, P.nn_scale_y)), P.hc - 1);
   }
-  const uint16_t dv = depth[((long long)b * P.Hd + dy + P.edge) * P.Wd + dx + P.edge];
-  depth_out[p] = __fdiv_rn((float)dv, P.depth_scale);
+  const DepthT dv = depth[((long long)b * P.Hd + dy + P.edge) * P.Wd + dx + P.edge];
+  depth_out[p] = depth_div(dv, P.depth_scale);
 }
 
 // cv::resize's scale per axis and its choice of path
@@ -253,9 +272,11 @@ extern "C" size_t xrd_frame_ingest_workspace_bytes(const XrdIngestCfg* cfg) {
   return IngestWs(nullptr, *cfg).bytes();
 }
 
-extern "C" int xrd_frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color,
-                                const uint16_t* depth, float* rgb, float* depth_out,
-                                void* workspace, size_t workspace_bytes, void* stream_) {
+namespace {
+
+template <class DepthT>
+int frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color, const DepthT* depth, float* rgb,
+                 float* depth_out, void* workspace, size_t workspace_bytes, void* stream_) {
   if (!cfg) return XRD_E_NULL;
   Params P;
   if (!params(cfg, &P)) return XRD_E_SHAPE;
@@ -278,7 +299,21 @@ extern "C" int xrd_frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color,
     src = L.undistorted;
   }
   const long long n = (long long)P.B * P.h * P.w;
-  k_ingest<<<blocks(n, kThreads), kThreads, 0, s>>>(src, depth, P, rgb, depth_out);
+  k_ingest<DepthT><<<blocks(n, kThreads), kThreads, 0, s>>>(src, depth, P, rgb, depth_out);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
+}
+
+}  // namespace
+
+extern "C" int xrd_frame_ingest(const XrdIngestCfg* cfg, const uint8_t* color,
+                                const uint16_t* depth, float* rgb, float* depth_out,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  return frame_ingest(cfg, color, depth, rgb, depth_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int xrd_frame_ingest_f32(const XrdIngestCfg* cfg, const uint8_t* color,
+                                    const float* depth, float* rgb, float* depth_out,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  return frame_ingest(cfg, color, depth, rgb, depth_out, workspace, workspace_bytes, stream);
 }

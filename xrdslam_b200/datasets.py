@@ -1,5 +1,6 @@
-"""RGB-D dataset readers (slam/common/datasets.py): the Replica folder layout, decoded on the host
-and turned into float32 device frames by one CUDA call (csrc/ingest.cu, `frame_ingest`).
+"""RGB-D dataset readers (slam/common/datasets.py): the Replica, TUM RGB-D, ScanNet, 7-Scenes,
+Azure Kinect and CoFusion folder layouts, decoded on the host and turned into float32 device
+frames by one CUDA call (csrc/ingest.cu, `frame_ingest`).
 
 `dataset[i]` returns `(i, rgb f32 [h,w,3], depth f32 [h,w], c2w f32 [4,4])` as device tensors,
 the protocol of the reference's BaseDataset.__getitem__ (datasets.py:95-134).  The colour is
@@ -12,8 +13,15 @@ reference's only up to the decoder.  `DECODER` names the one in use.
 
 Iterating a dataset in order prefetches: a host thread decodes frame i + 1 into pinned memory
 while frame i is being used (the reference's DataLoader(num_workers=1), without its float64 host
-work).  Only the Replica layout is read here; other layouts differ in file listing and pose
-parsing and can reuse `frame_ingest`."""
+work).
+
+The readers differ only in file listing, sort order and pose parsing, which follow the reference's
+classes line by line (`dataset_dict`): poses are built in float64 and handed out as float32
+tensors.  Depth is a 16-bit PNG (`xrd_frame_ingest`) or, for CoFusion, the float32 'Y' channel of
+an OpenEXR file read through cv2 (`xrd_frame_ingest_f32`).  Colour that the ingest resizes with
+INTER_LINEAR (ScanNet's and Azure's frames are larger than their depth) equals cv2 built without
+Intel IPP bit for bit; a cv2 built with IPP differs by up to about 2e-6 there.  EuRoC
+(monocular + IMU, read only by DPVO) is not supported."""
 from __future__ import annotations
 
 import glob
@@ -61,6 +69,39 @@ def read_depth(path):
     return img
 
 
+def read_depth_exr(path):
+    """float32 [H,W]: the 'Y' channel of a single-channel OpenEXR file (datasets.py:20-52,
+    readEXR_onlydepth), decoded by cv2 with its OpenEXR codec enabled.  Every bit of the stored
+    values is kept, NaN payloads included.  Raises where the reference's reader returns None."""
+    if cv2 is None:
+        raise RuntimeError(f'{path}: reading OpenEXR depth needs cv2')
+    # cv2 reads this switch once, at its first OpenEXR access; a user's own setting is kept
+    os.environ.setdefault('OPENCV_IO_ENABLE_OPENEXR', '1')
+    try:
+        img = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    except cv2.error as e:
+        raise RuntimeError(f'{path}: cv2 cannot decode OpenEXR ({e}); it needs '
+                           'OPENCV_IO_ENABLE_OPENEXR=1 before its first OpenEXR access') from e
+    if img is None:
+        if not os.path.exists(path):
+            raise FileNotFoundError(path)
+        raise RuntimeError(f'{path}: cv2 could not decode this OpenEXR file')
+    if img.dtype != np.float32 or img.ndim != 2:
+        raise ValueError(f'{path}: expected a single-channel (Y) float32 OpenEXR depth image, got '
+                         f'{img.dtype} {img.shape}')
+    return img
+
+
+def read_depth_any(path):
+    """The depth image of `path` as datasets.py:99-102 picks its decoder (by '.png' / '.exr' in
+    the path): uint16 [H,W] or float32 [H,W]."""
+    if '.png' in path:
+        return read_depth(path)
+    if '.exr' in path:
+        return read_depth_exr(path)
+    raise ValueError(f'{path}: depth must be a .png or an .exr file')
+
+
 def ingest_config(B, color_shape, depth_shape, fx, fy, cx, cy, distortion=None,
                   png_depth_scale=6553.5, crop_edge=0, downsample_factor=1):
     from . import _cabi
@@ -92,14 +133,21 @@ def frame_ingest(color, depth, fx, fy, cx, cy, distortion=None, png_depth_scale=
                  crop_edge=0, downsample_factor=1, out=None):
     """B decoded frames on the device -> (rgb f32 [B,h,w,3], depth f32 [B,h,w]) on the device.
 
-    color: uint8 [B,H0,W0,3] (BGR, cv2.imread's order); depth: uint16 or int16 (same bits)
-    [B,Hd,Wd].  One or two launches on the current stream, no host synchronisation.  `out` may
-    hold preallocated (rgb, depth) tensors."""
+    color: uint8 [B,H0,W0,3] (BGR, cv2.imread's order); depth [B,Hd,Wd]: uint16 or int16 (same
+    bits) from PNG, through xrd_frame_ingest, or float32 from OpenEXR, through
+    xrd_frame_ingest_f32.  One or two launches on the current stream, no host synchronisation.
+    `out` may hold preallocated (rgb, depth) tensors."""
     from . import _cabi
     if color.dim() == 3:
         color, depth = color[None], depth[None]
-    if color.dtype != torch.uint8 or depth.dtype not in (torch.int16, torch.uint16):
-        raise TypeError('frame_ingest needs uint8 colour and 16-bit depth')
+    if depth.dtype == torch.float32:
+        entry = 'xrd_frame_ingest_f32'
+    elif depth.dtype in (torch.int16, torch.uint16):
+        entry = 'xrd_frame_ingest'
+    else:
+        raise TypeError(f'frame_ingest needs 16-bit or float32 depth, got {depth.dtype}')
+    if color.dtype != torch.uint8:
+        raise TypeError(f'frame_ingest needs uint8 colour, got {color.dtype}')
     if color.device.type != 'cuda' or depth.device != color.device:
         raise ValueError('frame_ingest needs both images on the same CUDA device')
     B = color.shape[0]
@@ -119,19 +167,52 @@ def frame_ingest(color, depth, fx, fy, cx, cy, distortion=None, png_depth_scale=
     else:
         rgb, dep = out
     ws, nbytes = _cabi.workspace(dev, 'frame_ingest', cfg)
-    _cabi.launch_on(dev, 'xrd_frame_ingest', cfg, _cabi.ptr(color), _cabi.ptr(depth),
+    _cabi.launch_on(dev, entry, cfg, _cabi.ptr(color), _cabi.ptr(depth),
                     _cabi.ptr(rgb), _cabi.ptr(dep), _cabi.ptr(ws), nbytes)
     return rgb, dep
 
 
+EUROC_UNSUPPORTED = ("the 'euroc' layout (datasets.py:170-173) is monocular images plus IMU "
+                     "(data_format 'MonoImu'), read only by DPVO; none of this package's RGB-D "
+                     'algorithms can consume it')
+
+
 def get_dataset(data_path, data_type, device='cuda:0'):
+    if data_type == 'euroc':
+        raise NotImplementedError(EUROC_UNSUPPORTED)
+    if data_type not in dataset_dict:
+        raise ValueError(f'unknown data_type {data_type!r}; one of {sorted(dataset_dict)}')
     return dataset_dict[data_type](data_path, device=device)
 
 
+def update_recursive(dict1, dict2):
+    """slam/utils/config.py:41-52: merge dict2 into dict1, nested dicts key by key."""
+    for k, v in dict2.items():
+        if k not in dict1:
+            dict1[k] = dict()
+        if isinstance(v, dict):
+            update_recursive(dict1[k], v)
+        else:
+            dict1[k] = v
+
+
 def load_config(path):
+    """slam/utils/config.py:6-38: a YAML file, merged recursively over the file its
+    `inherit_from` names (NICE-SLAM's per-scene devices.yaml files inherit a dataset-wide one).
+    A relative `inherit_from` is looked up from the working directory, as the reference does, and
+    then next to the including file."""
     import yaml
     with open(path) as f:
-        return yaml.safe_load(f)
+        cfg_special = yaml.safe_load(f) or {}
+    inherit_from = cfg_special.get('inherit_from')
+    cfg = {}
+    if inherit_from is not None:
+        parent = str(inherit_from)
+        if not os.path.isabs(parent) and not os.path.exists(parent):
+            parent = os.path.join(os.path.dirname(os.path.abspath(path)), parent)
+        cfg = load_config(parent)
+    update_recursive(cfg, cfg_special)
+    return cfg
 
 
 class BaseDataset:
@@ -165,9 +246,11 @@ class BaseDataset:
 
     def read_raw(self, index):
         """Decoded frame `index` in pinned host memory: (uint8 BGR [H0,W0,3], int16 [Hd,Wd]
-        holding the uint16 depth bits)."""
+        holding the uint16 depth bits, or float32 [Hd,Wd] from an OpenEXR file)."""
         color = read_color(self.color_paths[index])
-        depth = read_depth(self.depth_paths[index]).view(np.int16)
+        depth = read_depth_any(self.depth_paths[index])
+        if depth.dtype == np.uint16:
+            depth = depth.view(np.int16)
         color, depth = torch.from_numpy(color), torch.from_numpy(depth)
         if torch.cuda.is_available():
             color, depth = color.pin_memory(), depth.pin_memory()
@@ -226,4 +309,200 @@ class Replica(BaseDataset):
         self.poses = load_replica_poses(f'{self.input_folder}/traj.txt', self.n_img)
 
 
-dataset_dict = {'replica': Replica}
+def _flip_pose(c2w):
+    """float64 [4,4] c2w in the dataset's camera axes -> the codebase's (columns 1 and 2
+    negated), as a float32 tensor."""
+    c2w[:3, 1] *= -1
+    c2w[:3, 2] *= -1
+    return torch.from_numpy(c2w).float()
+
+
+def _identity_poses(n):
+    return [torch.from_numpy(np.eye(4)).float() for _ in range(n)]
+
+
+class Azure(BaseDataset):
+    """datasets.py:336-370: color/*.jpg and depth/*.png in lexicographic order; scene/trajectory.log
+    in 5-line blocks (a header line, then four rows of the c2w), or the identity for every frame
+    when that file is missing."""
+
+    def __init__(self, data_path, device='cuda:0'):
+        super().__init__(data_path, device)
+        self.color_paths = sorted(glob.glob(os.path.join(self.input_folder, 'color', '*.jpg')))
+        self.depth_paths = sorted(glob.glob(os.path.join(self.input_folder, 'depth', '*.png')))
+        self.n_img = len(self.color_paths)
+        self.poses = self.load_poses(os.path.join(self.input_folder, 'scene', 'trajectory.log'))
+
+    def load_poses(self, path):
+        if not os.path.exists(path):
+            return _identity_poses(self.n_img)
+        with open(path) as f:
+            content = f.readlines()
+        poses = []
+        for i in range(0, len(content), 5):
+            rows = ''.join(content[i + 1:i + 5]).strip().split()
+            poses.append(_flip_pose(np.array(list(map(float, rows))).reshape((4, 4))))
+        return poses
+
+
+def _int_stem(path):
+    """ScanNet's sort key: the integer before the 4-character extension."""
+    return int(os.path.basename(path)[:-4])
+
+
+class ScanNet(BaseDataset):
+    """datasets.py:373-401: devices.yaml in the data root, frames under frames/: color/*.jpg,
+    depth/*.png and pose/*.txt, each sorted by the integer file stem; pose rows split on single
+    spaces (non-finite poses, as ScanNet has for lost frames, pass through)."""
+
+    def __init__(self, data_path, device='cuda:0'):
+        super().__init__(data_path, device)
+        self.input_folder = os.path.join(self.input_folder, 'frames')
+        self.color_paths = sorted(glob.glob(os.path.join(self.input_folder, 'color', '*.jpg')),
+                                  key=_int_stem)
+        self.depth_paths = sorted(glob.glob(os.path.join(self.input_folder, 'depth', '*.png')),
+                                  key=_int_stem)
+        self.poses = self.load_poses(os.path.join(self.input_folder, 'pose'))
+        self.n_img = len(self.color_paths)
+
+    def load_poses(self, path):
+        poses = []
+        for pose_path in sorted(glob.glob(os.path.join(path, '*.txt')), key=_int_stem):
+            with open(pose_path) as f:
+                vals = [list(map(float, line.split(' '))) for line in f.readlines()]
+            poses.append(_flip_pose(np.array(vals).reshape(4, 4)))
+        return poses
+
+
+def _scenes7_key(path):
+    """7-Scenes' sort key: the integer after the last '-' of the name's first dot-field
+    (frame-000012.color.png -> 12)."""
+    return int(os.path.basename(path).split('.')[0].split('-')[-1])
+
+
+class Scenes7(BaseDataset):
+    """datasets.py:404-435: *.color.png, *.depth.png and *.txt poses in one folder, sorted by
+    frame number; pose rows are tab-separated."""
+
+    def __init__(self, data_path, device='cuda:0'):
+        super().__init__(data_path, device)
+        self.color_paths = sorted(glob.glob(os.path.join(self.input_folder, '*.color.png')),
+                                  key=_scenes7_key)
+        self.depth_paths = sorted(glob.glob(os.path.join(self.input_folder, '*.depth.png')),
+                                  key=_scenes7_key)
+        self.poses = self.load_poses(self.input_folder)
+        self.n_img = len(self.color_paths)
+
+    def load_poses(self, path):
+        poses = []
+        for pose_path in sorted(glob.glob(os.path.join(path, '*.txt')), key=_scenes7_key):
+            with open(pose_path) as f:
+                vals = [list(map(float, line.strip().split('\t'))) for line in f.readlines()]
+            poses.append(_flip_pose(np.array(vals).reshape(4, 4)))
+        return poses
+
+
+class CoFusion(BaseDataset):
+    """datasets.py:438-458: colour/*.png and float32 OpenEXR depth_noise/*.exr.  Every pose is
+    the identity: the reference could not align CoFusion's trajectories with the codebase's
+    frame, and ATE aligns the trajectories anyway."""
+
+    def __init__(self, data_path, device='cuda:0'):
+        super().__init__(data_path, device)
+        self.color_paths = sorted(glob.glob(os.path.join(self.input_folder, 'colour', '*.png')))
+        self.depth_paths = sorted(glob.glob(os.path.join(self.input_folder, 'depth_noise',
+                                                         '*.exr')))
+        self.n_img = len(self.color_paths)
+        self.poses = _identity_poses(self.n_img)
+
+
+def tum_parse_list(filepath, skiprows=0):
+    """datasets.py:468-474: a space-separated list file as strings ('#' lines skipped)."""
+    import warnings
+    with warnings.catch_warnings():
+        # numpy notes that '#' lines do not count towards max_rows; nothing here sets it
+        warnings.filterwarnings('ignore', 'Input line', UserWarning)
+        return np.loadtxt(filepath, delimiter=' ', dtype=np.str_, skiprows=skiprows)
+
+
+def tum_associate(tstamp_image, tstamp_depth, tstamp_pose, max_dt=0.08):
+    """datasets.py:476-497: (image, depth, pose) index triples, each image paired with the
+    nearest depth and the nearest pose (argmin |dt|, first on ties), kept when both are closer
+    than max_dt seconds."""
+    associations = []
+    for i, t in enumerate(tstamp_image):
+        j = np.argmin(np.abs(tstamp_depth - t))
+        k = np.argmin(np.abs(tstamp_pose - t))
+        if (np.abs(tstamp_depth[j] - t) < max_dt) and (np.abs(tstamp_pose[k] - t) < max_dt):
+            associations.append((i, j, k))
+    return associations
+
+
+def tum_pose_matrix(pvec):
+    """datasets.py:546-553: tx ty tz qx qy qz qw -> float64 [4,4]."""
+    from scipy.spatial.transform import Rotation
+    pose = np.eye(4)
+    pose[:3, :3] = Rotation.from_quat(pvec[3:]).as_matrix()
+    pose[:3, 3] = pvec[:3]
+    return pose
+
+
+def load_tum(datapath, frame_rate=-1):
+    """datasets.py:499-544: -> (colour paths, depth paths, float32 c2w tensors).
+
+    The pose list is groundtruth.txt, else pose.txt, read with skiprows=1 as the reference does
+    (so a pose.txt without a header loses its first row).  Associated frames are subsampled:
+    an image is kept when it is more than 1 / frame_rate seconds after the last kept one."""
+    pose_list = None
+    for name in ('groundtruth.txt', 'pose.txt'):
+        if os.path.isfile(os.path.join(datapath, name)):
+            pose_list = os.path.join(datapath, name)
+            break
+    if pose_list is None:
+        raise FileNotFoundError(f'{datapath}: a TUM RGB-D folder needs groundtruth.txt or '
+                                'pose.txt')
+    image_data = tum_parse_list(os.path.join(datapath, 'rgb.txt'))
+    depth_data = tum_parse_list(os.path.join(datapath, 'depth.txt'))
+    pose_data = tum_parse_list(pose_list, skiprows=1)
+    pose_vecs = pose_data[:, 1:].astype(np.float64)
+    tstamp_image = image_data[:, 0].astype(np.float64)
+    tstamp_depth = depth_data[:, 0].astype(np.float64)
+    tstamp_pose = pose_data[:, 0].astype(np.float64)
+    associations = tum_associate(tstamp_image, tstamp_depth, tstamp_pose)
+    if not associations:
+        raise ValueError(f'{datapath}: no image has a depth image and a pose within 0.08 s')
+    indices = [0]
+    for i in range(1, len(associations)):
+        t0 = tstamp_image[associations[indices[-1]][0]]
+        t1 = tstamp_image[associations[i][0]]
+        if t1 - t0 > 1.0 / frame_rate:
+            indices += [i]
+    images, depths, poses = [], [], []
+    for ix in indices:
+        i, j, k = associations[ix]
+        images.append(os.path.join(datapath, image_data[i, 1]))
+        depths.append(os.path.join(datapath, depth_data[j, 1]))
+        poses.append(_flip_pose(tum_pose_matrix(pose_vecs[k])))
+    return images, depths, poses
+
+
+class TUM_RGBD(BaseDataset):
+    """datasets.py:461-553: rgb.txt / depth.txt / groundtruth.txt (or pose.txt) associated by
+    timestamp and subsampled at 32 frames per second (`load_tum`)."""
+
+    def __init__(self, data_path, device='cuda:0'):
+        super().__init__(data_path, device)
+        self.color_paths, self.depth_paths, self.poses = load_tum(self.input_folder,
+                                                                  frame_rate=32)
+        self.n_img = len(self.color_paths)
+
+
+# datasets.py:556-564 without 'euroc' (get_dataset explains why)
+dataset_dict = {
+    'replica': Replica,
+    'scannet': ScanNet,
+    'cofusion': CoFusion,
+    'azure': Azure,
+    'tumrgbd': TUM_RGBD,
+    '7scenes': Scenes7,
+}

@@ -163,18 +163,50 @@ def preset_differences(method):
     return out
 
 
+OVERRIDE_SECTIONS = ('model', 'mesher', 'tracker', 'mapper')
+
+
+def split_overrides(method, overrides):
+    """Sort config overrides by the config they reach: -> {'algorithm' | 'model' | 'mesher' |
+    'tracker' | 'mapper': {field: value}}.  A plain name is a field of the method's algorithm
+    config; 'model.', 'mesher.', 'tracker.' and 'mapper.' prefixes name a field of the nested
+    model / mesher config or of TrackerConfig / MapperConfig.  An unknown name raises ValueError
+    listing the fields it could have been."""
+    default = algorithm_config_class(method)()
+    fields = {'algorithm': default, 'model': getattr(default, 'model', None),
+              'mesher': getattr(default, 'mesher', None), 'tracker': TrackerConfig(),
+              'mapper': MapperConfig()}
+    fields = {k: set() if c is None else {f.name for f in dataclasses.fields(c)}
+              for k, c in fields.items()}
+    out = {k: {} for k in fields}
+    for key, value in overrides.items():
+        section, _, name = key.rpartition('.')
+        section = section or 'algorithm'
+        if section not in fields or (section == 'algorithm' and '.' in key):
+            raise ValueError(f'{key!r}: a field of the algorithm config, or one prefixed with '
+                             f'{", ".join(s + "." for s in OVERRIDE_SECTIONS)}')
+        if name not in fields[section]:
+            raise ValueError(f'{method} has no {section} config field {name!r}; its fields: '
+                             f'{sorted(fields[section])}')
+        out[section][name] = value
+    return out
+
+
 def make_config(method, data=None, data_type='replica', out_dir='outputs', device='cuda:0',
                 pretrained_decoders_coarse=None, pretrained_decoders_middle_fine=None,
-                **algorithm_overrides):
+                **overrides):
     """XRDSLAMConfig of a preset: the reference's tracker and mapper values, and the package's
     algorithm config with the reference preset's algorithm, model and mesher values and then
-    `algorithm_overrides` applied.  The pretrained_decoders_* paths (NICE-SLAM: coarse and
-    middle_fine; Point-SLAM: middle_fine) go to the model config."""
+    `overrides` applied (`split_overrides`: a plain name sets an algorithm-config field,
+    'model.x', 'mesher.x', 'tracker.x' and 'mapper.x' the nested ones, e.g.
+    make_config('co-slam', **{'mesher.resolution': 128})).  The pretrained_decoders_* paths
+    (NICE-SLAM: coarse and middle_fine; Point-SLAM: middle_fine) go to the model config."""
     if method not in PRESETS:
         raise ValueError(f'unknown method {method!r}; one of {sorted(PRESETS)}')
     p = PRESETS[method]
     cls = algorithm_config_class(method)
-    algo = cls(**{**p['algorithm_values'], **algorithm_overrides})
+    sets = split_overrides(method, overrides)
+    algo = cls(**{**p['algorithm_values'], **sets['algorithm']})
     model_values = dict(p['model_values'])
     for name, path in (('pretrained_decoders_coarse', pretrained_decoders_coarse),
                        ('pretrained_decoders_middle_fine', pretrained_decoders_middle_fine)):
@@ -182,13 +214,17 @@ def make_config(method, data=None, data_type='replica', out_dir='outputs', devic
             if name not in p['pretrained']:
                 raise ValueError(f'{method} has no {name}')
             model_values[name] = Path(path)
+    model_values.update(sets['model'])
+    mesher_values = {**p['mesher_values'], **sets['mesher']}
     if model_values:
         algo.model = dataclasses.replace(algo.model, **model_values)
-    if p['mesher_values']:
-        algo.mesher = dataclasses.replace(algo.mesher, **p['mesher_values'])
+    if mesher_values:
+        algo.mesher = dataclasses.replace(algo.mesher, **mesher_values)
     return XRDSLAMConfig(data=data, data_type=data_type, out_dir=Path(out_dir),
-                         algorithm_name=method, tracker=TrackerConfig(**p['tracker']),
-                         mapper=MapperConfig(**p['mapper']), algorithm=algo, device=device)
+                         algorithm_name=method,
+                         tracker=TrackerConfig(**{**p['tracker'], **sets['tracker']}),
+                         mapper=MapperConfig(**{**p['mapper'], **sets['mapper']}),
+                         algorithm=algo, device=device)
 
 
 def relative_pose(idx, gt_c2w_np, state, init_pose_offset):
