@@ -1090,6 +1090,8 @@ int xrd_frame_ingest_f32(const XrdIngestCfg* cfg, const uint8_t* color, const fl
  *                            :276-292), raw2outputs_nerf_color2
  *                            slam/model_components/utils.py:247-295, get_loss_dict
  *                            conv_onet_pointslam.py:144-195 and autograd's backward.
+ *   xrd_pointslam_sample_near_pcl  neural_point_cloud.py:284-348 sample_near_pcl
+ *                            (rendering_sample_near_pcl; its result feeds XrdPointCfg).
  */
 typedef struct {
   const float* pos;           /* DEVICE [N][3] neural point positions                      */
@@ -1115,6 +1117,28 @@ int xrd_pointslam_knn_query(const XrdPointIndex* index, const float* queries, co
                             int radius_stride, int n_queries, float* D, int32_t* I,
                             int32_t* neighbor_num, void* stream);
 
+/* Samples of the rays without depth near the neural point cloud: NeuralPointCloud.sample_near_pcl
+ * (slam/model_components/neural_point_cloud.py:284-348) as render_batch_ray calls it with
+ * rendering_sample_near_pcl on (slam/models/conv_onet_pointslam.py:379-409).  DEVICE pointers,
+ * asynchronous, no host synchronisation (far stays on the device).  For every ray r with
+ * !(target_d[r] > 0) (NaN included):
+ *   1. zq = torch.linspace(near_end, far[0], 25) in f32 (torch's two-sided formula), march
+ *      points p_k = o + d * zq_k (f32 multiply, then add);
+ *   2. hit_k = some cloud point at squared distance ((dx^2 + dy^2) + dz^2) < f32(radius_query^2)
+ *      (find_neighbors_faiss(step='query'): the FIXED query radius, "at least one neighbour";
+ *      exact search, SURVEY A.4);
+ *   3. with >= 2 hits: z[r] = f32(np.linspace(sec[c0], sec[c1], n_surface)) in float64, where
+ *      sec = np.linspace(near_end, (double)far[0], 25) and c0, c1 are the FIRST and SECOND hit
+ *      (the reference's item[0], item[1]); near[r] = 1;
+ *   4. otherwise z[r] = f32(np.linspace(near_end, (double)far[0], n_surface)) in float64 (not
+ *      the f32 torch.linspace of the option-off path); near[r] = 0.
+ * Rays with depth get near[r] = 1 and their row of z is left untouched.  An empty cloud
+ * (n_points 0, pos may be NULL) has no hits.  n_surface in [2, 16]. */
+int xrd_pointslam_sample_near_pcl(const XrdPointIndex* index, const float* rays_o,
+                                  const float* rays_d, const float* target_d, int n_rays,
+                                  const float* far, double near_end, double radius_query,
+                                  int n_surface, float* z, uint8_t* near, void* stream);
+
 typedef struct {
   int stage;               /* 0 = 'geometry', 1 = 'color'                                   */
   int is_mapping;
@@ -1133,6 +1157,12 @@ typedef struct {
   const float* rand_feat;  /* DEVICE [32] feature of samples with < min_nn neighbours (Q6)
                               or NULL = zeros                                               */
   const float* rand_feat_color; /* the colour decoder's own draw (decoder_pointslam.py:463) */
+  /* rendering_sample_near_pcl (conv_onet_pointslam.py:379-409, 450-451): both NULL, or both
+   * filled by xrd_pointslam_sample_near_pcl for this batch (same rays, depth and far).  Then
+   * the rays without depth take their samples from near_pcl_z, their rendered depth is kept
+   * (not overwritten by 0), and valid_ray_mask is ANDed with near_pcl_mask on them. */
+  const float* near_pcl_z;        /* DEVICE [R][n_surface]                                  */
+  const uint8_t* near_pcl_mask;   /* DEVICE [R]                                             */
 } XrdPointCfg;
 
 typedef struct {

@@ -222,7 +222,8 @@ class XrdPointCfg(C.Structure):
                 ('near_end', C.c_float), ('sigmoid_coef', C.c_float), ('min_nn_num', C.c_int),
                 ('w_color', C.c_float), ('handle_dynamic', C.c_int),
                 ('use_color_in_tracking', C.c_int), ('t_surface', vp), ('far', vp),
-                ('radius_query', vp), ('rand_feat', vp), ('rand_feat_color', vp)]
+                ('radius_query', vp), ('rand_feat', vp), ('rand_feat_color', vp),
+                ('near_pcl_z', vp), ('near_pcl_mask', vp)]
 
 
 class XrdPointFeats(C.Structure):
@@ -384,6 +385,9 @@ SYMBOLS = {
                                        vp]),
     'xrd_pointslam_knn_query': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp]),
+    'xrd_pointslam_sample_near_pcl': (C.c_int, [C.POINTER(XrdPointIndex), vp, vp, vp, C.c_int,
+                                                vp, C.c_double, C.c_double, C.c_int, vp, vp,
+                                                vp]),
     'xrd_coslam_query': (C.c_int, [C.POINTER(XrdHashGrid), C.POINTER(XrdCoslamMlp), vp, C.c_int,
                                    C.c_int, vp, vp, vp, vp]),
     'xrd_debug_gemm_mode': (C.c_int, [C.c_int]),

@@ -181,7 +181,7 @@ class ConvOnet2(Model):
         super().populate_modules()
         cfg = self.config
         if not cfg.use_dynamic_radius or cfg.pointcloud_nn_weighting != 'distance' or \
-                cfg.rendering_sample_near_pcl or cfg.model_encode_exposure:
+                cfg.model_encode_exposure:
             raise NotImplementedError('CUDA path covers the reference point-slam config')
         self.decoder = POINT(cfg.model_c_dim)
         self.load_pretrain()
@@ -240,11 +240,18 @@ class ConvOnet2(Model):
         rays_o = rays_o.detach().to(**f32).contiguous()
         rays_d = rays_d.detach().to(**f32).contiguous()
         R, S = rays_o.shape[0], cfg.rendering_n_surface
-        td = target_d.detach().to(**f32).reshape(-1).contiguous()
         ts = target_s.detach().to(**f32).contiguous() if target_s is not None else None
         radius = radius.detach().to(**f32).reshape(-1).contiguous()
-        # far = min(5 * mean(d), max(1.2 * d)) (conv_onet_pointslam.py:340-342), batch-global
-        far = torch.minimum(5 * td.mean(), torch.max(td * 1.2)).reshape(1).float().contiguous()
+        if target_d is not None:
+            td = target_d.detach().to(**f32).reshape(-1).contiguous()
+            # far = min(5 * mean(d), max(1.2 * d)) (conv_onet_pointslam.py:340-342), batch-global
+            far = torch.minimum(5 * td.mean(), torch.max(td * 1.2)).reshape(1).float().contiguous()
+        else:  # no depth at all: every ray is rendered over 10 m (conv_onet_pointslam.py:350-354)
+            td = torch.zeros(R, **f32)
+            far = torch.full((1,), 10.0, **f32)
+        zn = nm = None
+        if cfg.rendering_sample_near_pcl:
+            zn, nm = npc.near_pcl_samples(rays_o, rays_d, td, far, cfg.rendering_near_end, S)
         o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f32),
                  uncertainty=torch.empty(R, **f32),
                  valid_ray_mask=torch.empty(R, dtype=torch.uint8, device=dev),
@@ -265,7 +272,8 @@ class ConvOnet2(Model):
                         cfg.rendering_sigmoid_coef_mapper, cfg.pointcloud_min_nn_num,
                         cfg.mapping_w_color_loss if is_mapping else cfg.tracking_w_color_loss,
                         int(cfg.tracking_handle_dynamic), int(cfg.tracking_use_color_in_tracking),
-                        ptr(self._t_surface), ptr(far), ptr(radius), ptr(rf), ptr(rfc))
+                        ptr(self._t_surface), ptr(far), ptr(radius), ptr(rf), ptr(rfc),
+                        ptr(zn), ptr(nm))
         zc = getattr(self, '_z_capture', None)
         out = XrdPointOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['uncertainty']),
                           ptr(o['valid_ray_mask']), ptr(zc), ptr(o['losses']))

@@ -70,6 +70,35 @@ __device__ __forceinline__ void knn_insert(float (&bd)[KNN], int (&bi)[KNN], flo
   }
 }
 
+// The hash-grid cell walk: visit(id, x) for every cloud point in the cells c0, c0 + cstep, ..
+// of the box [q - r, q + r]; a visit returning true ends the walk.
+template <class Visit>
+__device__ __forceinline__ void walk_cells(const XrdPointIndex& ix, const float q[3], float r,
+                                           int c0, int cstep, Visit&& visit) {
+  const float inv = 1.0f / ix.cell;
+  int lo[3], n[3];
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    lo[d] = (int)floorf((q[d] - r) * inv);
+    n[d] = (int)floorf((q[d] + r) * inv) - lo[d] + 1;
+  }
+  const int ncell = n[0] * n[1] * n[2];
+  for (int c = c0; c < ncell; c += cstep) {
+    const int ixx = lo[0] + c % n[0], iy = lo[1] + (c / n[0]) % n[1], iz = lo[2] + c / (n[0] * n[1]);
+    const uint32_t b = bucket_of(ixx, iy, iz, ix.table_size);
+    const int s = ix.cell_start[b], e = ix.cell_end[b];
+    for (int j = s; j < e; ++j) {
+      const int id = ix.sorted_ids[j];
+      const float* x = ix.pos + (size_t)id * 3;
+      // a bucket can hold several cells: accept the point only in its own cell's turn
+      if ((int)floorf(x[0] * inv) != ixx || (int)floorf(x[1] * inv) != iy ||
+          (int)floorf(x[2] * inv) != iz)
+        continue;
+      if (visit(id, x)) return;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(128) k_knn(const KnnParams K) {
   const int gt = blockIdx.x * blockDim.x + threadIdx.x;
   const int p = gt / KG, sub = gt % KG;
@@ -83,30 +112,11 @@ __global__ void __launch_bounds__(128) k_knn(const KnnParams K) {
     query_point(K, p, q);
     const float r = K.radius[p / K.radius_div];
     r2 = r * r;
-    const float inv = 1.0f / K.ix.cell;
-    int lo[3], n[3];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-      lo[d] = (int)floorf((q[d] - r) * inv);
-      n[d] = (int)floorf((q[d] + r) * inv) - lo[d] + 1;
-    }
-    const int ncell = n[0] * n[1] * n[2];
-    for (int c = sub; c < ncell; c += KG) {
-      const int ixx = lo[0] + c % n[0], iy = lo[1] + (c / n[0]) % n[1], iz = lo[2] + c / (n[0] * n[1]);
-      const uint32_t b = bucket_of(ixx, iy, iz, K.ix.table_size);
-      const int s = K.ix.cell_start[b], e = K.ix.cell_end[b];
-      for (int j = s; j < e; ++j) {
-        const int id = K.ix.sorted_ids[j];
-        const float* x = K.ix.pos + (size_t)id * 3;
-        // a bucket can hold several cells: accept the point only in its own cell's turn
-        if ((int)floorf(x[0] * inv) != ixx || (int)floorf(x[1] * inv) != iy ||
-            (int)floorf(x[2] * inv) != iz)
-          continue;
-        const float d2 = sqdist(q, x);
-        if (d2 > r2) continue;
-        knn_insert(bd, bi, d2, id);
-      }
-    }
+    walk_cells(K.ix, q, r, sub, KG, [&](int id, const float* x) {
+      const float d2 = sqdist(q, x);
+      if (!(d2 > r2)) knn_insert(bd, bi, d2, id);
+      return false;
+    });
   }
   // butterfly merge inside the group of KG lanes (all 32 lanes take part in the shuffles)
 #pragma unroll
@@ -257,10 +267,79 @@ __global__ void __launch_bounds__(128) k_interp_bwd(const InterpParams Q) {
 }
 
 // ------------------------------------------------------------- per ray ---
+// torch.linspace(start, end, n)[k] in f32: the two-sided formula of torch's kernel
+__device__ __forceinline__ float linspace_f32(float start, float end, int n, int k) {
+  const float step = (end - start) / (float)(n - 1);
+  return (k < n / 2) ? __fadd_rn(start, __fmul_rn(step, (float)k))
+                     : __fsub_rn(end, __fmul_rn(step, (float)(n - 1 - k)));
+}
+
+// np.linspace(start, stop, n)[k] in f64 (numpy's function_base.linspace: arange * step + start,
+// the step == 0 branch (arange / div) * delta, and the last element set to stop)
+__device__ __forceinline__ double linspace_np(double start, double stop, int n, int k) {
+  if (k == n - 1) return stop;
+  const double div = (double)(n - 1), delta = __dsub_rn(stop, start);
+  const double step = __ddiv_rn(delta, div);
+  const double y = (step == 0.0) ? __dmul_rn(__ddiv_rn((double)k, div), delta)
+                                 : __dmul_rn((double)k, step);
+  return __dadd_rn(y, start);
+}
+
+// ---------------------------------------------------- samples near the cloud ---
+// NeuralPointCloud.sample_near_pcl (neural_point_cloud.py:284-348) for the rays without depth:
+// one warp per ray, lane k < 25 tests march point k for a cloud point with D < r^2.
+constexpr int NEAR_MARCH = 25;
+
+struct NearP {
+  XrdPointIndex ix;
+  int R, S;
+  const float *rays_o, *rays_d, *target_d, *far;
+  double near_end;
+  float r_walk, r2;
+  float* z;                 // [R][S]
+  unsigned char* near;      // [R]
+};
+
+__global__ void __launch_bounds__(128) k_near_pcl(const NearP N) {
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (r >= N.R) return;  // warp-uniform
+  if (N.target_d[r] > 0.f) {
+    if (lane == 0) N.near[r] = 1;
+    return;
+  }
+  bool hit = false;
+  if (lane < NEAR_MARCH && N.ix.n_points > 0) {
+    const float zq = linspace_f32((float)N.near_end, N.far[0], NEAR_MARCH, lane);
+    float q[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d)
+      q[d] = __fadd_rn(N.rays_o[r * 3 + d], __fmul_rn(N.rays_d[r * 3 + d], zq));
+    walk_cells(N.ix, q, N.r_walk, 0, 1, [&](int, const float* x) {
+      hit = sqdist(q, x) < N.r2;
+      return hit;
+    });
+  }
+  const unsigned m = __ballot_sync(0xffffffffu, hit);
+  const bool valid = __popc(m) >= 2;
+  if (lane == 0) N.near[r] = valid;
+  if (lane >= N.S) return;
+  // first and second hit (the reference's item[0], item[1]), else near_end .. far
+  const double far = (double)N.far[0];
+  double a = N.near_end, b = far;
+  if (valid) {
+    const int c0 = __ffs(m) - 1, c1 = __ffs(m & (m - 1)) - 1;
+    a = linspace_np(N.near_end, far, NEAR_MARCH, c0);
+    b = linspace_np(N.near_end, far, NEAR_MARCH, c1);
+  }
+  N.z[r * N.S + lane] = __double2float_rn(linspace_np(a, b, N.S, lane));
+}
+
 struct RayP {
   int R, S;
   const float *rays_o, *rays_d, *target_s, *target_d;
   const float *t_surface, *far;
+  const float* z_near;            // [R][S] samples of the zero-depth rays, or NULL
+  const unsigned char* near;      // [R] with z_near: zero-depth ray close to the cloud
   float near_s, far_s, near_end, coef;
   float* z;                       // [R][S]
   const float* occ;               // [P]
@@ -292,13 +371,11 @@ __global__ void __launch_bounds__(128) k_sample_z(const RayP P) {
       const float t = P.t_surface[k];
       P.z[r * S + k] = __fadd_rn(__fmul_rn(a, __fsub_rn(1.f, t)), __fmul_rn(b, t));
     }
+  } else if (P.z_near) {
+    for (int k = 0; k < S; ++k) P.z[r * S + k] = P.z_near[r * S + k];
   } else {
     // torch.linspace(near_end, max(far), S): scalar formula (S < SIMD width)
-    const float end = P.far[0], start = P.near_end;
-    const float step = (end - start) / (float)(S - 1);
-    for (int k = 0; k < S; ++k)
-      P.z[r * S + k] = (k < S / 2) ? __fadd_rn(start, __fmul_rn(step, (float)k))
-                                   : __fsub_rn(end, __fmul_rn(step, (float)(S - 1 - k)));
+    for (int k = 0; k < S; ++k) P.z[r * S + k] = linspace_f32(P.near_end, P.far[0], S, k);
   }
 }
 
@@ -326,7 +403,8 @@ __global__ void __launch_bounds__(128) k_composite_fwd(const RayP P) {
   float var = 0.f;
   for (int k = 0; k < S; ++k) { const float t = P.z[r * S + k] - depth; var = fmaf(w[k] * t, t, var); }
   const bool nz = P.target_d[r] > 0.f;
-  P.o_depth[r] = nz ? depth : 0.f;   // depth[~gt_non_zero_mask] = 0
+  // depth[~gt_non_zero_mask] = 0 unless rendering_sample_near_pcl
+  P.o_depth[r] = (nz || P.z_near) ? depth : 0.f;
   P.o_var[r] = var;
   for (int c = 0; c < 3; ++c) {
     float acc = 0.f;
@@ -334,7 +412,7 @@ __global__ void __launch_bounds__(128) k_composite_fwd(const RayP P) {
       for (int k = 0; k < S; ++k) acc = fmaf(w[k], P.rgb3[(size_t)c * P.Pp + r * S + k], acc);
     P.o_rgb[r * 3 + c] = acc / wsum;
   }
-  P.o_valid[r] = !(nvalid < P.min_valid);
+  P.o_valid[r] = !(nvalid < P.min_valid) && (nz || !P.z_near || P.near[r]);
 }
 
 __global__ void __launch_bounds__(1024) k_loss(const RayP P) {
@@ -412,7 +490,8 @@ __global__ void __launch_bounds__(128) k_composite_bwd(const RayP P) {
   if (r >= P.R) return;
   const int S = P.S;
   const bool nz = P.target_d[r] > 0.f;
-  const float gd = nz ? P.gd[r] : 0.f;  // zero-depth rays: depth overwritten by 0 (no gradient)
+  // zero-depth rays: depth overwritten by 0 (no gradient) unless rendering_sample_near_pcl
+  const float gd = (nz || P.z_near) ? P.gd[r] : 0.f;
   float alpha[16], Tt[16], w[16];
   float T = 1.f, ws = 0.f, nd = 0.f;
   for (int k = 0; k < S; ++k) {
@@ -609,6 +688,33 @@ extern "C" int xrd_pointslam_knn_query(const XrdPointIndex* index, const float* 
   return XRD_OK;
 }
 
+extern "C" int xrd_pointslam_sample_near_pcl(const XrdPointIndex* index, const float* rays_o,
+                                             const float* rays_d, const float* target_d,
+                                             int n_rays, const float* far, double near_end,
+                                             double radius_query, int n_surface, float* z,
+                                             uint8_t* near, void* stream) {
+  if (!index || !rays_o || !rays_d || !target_d || !far || !z || !near) return XRD_E_NULL;
+  if (!index->cell_start || !index->cell_end || !index->sorted_ids) return XRD_E_NULL;
+  if (index->n_points > 0 && !index->pos) return XRD_E_NULL;
+  if (index->n_points < 0 || index->table_size < 1 || (index->table_size & (index->table_size - 1)) ||
+      !(index->cell > 0.f) || !(radius_query >= 0.0))
+    return XRD_E_SHAPE;
+  if (n_rays <= 0) return XRD_OK;
+  if (n_surface < 2 || n_surface > 16) return XRD_E_SHAPE;
+  NearP N;
+  N.ix = *index; N.R = n_rays; N.S = n_surface;
+  N.rays_o = rays_o; N.rays_d = rays_d; N.target_d = target_d; N.far = far;
+  N.near_end = near_end;
+  // D < radius_query**2: torch compares the f32 distances with the f64 square rounded to f32;
+  // the cell box is widened by 1e-4 so that rounding cannot drop a cell holding such a point
+  N.r2 = (float)(radius_query * radius_query);
+  N.r_walk = (float)radius_query * 1.0001f;
+  N.z = z; N.near = near;
+  k_near_pcl<<<(int)(((long long)n_rays * 32 + 127) / 128), 128, 0, (cudaStream_t)stream>>>(N);
+  XRD_LAUNCH_CHECK();
+  return XRD_OK;
+}
+
 namespace {
 struct PWs : Carver {
   PWs(void* base, int R, int S, int stage, int with_grads)
@@ -768,6 +874,7 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   if (!rays || !index || !feats || !dec || !cfg || !out || !workspace) return XRD_E_NULL;
   if (!rays->rays_o || !rays->rays_d || !rays->target_d || !feats->geo_feats) return XRD_E_NULL;
   if (!cfg->t_surface || !cfg->far || !cfg->radius_query) return XRD_E_NULL;
+  if (!cfg->near_pcl_z != !cfg->near_pcl_mask) return XRD_E_NULL;
   if (!out->rgb || !out->depth || !out->uncertainty || !out->valid_ray_mask) return XRD_E_NULL;
   const int stage = cfg->stage;
   if (stage != 0 && stage != 1) return XRD_E_SHAPE;
@@ -803,6 +910,7 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   Y.R = R; Y.S = S; Y.rays_o = rays->rays_o; Y.rays_d = rays->rays_d;
   Y.target_s = rays->target_s; Y.target_d = rays->target_d; Y.t_surface = cfg->t_surface;
   Y.far = cfg->far; Y.near_s = cfg->near_end_surface; Y.far_s = cfg->far_end_surface;
+  Y.z_near = cfg->near_pcl_z; Y.near = cfg->near_pcl_mask;
   Y.near_end = cfg->near_end; Y.coef = cfg->sigmoid_coef; Y.z = z;
   Y.occ = L.occ;
   Y.has_nb = L.has;

@@ -118,6 +118,33 @@ class NeuralPointCloud(nn.Module):
                         stride, P, ptr(D), ptr(I), ptr(n))
         return D, I, n
 
+    def near_pcl_samples(self, rays_o, rays_d, target_d, far, near, num):
+        """xrd_pointslam_sample_near_pcl on contiguous DEVICE f32 rays [R,3], depth [R] and
+        far [1] -> (z [R,num] f32, near_mask [R] uint8).  Rays with depth keep an
+        uninitialised row of z and a mask of 1."""
+        dev = self.device
+        R = rays_o.shape[0]
+        z = torch.empty(R, num, dtype=torch.float32, device=dev)
+        mask = torch.empty(R, dtype=torch.uint8, device=dev)
+        ix = self.index_struct()
+        _cabi.launch_on(dev, 'xrd_pointslam_sample_near_pcl', C.byref(ix), ptr(rays_o),
+                        ptr(rays_d), ptr(target_d), R, ptr(far), float(near),
+                        float(self.radius_query), int(num), ptr(z), ptr(mask))
+        return z, mask
+
+    def sample_near_pcl(self, rays_o, rays_d, near, far, num):
+        """neural_point_cloud.py:284-348: samples of rays without depth near the cloud, on the
+        device.  -> (z_vals [R,num] f32, invalid_mask [R] bool: fewer than two of the 25 march
+        points from near to far have a cloud point within radius_query).  `far` (a tensor
+        or a number) is taken as float32, as render_batch_ray's torch.max(far) is."""
+        f32 = dict(dtype=torch.float32, device=self.device)
+        rays_o = rays_o.detach().to(**f32).reshape(-1, 3).contiguous()
+        rays_d = rays_d.detach().to(**f32).reshape(-1, 3).contiguous()
+        far = torch.as_tensor(far).detach().to(**f32).reshape(1).contiguous()
+        depth = torch.zeros(rays_o.shape[0], **f32)
+        z, mask = self.near_pcl_samples(rays_o, rays_d, depth, far, near, num)
+        return z, mask == 0
+
     # ---- map update (neural_point_cloud.py:109-221) -----------------------------
     def add_neural_points(self, batch_rays_o, batch_rays_d, batch_gt_depth, batch_gt_color=None,
                           is_pts_grad=False, dynamic_radius=None, feats=None):
