@@ -89,14 +89,17 @@ class _PinnedStaging:
         self.cur = (sl, n)
         return sl['rows'][:n], sl['ids'][:n]
 
-    def upload(self, dev):
+    def upload(self, dev, out=None):
+        """Copy the current block to `dev` (into the device tensors `out` when given)."""
         sl, n = self.cur
-        rows = sl['rows'][:n].to(dev, non_blocking=True)
-        ids = sl['ids'][:n].to(dev, non_blocking=True)
+        src = sl['rows'][:n], sl['ids'][:n]
+        out = out or tuple(torch.empty_like(t, device=dev) for t in src)
+        for d, s in zip(out, src):
+            d.copy_(s, non_blocking=True)
         if sl['ev'] is None:
             sl['ev'] = torch.cuda.Event()
         sl['ev'].record(torch.cuda.current_stream(dev))
-        return rows, ids
+        return out
 
 
 class CoSLAM(Algorithm):
@@ -178,6 +181,25 @@ class CoSLAM(Algorithm):
                 keyframe.__dict__.pop(k, None)
             self.keyframe_graph.append(keyframe)
 
+    def _mapping_counts(self):
+        """(n_bank, n_cur): rows from the ray bank and the current frame (coslam.py:158-173)."""
+        n_kf, n = len(self.keyframe_graph), self.config.mapping_sample
+        if n_kf == 0:
+            return 0, n
+        return n, int(np.maximum(n // n_kf, self.config.min_sample_pixels))
+
+    def _sample_mapping_rows(self, cur_frame, rows, ids, n_bank):
+        """n_bank ray-bank rows (id = keyframe), then current-frame rows (id -1, its pose comes
+        last) into rows [n,7] / ids [n]; the bank ids are drawn first."""
+        if n_bank > 0:
+            idxs = self._sample_ids(len(self.keyframe_graph) * self.num_rays_to_save, n_bank)
+            torch.index_select(self.rays, 0, idxs, out=rows[:n_bank])
+            torch.div(idxs, self.num_rays_to_save, rounding_mode='floor', out=ids[:n_bank])
+        cur_tab = self._frame_rays(cur_frame)
+        torch.index_select(cur_tab, 0, self._sample_ids(cur_tab.shape[0], rows.shape[0] - n_bank),
+                           out=rows[n_bank:])
+        ids[n_bank:] = -1
+
     def sample_global_rays(self, bs):
         n_kf = len(self.keyframe_graph)
         idxs = self._sample_ids(n_kf * self.num_rays_to_save, bs)
@@ -192,11 +214,7 @@ class CoSLAM(Algorithm):
             # into a pinned staging block; device side: ONE copy of the rows, one of the
             # pose ids, rays built by csrc/rays.cu (per-ray pose gather + its backward).
             n_kf = len(self.keyframe_graph)
-            n_bank = self.config.mapping_sample if n_kf > 0 else 0
-            n_cur = self.config.mapping_sample
-            if n_kf > 0:
-                n_cur = int(np.maximum(self.config.mapping_sample // n_kf,
-                                       self.config.min_sample_pixels))
+            n_bank, n_cur = self._mapping_counts()
             n = n_bank + n_cur
             rows, ids = self._staging.acquire(n) if dev.type == 'cuda' else (
                 torch.empty(n, 7), torch.empty(n, dtype=torch.int64))
@@ -209,17 +227,10 @@ class CoSLAM(Algorithm):
                     raise IndexError(
                         f'co-slam mapping window has {len(optimize_frames) - 1} keyframes but '
                         f'the ray bank indexes {n_kf}: use keyframe_selection_method="all"')
-                idxs = self._sample_ids(n_kf * self.num_rays_to_save, n_bank)
-                torch.index_select(self.rays, 0, idxs, out=rows[:n_bank])
-                torch.div(idxs, self.num_rays_to_save, rounding_mode='floor',
-                          out=ids[:n_bank])
                 for frame in optimize_frames[:-1]:
                     pose_list.append(frame.pose)
                     detach.append(frame.fid == 0)
-            cur_tab = self._frame_rays(cur_frame)
-            torch.index_select(cur_tab, 0, self._sample_ids(cur_tab.shape[0], n_cur),
-                               out=rows[n_bank:])
-            ids[n_bank:] = -1  # the current frame's pose is appended last
+            self._sample_mapping_rows(cur_frame, rows, ids, n_bank)
             pose_list.append(cur_frame.pose)
             detach.append(False)
             poses_all = pose_matrices(pose_list, detach).to(dev)
@@ -245,10 +256,13 @@ class CoSLAM(Algorithm):
         }
 
     # ---- CUDA-graph mapping (row f1) -------------------------------------------------
-    def _graph_ok(self, optimize_frames):
+    def _graph_config_ok(self):
         cfg = self.config
-        if not (cfg.graph_mapping and self.device.type == 'cuda' and cfg.separate_LR
-                and cfg.rot_rep == 'axis_angle'):
+        return (cfg.graph_mapping and self.device.type == 'cuda' and cfg.separate_LR
+                and cfg.rot_rep == 'axis_angle')
+
+    def _graph_ok(self, optimize_frames):
+        if not self._graph_config_ok():
             return False
         n_kf = len(self.keyframe_graph)
         return n_kf == 0 or len(optimize_frames) == n_kf + 1  # ids index the window 1:1
@@ -256,11 +270,8 @@ class CoSLAM(Algorithm):
     def mapping_session(self, optimize_frames):
         """The captured iteration for this window shape (cached by shape)."""
         from .coslam_graph import MappingGraphSession
-        n_kf = len(self.keyframe_graph)
-        first = n_kf == 0
-        n_bank = 0 if first else self.config.mapping_sample
-        n_cur = self.config.mapping_sample if first else int(np.maximum(
-            self.config.mapping_sample // n_kf, self.config.min_sample_pixels))
+        first = len(self.keyframe_graph) == 0
+        n_bank, n_cur = self._mapping_counts()
         ba = self.bundle_adjust and len(optimize_frames) > 1
         key = (n_bank, n_cur, len(optimize_frames), first, ba)
         # ONE live session: under keyframe_selection 'all' the window grows with every keyframe,
@@ -287,9 +298,7 @@ class CoSLAM(Algorithm):
         return s
 
     def optimize_update(self, n_iters, optimize_frames, is_mapping, coarse=False):
-        cfg = self.config
-        if not is_mapping and cfg.graph_mapping and self.device.type == 'cuda' and \
-                cfg.separate_LR and cfg.rot_rep == 'axis_angle':
+        if not is_mapping and self._graph_config_ok():
             with self.lock:
                 sess = self.tracking_session()
                 sess.begin(optimize_frames[-1])

@@ -266,6 +266,49 @@ class JointEncoding(Model):
         return (d.sdf_net.model[0].weight, d.sdf_net.model[2].weight,
                 d.color_net.model[0].weight, d.color_net.model[2].weight)
 
+    def _n_samples(self, with_depth=True):
+        cfg = self.config
+        return (cfg.training_n_sample_d +
+                cfg.training_n_range_d) if with_depth else cfg.training_n_samples
+
+    def _mlp_struct(self, weights):
+        return XrdCoslamMlp(*(ptr(w.detach()) for w in weights))
+
+    def _cfg_struct(self, S, seed=0, seed_dev=None, phase=0, n_rays_global=0,
+                    counts_global=None, counts_out=None):
+        """XrdCoslamCfg for S samples per ray; seed_dev and the counts are device tensors."""
+        cfg = self.config
+        return XrdCoslamCfg(
+            n_samples=S, n_sample_d=cfg.training_n_sample_d, n_range_d=cfg.training_n_range_d,
+            perturb=int(cfg.training_perturb > 0),
+            trunc=cfg.training_trunc * cfg.data_sc_factor, depth_trunc=cfg.cam_depth_trunc,
+            w_rgb=cfg.trainging_rgb_weight, w_depth=cfg.trainging_depth_weight,
+            w_sdf=cfg.trainging_sdf_weight, w_fs=cfg.trainging_fs_weight,
+            lin_uniform=ptr(self._lin_uniform), lin_range=ptr(self._lin_range),
+            lin_nodepth=ptr(self._lin_nodepth), lin_full=ptr(self._lin_full),
+            seed=seed, rays_per_tile=cfg.rays_per_tile, precision=cfg.precision, phase=phase,
+            n_rays_global=n_rays_global, counts_global=ptr(counts_global),
+            counts_out=ptr(counts_out), seed_dev=ptr(seed_dev))
+
+    def _outputs(self, R, S, dev):
+        """-> (buffers, XrdCoslamOut) of one pass over R rays of S samples."""
+        f32 = dict(dtype=torch.float32, device=dev)
+        o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f32),
+                 disp_map=torch.empty(R, **f32), acc_map=torch.empty(R, **f32),
+                 depth_var=torch.empty(R, **f32),
+                 z_vals=torch.empty(R, S, **f32),
+                 raw=torch.empty(R, S, 4, **f32),
+                 losses=torch.zeros(4, **f32))
+        out = XrdCoslamOut(rgb=ptr(o['rgb']), depth=ptr(o['depth']), disp=ptr(o['disp_map']),
+                           acc=ptr(o['acc_map']), depth_var=ptr(o['depth_var']),
+                           z_vals=ptr(o['z_vals']), raw=ptr(o['raw']), losses=ptr(o['losses']))
+        return o, out
+
+    def _next_seed(self, rank=0):
+        """Philox seed of the next pass, distinct per rank when mapping rays are sharded."""
+        self._step_count += 1
+        return (self.config.seed << 32) + self._step_count + (rank << 24)
+
     def _launch(self, rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
                 target_d, noise, with_grads, need_ray_grads=True,
                 loss_scale=None, seed=None, map_grads=True):
@@ -277,8 +320,7 @@ class JointEncoding(Model):
         rays_d = rays_d.detach().to(**f32).contiguous()
         R = rays_o.shape[0]
         has_d = target_d is not None
-        S = (cfg.training_n_sample_d +
-             cfg.training_n_range_d) if has_d else cfg.training_n_samples
+        S = self._n_samples(has_d)
         if has_d and cfg.training_n_sample_d <= 0:
             raise NotImplementedError('training_n_sample_d must be > 0')
         td = target_d.detach().to(**f32).reshape(-1).contiguous() if has_d \
@@ -288,34 +330,16 @@ class JointEncoding(Model):
         if noise is not None:
             noise = noise.detach().to(**f32).contiguous()
             assert noise.shape == (R, S)
-        o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f32),
-                 disp_map=torch.empty(R, **f32), acc_map=torch.empty(R, **f32),
-                 depth_var=torch.empty(R, **f32),
-                 z_vals=torch.empty(R, S, **f32),
-                 raw=torch.empty(R, S, 4, **f32),
-                 losses=torch.zeros(4, **f32))
+        o, out = self._outputs(R, S, dev)
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), ptr(ts), ptr(td))
         grid = self._grid_struct(table.detach())
-        mlp = XrdCoslamMlp(ptr(w0.detach()), ptr(w1.detach()),
-                           ptr(wc0.detach()), ptr(wc1.detach()))
+        mlp = self._mlp_struct((w0, w1, wc0, wc1))
         if seed is None:
-            self._step_count += 1
-            seed = (cfg.seed << 32) + self._step_count
+            seed = self._next_seed()
         # sharding applies to mapping only (tracking is per-frame sequential, single GPU)
         dp = self.dp if (self.dp is not None and self.dp.world > 1 and with_grads
                          and map_grads) else None
-        c = XrdCoslamCfg(
-            S, cfg.training_n_sample_d, cfg.training_n_range_d,
-            int(cfg.training_perturb > 0),
-            cfg.training_trunc * cfg.data_sc_factor, cfg.cam_depth_trunc,
-            cfg.trainging_rgb_weight, cfg.trainging_depth_weight,
-            cfg.trainging_sdf_weight, cfg.trainging_fs_weight,
-            ptr(self._lin_uniform), ptr(self._lin_range),
-            ptr(self._lin_nodepth), ptr(self._lin_full),
-            seed, cfg.rays_per_tile, cfg.precision, 0, 0, None, None, None)
-        out = XrdCoslamOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['disp_map']),
-                           ptr(o['acc_map']), ptr(o['depth_var']),
-                           ptr(o['z_vals']), ptr(o['raw']), ptr(o['losses']))
+        c = self._cfg_struct(S, seed=seed)
         g = None
         gs = None
         if with_grads:
@@ -450,7 +474,7 @@ class JointEncoding(Model):
         geo = torch.empty(P, 15, **f32) if want_geo else None
         feat = torch.empty(P, 32, **f32) if want_feat else None
         grid = self._grid_struct(table.detach())
-        mlp = XrdCoslamMlp(*(ptr(w.detach()) for w in self._weights()))
+        mlp = self._mlp_struct(self._weights())
         _cabi.launch_on(dev, 'xrd_coslam_query', C.byref(grid), C.byref(mlp), ptr(flat), P,
                         int(normalised), ptr(raw), ptr(geo), ptr(feat))
         return dict(raw=raw, geo=geo, feat=feat)

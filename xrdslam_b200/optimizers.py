@@ -8,6 +8,31 @@ from typing import Any, Dict, List, Optional, Tuple, Type
 import torch
 from torch.nn.parameter import Parameter
 
+from . import _cabi
+
+
+def adam_desc(param, grad, exp_avg, exp_avg_sq, lr, betas, eps, weight_decay,
+              bias_corrections=(1.0, 1.0), dyn=None, row_mask=None):
+    """XrdAdamTensor of one device fp32 tensor.  `dyn`, a device pointer to {lr, bias_correction1,
+    bias_correction2}, overrides those host values; rows whose `row_mask` entry is 0 are kept."""
+    a = _cabi.XrdAdamTensor(
+        param=param.data_ptr(), grad=grad.data_ptr(), exp_avg=exp_avg.data_ptr(),
+        exp_avg_sq=exp_avg_sq.data_ptr(), n=param.numel(), lr=lr, beta1=betas[0],
+        beta2=betas[1], eps=eps, weight_decay=weight_decay,
+        bias_correction1=bias_corrections[0], bias_correction2=bias_corrections[1], dyn=dyn)
+    if row_mask is not None:
+        a.row_mask, a.row_len = row_mask.data_ptr(), param.numel() // row_mask.numel()
+    return a
+
+
+def init_adam_state(state, p):
+    """Fill an empty `state` with torch.optim.Adam's `step`, `exp_avg` and `exp_avg_sq`."""
+    if not state:
+        state['step'] = torch.tensor(0.0)
+        state['exp_avg'] = torch.zeros_like(p)
+        state['exp_avg_sq'] = torch.zeros_like(p)
+    return state
+
 
 class FusedAdam(torch.optim.Optimizer):
     """torch.optim.Adam (amsgrad=False) for device-resident fp32 parameters: every tensor of
@@ -21,10 +46,8 @@ class FusedAdam(torch.optim.Optimizer):
 
     @torch.no_grad()
     def step(self, closure=None):
-        import ctypes as C
-        from . import _cabi
         loss = closure() if closure is not None else None
-        descs, dev = [], None
+        descs, grads, dev = [], [], None
         for group in self.param_groups:
             b1, b2 = group['betas']
             for p in group['params']:
@@ -32,30 +55,22 @@ class FusedAdam(torch.optim.Optimizer):
                     continue
                 if not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous():
                     raise RuntimeError('FusedAdam needs contiguous fp32 CUDA parameters')
-                st = self.state[p]
-                if not st:
-                    st['step'] = torch.tensor(0.0)
-                    st['exp_avg'] = torch.zeros_like(p)
-                    st['exp_avg_sq'] = torch.zeros_like(p)
+                st = init_adam_state(self.state[p], p)
                 st['step'] += 1
                 t = float(st['step'])
                 g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
-                descs.append((p, g, st, float(group['lr']), b1, b2, group['eps'],
-                              group['weight_decay'], 1.0 - b1**t, 1.0 - b2**t))
+                grads.append(g)  # a contiguous copy must outlive the launch
+                mask = getattr(p, '_xrd_row_mask', None)  # frustum feature selection (NICE-SLAM)
+                if mask is not None:
+                    assert mask.is_cuda and mask.dtype == torch.uint8 and mask.is_contiguous() and \
+                        p.numel() % mask.numel() == 0
+                descs.append(adam_desc(p, g, st['exp_avg'], st['exp_avg_sq'], float(group['lr']),
+                                       (b1, b2), group['eps'], group['weight_decay'],
+                                       (1.0 - b1**t, 1.0 - b2**t), row_mask=mask))
                 dev = p.device
         if not descs:
             return loss
-        arr = (_cabi.XrdAdamTensor * len(descs))()
-        for a, (p, g, st, lr, b1, b2, eps, wd, c1, c2) in zip(arr, descs):
-            a.param, a.grad = p.data_ptr(), g.data_ptr()
-            a.exp_avg, a.exp_avg_sq = st['exp_avg'].data_ptr(), st['exp_avg_sq'].data_ptr()
-            a.n, a.lr, a.beta1, a.beta2, a.eps = p.numel(), lr, b1, b2, eps
-            a.weight_decay, a.bias_correction1, a.bias_correction2 = wd, c1, c2
-            mask = getattr(p, '_xrd_row_mask', None)  # frustum feature selection (NICE-SLAM)
-            if mask is not None:
-                assert mask.is_cuda and mask.dtype == torch.uint8 and mask.is_contiguous() and \
-                    p.numel() % mask.numel() == 0
-                a.row_mask, a.row_len = mask.data_ptr(), p.numel() // mask.numel()
+        arr = (_cabi.XrdAdamTensor * len(descs))(*descs)
         _cabi.launch_on(dev, 'xrd_adam_step', arr, len(descs), 0)
         return loss
 
