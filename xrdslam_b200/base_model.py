@@ -51,6 +51,29 @@ def scale_grads(grads, s):
     return out
 
 
+class FusedStep(torch.autograd.Function):
+    """``(losses, *outputs) = FusedStep.apply(launch, n_live, *inputs)``: autograd bridge of a
+    fused step, which computes its gradients during forward.
+
+    ``inputs`` are the tensors autograd may differentiate.  ``launch(needs)`` receives their
+    ``needs_input_grad`` flags and returns ``(losses, outputs, grads)``: ``outputs`` is a tuple
+    of non-differentiable tensors, ``grads`` a list aligned with ``inputs`` (None where no
+    gradient exists), or None for a forward-only launch.  backward hands ``grads`` out scaled
+    by ``upstream_scale(g_losses, n_live)``."""
+    @staticmethod
+    def forward(ctx, launch, n_live, *inputs):
+        losses, outputs, grads = launch(ctx.needs_input_grad[2:])
+        ctx.grads, ctx.n_live = grads, n_live
+        ctx.mark_non_differentiable(*outputs)
+        return (losses, *outputs)
+
+    @staticmethod
+    def backward(ctx, g_losses, *_):
+        if ctx.grads is None:
+            raise RuntimeError('backward through a forward-only fused pass')
+        return (None, None, *scale_grads(ctx.grads, upstream_scale(g_losses, ctx.n_live)))
+
+
 @dataclass
 class InstantiateConfig:
     """A config knows the class it configures: ``cfg.setup(**kw)`` builds ``_target(cfg, **kw)``."""
@@ -89,6 +112,11 @@ class Model(nn.Module):
 
     def forward(self, input) -> Outputs:
         return self.get_outputs(input)
+
+    def map_inputs(self, *tensors) -> List[torch.Tensor]:
+        """Map / decoder tensors as they enter a fused step: detached while
+        ``freeze_map_grads`` is set, so the step computes pose gradients only."""
+        return [t.detach() for t in tensors] if self.freeze_map_grads else list(tensors)
 
     # ---- the contract every representation implements -------------------------------
     def get_outputs(self, input) -> Outputs:

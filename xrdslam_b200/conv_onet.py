@@ -25,9 +25,10 @@ from torch.nn import Parameter
 from . import _cabi
 from ._cabi import (XrdNiceCfg, XrdNiceCoarseCfg, XrdNiceCoarseDecoder, XrdNiceDecoder,
                     XrdNiceDecoderGrads, XrdNiceGrads, XrdNiceGrid, XrdNiceOut, XrdRays, ptr)
-from .base_model import Model, ModelConfig, scale_grads, upstream_scale
+from .base_model import FusedStep, Model, ModelConfig
 
 STAGES = {'middle': 0, 'fine': 1, 'color': 2}  # 'coarse' has its own entry (xrd_nice_coarse_step)
+GRIDS = ('grid_middle', 'grid_fine', 'grid_color')  # indexed by STAGES
 
 
 @dataclass
@@ -138,58 +139,6 @@ def _dec_struct(tensors, c_dim, n_out, cls=XrdNiceDecoder):
     return d
 
 
-class _NiceStep(torch.autograd.Function):
-    """(losses[2], rgb, depth, uncertainty) = fused(rays, 3 grids, colour decoder)."""
-    @staticmethod
-    def forward(ctx, model, stage, is_mapping, target_s, target_d, rays_o, rays_d, gm, gf,
-                gc, *color_params):
-        need_rays = ctx.needs_input_grad[5] or ctx.needs_input_grad[6]
-        need_grid = [ctx.needs_input_grad[7 + i] for i in range(3)]
-        need_col = any(ctx.needs_input_grad[10:])
-        with_grads = need_rays or any(need_grid) or need_col
-        outs, grads = model._launch(stage, is_mapping, rays_o, rays_d, target_s, target_d,
-                                    with_grads, need_rays, need_grid, need_col)
-        ctx.grads = grads
-        cfg = model.config  # the colour term is live exactly when get_loss_dict returns it
-        ctx.n_live = 2 if ((not is_mapping and cfg.tracking_use_color_in_tracking) or
-                           (is_mapping and stage == 'color')) else 1
-        ret = (outs['losses'], outs['rgb'], outs['depth'], outs['uncertainty'])
-        ctx.mark_non_differentiable(*ret[1:])
-        return ret
-
-    @staticmethod
-    def backward(ctx, g_losses, *_):
-        g = ctx.grads
-        if g is None:
-            raise RuntimeError('backward through a forward-only NICE pass')
-        ro, rd, dg, dc = scale_grads([g['d_rays_o'], g['d_rays_d'], list(g['d_grid']),
-                                      list(g['d_color'])], upstream_scale(g_losses, ctx.n_live))
-        return (None, None, None, None, None, ro, rd, dg[0], dg[1], dg[2], *dc)
-
-
-class _NiceCoarseStep(torch.autograd.Function):
-    """(losses[2], rgb, depth, uncertainty) = fused coarse stage(rays, coarse grid)."""
-    @staticmethod
-    def forward(ctx, model, target_d, rays_o, rays_d, grid):
-        need_rays = ctx.needs_input_grad[2] or ctx.needs_input_grad[3]
-        need_grid = ctx.needs_input_grad[4]
-        outs, grads = model._launch_coarse(rays_o, rays_d, target_d, need_rays or need_grid,
-                                           need_rays, need_grid)
-        ctx.grads = grads
-        ret = (outs['losses'], outs['rgb'], outs['depth'], outs['uncertainty'])
-        ctx.mark_non_differentiable(*ret[1:])
-        return ret
-
-    @staticmethod
-    def backward(ctx, g_losses, *_):
-        g = ctx.grads
-        if g is None:
-            raise RuntimeError('backward through a forward-only NICE coarse pass')
-        ro, rd, dg = scale_grads([g['d_rays_o'], g['d_rays_d'], g['d_grid']],
-                                 upstream_scale(g_losses, 1))
-        return None, None, ro, rd, dg
-
-
 class ConvOnet(Model):
     """Model class (slam/models/conv_onet.py:66-524)."""
 
@@ -291,6 +240,27 @@ class ConvOnet(Model):
             self.grids[key].copy_(val_ref_layout.squeeze(0).permute(1, 2, 3, 0))
 
     # ------------------------------------------------------------- C-ABI ---
+    def _level_structs(self):
+        """(XrdNiceGrid[3], XrdNiceDecoder[3], keep) of the middle / fine / colour levels;
+        ``keep`` holds the detached tensors the structs point into, for the caller to keep
+        alive until its launch."""
+        grids, decs, keep = (XrdNiceGrid * 3)(), (XrdNiceDecoder * 3)(), []
+        dmods = (self.decoder.middle_decoder, self.decoder.fine_decoder,
+                 self.decoder.color_decoder)
+        for i, (k, m) in enumerate(zip(GRIDS, dmods)):
+            g = self.grids[k].detach()
+            t = [x.detach() for x in m.tensors()]
+            keep += [g, t]
+            grids[i] = XrdNiceGrid(ptr(g), g.shape[2], g.shape[1], g.shape[0])
+            decs[i] = _dec_struct(t, m.c_dim, 4 if m.color else 1)
+        return grids, decs, keep
+
+    def _out_struct(self, o):
+        """XrdNiceOut over the output dict of a launch (sample depths go to the test hook
+        ``_z_capture`` when it is set)."""
+        return XrdNiceOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['uncertainty']),
+                          ptr(getattr(self, '_z_capture', None)), None, ptr(o['losses']))
+
     def _launch(self, stage, is_mapping, rays_o, rays_d, target_s, target_d, with_grads,
                 need_rays=False, need_grid=(False, False, False), need_col=False):
         cfg = self.config
@@ -307,16 +277,7 @@ class ConvOnet(Model):
         o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f64),
                  uncertainty=torch.empty(R, **f64), losses=torch.zeros(2, **f32))
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), ptr(ts), ptr(td))
-        keys = ('grid_middle', 'grid_fine', 'grid_color')
-        grids = (XrdNiceGrid * 3)()
-        for i, k in enumerate(keys):
-            g = self.grids[k].detach()
-            grids[i] = XrdNiceGrid(ptr(g), g.shape[2], g.shape[1], g.shape[0])
-        decs = (XrdNiceDecoder * 3)()
-        dmods = (self.decoder.middle_decoder, self.decoder.fine_decoder,
-                 self.decoder.color_decoder)
-        for i, m in enumerate(dmods):
-            decs[i] = _dec_struct([t.detach() for t in m.tensors()], m.c_dim, 4 if m.color else 1)
+        grids, decs, keep = self._level_structs()
         c = XrdNiceCfg()
         c.stage = STAGES[stage]
         c.is_mapping = int(is_mapping)
@@ -332,17 +293,14 @@ class ConvOnet(Model):
         if self.dp is not None and self.dp.world > 1 and is_mapping and with_grads:
             maxd = self.dp.all_reduce_max(td.max().reshape(1))  # batch-global (Q9), no host sync
         c.max_depth_global = ptr(maxd)
-        zc = getattr(self, '_z_capture', None)  # tests: capture the f64 sample depths
-        out = XrdNiceOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['uncertainty']), ptr(zc), None,
-                         ptr(o['losses']))
+        out = self._out_struct(o)
         g = None
         gs = None
-        keep = []
         if with_grads:
             if ts is None:
                 raise RuntimeError('gradients need target_s')
             dgrid = [torch.zeros_like(self.grids[k]) if (need_grid[i] and i <= c.stage) else None
-                     for i, k in enumerate(keys)]
+                     for i, k in enumerate(GRIDS)]
             dcol = None
             if need_col and c.stage == 2:
                 dcol = [torch.zeros_like(t) for t in self.decoder.color_decoder.tensors()]
@@ -398,9 +356,7 @@ class ConvOnet(Model):
             c.coarse_bound_min[k] = float(self.bounding_box[k, 0] * e)
             c.coarse_bound_max[k] = float(self.bounding_box[k, 1] * e)
         c.t_uniform = ptr(self._t_uniform)
-        zc = getattr(self, '_z_capture', None)
-        out = XrdNiceOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['uncertainty']), ptr(zc), None,
-                         ptr(o['losses']))
+        out = self._out_struct(o)
         gr = None
         if with_grads:
             if td is None:
@@ -422,33 +378,40 @@ class ConvOnet(Model):
         rays_o, rays_d = input['rays_o'], input['rays_d']
         target_d, target_s = input['target_d'], input.get('target_s')
         fused = torch.is_grad_enabled() and target_s is not None and 'is_mapping' in input
-        if stage == 'coarse':
+        if not fused:
             # conv_onet.py:137-138: the coarse level renders without depth guidance; the
             # target depth only enters the (mapping) loss
-            if fused:
-                grid = self.grids['grid_coarse']
-                if getattr(self, 'freeze_map_grads', False):
-                    grid = grid.detach()
-                losses, rgb, depth, unc = _NiceCoarseStep.apply(self, target_d, rays_o, rays_d, grid)
-                return {'rgb': rgb, 'depth': depth, 'uncertainty': unc, '_losses': losses}
-            o, _ = self._launch_coarse(rays_o, rays_d, target_d, False)
+            o, _ = self._launch_coarse(rays_o, rays_d, target_d, False) if stage == 'coarse' \
+                else self._launch(stage, True, rays_o, rays_d, target_s, target_d, False)
             o.pop('losses')
             return o
-        if fused:
-            cparams = self.decoder.color_decoder.tensors()
-            grids = [self.grids[k] for k in ('grid_middle', 'grid_fine', 'grid_color')]
-            if getattr(self, 'freeze_map_grads', False):
-                # tracking optimises the pose only: skip grid / decoder gradients (the
-                # reference computes and discards them)
-                cparams = [t.detach() for t in cparams]
-                grids = [g.detach() for g in grids]
-            losses, rgb, depth, unc = _NiceStep.apply(
-                self, stage, input['is_mapping'], target_s, target_d, rays_o, rays_d,
-                *grids, *cparams)
-            return {'rgb': rgb, 'depth': depth, 'uncertainty': unc, '_losses': losses}
-        o, _ = self._launch(stage, True, rays_o, rays_d, target_s, target_d, False)
-        o.pop('losses')
-        return o
+        if stage == 'coarse':
+            maps, n_live = [self.grids['grid_coarse']], 1
+
+            def launch(needs):
+                need_rays, need_grid = needs[0] or needs[1], needs[2]
+                o, g = self._launch_coarse(rays_o, rays_d, target_d, need_rays or need_grid,
+                                           need_rays, need_grid)
+                grads = None if g is None else [g['d_rays_o'], g['d_rays_d'], g['d_grid']]
+                return o['losses'], (o['rgb'], o['depth'], o['uncertainty']), grads
+        else:
+            is_mapping, cfg = input['is_mapping'], self.config
+            maps = [self.grids[k] for k in GRIDS] + self.decoder.color_decoder.tensors()
+            # the colour term is live exactly when get_loss_dict returns it
+            n_live = 2 if ((not is_mapping and cfg.tracking_use_color_in_tracking) or
+                           (is_mapping and stage == 'color')) else 1
+
+            def launch(needs):
+                need_rays, need_grid, need_col = needs[0] or needs[1], needs[2:5], any(needs[5:])
+                o, g = self._launch(stage, is_mapping, rays_o, rays_d, target_s, target_d,
+                                    need_rays or any(need_grid) or need_col, need_rays,
+                                    need_grid, need_col)
+                grads = None if g is None else \
+                    [g['d_rays_o'], g['d_rays_d'], *g['d_grid'], *g['d_color']]
+                return o['losses'], (o['rgb'], o['depth'], o['uncertainty']), grads
+        losses, rgb, depth, unc = FusedStep.apply(launch, n_live, rays_o, rays_d,
+                                                  *self.map_inputs(*maps))
+        return {'rgb': rgb, 'depth': depth, 'uncertainty': unc, '_losses': losses}
 
     # ---- mesher-facing queries (conv_onet.py:213-240) -----------------------------------
     def _query(self, pi, stage):
@@ -456,18 +419,7 @@ class ConvOnet(Model):
         _cabi.require_cuda(dev, 'model')
         pts = pi.detach().reshape(-1, 3).to(device=dev, dtype=torch.float32).contiguous()
         P = pts.shape[0]
-        keys = ('grid_middle', 'grid_fine', 'grid_color')
-        grids = (XrdNiceGrid * 3)()
-        for i, k in enumerate(keys):
-            g = self.grids[k].detach()
-            grids[i] = XrdNiceGrid(ptr(g), g.shape[2], g.shape[1], g.shape[0])
-        decs = (XrdNiceDecoder * 3)()
-        keep = []
-        for i, m in enumerate((self.decoder.middle_decoder, self.decoder.fine_decoder,
-                               self.decoder.color_decoder)):
-            t = [x.detach() for x in m.tensors()]
-            keep.append(t)
-            decs[i] = _dec_struct(t, m.c_dim, 4 if m.color else 1)
+        grids, decs, keep = self._level_structs()
         bmin = (C.c_double * 3)(*[float(self.bounding_box[d, 0]) for d in range(3)])
         bmax = (C.c_double * 3)(*[float(self.bounding_box[d, 1]) for d in range(3)])
         raw = torch.empty(P, 4, dtype=torch.float32, device=dev)

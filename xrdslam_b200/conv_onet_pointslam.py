@@ -21,7 +21,7 @@ from . import _cabi
 from ._cabi import (XrdNiceDecoder, XrdPointCfg, XrdPointColorDecoder,
                     XrdPointColorDecoderGrads, XrdPointFeats, XrdPointGrads, XrdPointOut,
                     XrdRays, ptr)
-from .base_model import Model, ModelConfig, scale_grads, upstream_scale
+from .base_model import FusedStep, Model, ModelConfig
 from .conv_onet import MLP as _GeoMLP
 from .conv_onet import _dec_struct
 from .neural_point_cloud import NeuralPointCloud
@@ -136,39 +136,6 @@ class POINT(nn.Module):
         super().__init__()
         self.geo_decoder = _GeoMLP('geometry', c_dim, False)
         self.color_decoder = MLPColor(c_dim)
-
-
-class _PointStep(torch.autograd.Function):
-    """forward launches the whole fused step (fwd + loss + bwd); backward hands out the
-    gradients computed there (unit upstream gradient, as loss = sum(loss_dict.values()))."""
-    @staticmethod
-    def forward(ctx, model, stage, is_mapping, target_s, target_d, radius, rand_feat,
-                rand_feat_color, rays_o, rays_d, geo_feats, col_feats, *cparams):
-        need = ctx.needs_input_grad
-        need_rays = need[8] or need[9]
-        color = stage == 'color'
-        outs, grads = model._launch(
-            stage, is_mapping, rays_o, rays_d, target_s, target_d, radius, rand_feat, True,
-            need_rays=need_rays, need_feats=need[10], rand_feat_color=rand_feat_color,
-            need_col_feats=color and need[11], need_cdec=color and any(need[12:]))
-        ctx.grads = grads
-        ctx.n_c = len(cparams)
-        # the colour term enters the in-kernel gradient only in stage 'color' (get_loss_dict
-        # lists ls[1] in geometry-stage tracking too, where it is identically 0)
-        ctx.n_live = 2 if (color and (is_mapping or model.config.tracking_use_color_in_tracking)) \
-            else 1
-        ret = (outs['losses'], outs['rgb'], outs['depth'], outs['uncertainty'],
-               outs['valid_ray_mask'])
-        ctx.mark_non_differentiable(*ret[1:])
-        return ret
-
-    @staticmethod
-    def backward(ctx, g_losses, *_):
-        g = ctx.grads
-        dc = g['d_cdec'] if g['d_cdec'] is not None else [None] * ctx.n_c
-        ro, rd, gf, cf, dc = scale_grads([g['d_rays_o'], g['d_rays_d'], g['d_geo_feats'],
-                                          g['d_col_feats'], list(dc)], upstream_scale(g_losses, ctx.n_live))
-        return (None, None, None, None, None, None, None, None, ro, rd, gf, cf, *dc)
 
 
 class ConvOnet2(Model):
@@ -307,12 +274,25 @@ class ConvOnet2(Model):
         npc = self.neural_point_cloud
         fused = torch.is_grad_enabled() and 'is_mapping' in input
         if fused:
-            gf, cf, cp = npc.geo_feats, npc.col_feats, self.decoder.color_decoder.tensors()
-            if getattr(self, 'freeze_map_grads', False):  # tracking: pose gradients only
-                gf, cf, cp = gf.detach(), cf.detach(), [t.detach() for t in cp]
-            losses, rgb, depth, unc, valid = _PointStep.apply(
-                self, stage, input['is_mapping'], ts, td, radius, input.get('rand_feat'),
-                input.get('rand_feat_color'), rays_o, rays_d, gf, cf, *cp)
+            is_mapping, color = input['is_mapping'], stage == 'color'
+            maps = [npc.geo_feats, npc.col_feats, *self.decoder.color_decoder.tensors()]
+            # the colour term enters the in-kernel gradient only in stage 'color' (get_loss_dict
+            # lists ls[1] in geometry-stage tracking too, where it is identically 0)
+            n_live = 2 if (color and (is_mapping or self.config.tracking_use_color_in_tracking)) \
+                else 1
+
+            def launch(needs):
+                o, g = self._launch(
+                    stage, is_mapping, rays_o, rays_d, ts, td, radius, input.get('rand_feat'),
+                    True, need_rays=needs[0] or needs[1], need_feats=needs[2],
+                    rand_feat_color=input.get('rand_feat_color'),
+                    need_col_feats=color and needs[3], need_cdec=color and any(needs[4:]))
+                dc = g['d_cdec'] if g['d_cdec'] is not None else [None] * len(needs[4:])
+                grads = [g['d_rays_o'], g['d_rays_d'], g['d_geo_feats'], g['d_col_feats'], *dc]
+                return (o['losses'], (o['rgb'], o['depth'], o['uncertainty'], o['valid_ray_mask']),
+                        grads)
+            losses, rgb, depth, unc, valid = FusedStep.apply(launch, n_live, rays_o, rays_d,
+                                                             *self.map_inputs(*maps))
             return {'rgb': rgb, 'depth': depth, 'uncertainty': unc, 'valid_ray_mask': valid,
                     'stage': stage, '_losses': losses}
         o, _ = self._launch(stage, True, rays_o, rays_d, ts, td, radius, input.get('rand_feat'),

@@ -23,7 +23,7 @@ from torch.nn import Parameter
 from . import _cabi
 from ._cabi import (XrdRays, XrdVoxDecoder, XrdVoxDecoderGrads, XrdVoxGrads, XrdVoxMap,
                     XrdVoxMarch, XrdVoxMarchCfg, XrdVoxOut, XrdVoxRenderCfg, check, ptr)
-from .base_model import Model, ModelConfig, scale_grads, upstream_scale
+from .base_model import FusedStep, Model, ModelConfig
 
 MAX_DEPTH = 10.0  # voxel_helpers_voxfusion.py:11
 
@@ -81,28 +81,6 @@ def _dec_struct(tensors, cls):
     for n, t in zip(('w0', 'b0', 'w1', 'b1', 'ws', 'bs', 'wc0', 'bc0', 'wc1', 'bc1'), tensors):
         setattr(d, n, ptr(t))
     return d
-
-
-class _VoxStep(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, model, target_s, target_d, noise, rays_o, rays_d, emb, *dec):
-        need_rays = ctx.needs_input_grad[4] or ctx.needs_input_grad[5]
-        need_map = any(ctx.needs_input_grad[6:])
-        outs, grads = model._launch(rays_o, rays_d, target_s, target_d, noise,
-                                    need_rays or need_map, need_rays, need_map)
-        ctx.grads = grads
-        if outs is None:
-            raise RuntimeError('render_rays: no ray hit any voxel')
-        ret = (outs['losses'], outs['rgb'], outs['depth'], outs['ray_mask'])
-        ctx.mark_non_differentiable(*ret[1:])
-        return ret
-
-    @staticmethod
-    def backward(ctx, g_losses, *_):
-        g = ctx.grads
-        ro, rd, emb, dec = scale_grads([g['d_rays_o'], g['d_rays_d'], g['d_emb'], list(g['d_dec'])],
-                                       upstream_scale(g_losses))
-        return (None, None, None, None, ro, rd, emb, *dec)
 
 
 class SparseVoxel(Model):
@@ -350,12 +328,19 @@ class SparseVoxel(Model):
         noise = input.get('noise')
         fused = torch.is_grad_enabled() and target_s is not None and target_d is not None
         if fused:
+            def launch(needs):
+                need_rays, need_map = needs[0] or needs[1], any(needs[2:])
+                o, g = self._launch(rays_o, rays_d, target_s, target_d, noise,
+                                    need_rays or need_map, need_rays, need_map)
+                if o is None:
+                    raise RuntimeError('render_rays: no ray hit any voxel')
+                grads = None if g is None else \
+                    [g['d_rays_o'], g['d_rays_d'], g['d_emb'], *g['d_dec']]
+                return o['losses'], (o['rgb'], o['depth'], o['ray_mask']), grads
             try:
-                emb, dec = self.embeddings, self.decoder.tensors()
-                if getattr(self, 'freeze_map_grads', False):  # tracking: pose gradients only
-                    emb, dec = emb.detach(), [t.detach() for t in dec]
-                losses, rgb, depth, ray_mask = _VoxStep.apply(
-                    self, target_s, target_d, noise, rays_o, rays_d, emb, *dec)
+                losses, rgb, depth, ray_mask = FusedStep.apply(
+                    launch, None, rays_o, rays_d,
+                    *self.map_inputs(self.embeddings, *self.decoder.tensors()))
             except RuntimeError as e:
                 if 'no ray hit' in str(e):
                     print('\n\n', '!' * 20, 'render_rays. no hit', '!' * 20, '\n\n')
