@@ -264,7 +264,9 @@ size_t xrd_coslam_smoothness_workspace_bytes(int sample_points);
 /* Smoothness / TV regulariser on the hash features (joint_encoding.py:165-197).
  * smooth_rand: HOST [6] = torch.rand(3) ++ torch.rand((1,1,1,3)).  Writes
  * weight*loss to DEVICE loss[0]; if d_table != NULL accumulates
- * grad_scale*weight*dloss/dtable into it (16-byte aligned, as in XrdCoslamGrads). */
+ * grad_scale*weight*dloss/dtable into it (16-byte aligned, as in XrdCoslamGrads).
+ * 3 <= sample_points <= 76 (planes of the lattice's features stay in shared memory), else
+ * XRD_E_SHAPE. */
 /* (xrd_coslam_smoothness_dev: the same with smooth_rand in DEVICE memory, read by the
  * kernels -- for CUDA-graph replay.) */
 int xrd_coslam_smoothness(const XrdHashGrid* grid, int sample_points,

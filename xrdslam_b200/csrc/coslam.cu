@@ -176,8 +176,8 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p) {
 // --------------------------------------------------------------- encoding ---
 
 // Per-level constants, staged in SHARED memory: the level index differs between the lanes
-// of a warp in the hash backward (fragment layout: l = 4 nt + t) and in the smoothness
-// kernels, and a lane-varying index into the kernel-parameter constant bank serialises
+// of a warp in the hash backward (fragment layout: l = 4 nt + t) and in k_encode, and a
+// lane-varying index into the kernel-parameter constant bank serialises
 // (ncu source view: ~20 % of the samples of k_fused sat on these loads).
 struct __align__(16) Lv {
   float scale;
@@ -1652,6 +1652,28 @@ __global__ void k_finalize(FinalizeParams p) {
 }
 
 // ------------------------------------------------------------- smoothness ---
+// One CTA per (level, slab of kSmoothPlanes x planes of the n^3 lattice).  It sweeps its planes
+// with a window of plane features in shared memory: plane x sits in slot x & 3, so the plane
+// written in one step (x + 1) never overwrites one the previous step still reads (x - 2 is its
+// oldest) and one __syncthreads per plane suffices.  A slab recomputes the features of its two
+// boundary planes instead of reading them from a lattice-sized buffer.
+//
+// The lattice is axis-aligned, so a point's cell and weight along an axis depend only on its
+// index along that axis, and the cells a slab touches form a box.  Where that box of table
+// entries fits in shared memory (the coarse levels, where many points share a cell) the CTA
+// loads it once and interpolates from it, and gathers the gradient per vertex: plane x adds to
+// the two vertex planes of its x cell, and each (y, z) vertex sums the points of the rows whose
+// cells touch it (no atomics).  The box leaves with one reduction per touched x pair of entries.
+// Elsewhere each point gathers its 8 corners and scatters to them.
+constexpr int kSmoothThreads = 512, kSmoothPlanes = 4, kSmoothMaxN = 75;  // 5 n^2 float2 fit
+// entries of the shared-memory box (table values + gradient: 16 B each), at most
+constexpr int kSmoothBox = 9216;
+
+struct SmoothHdr {
+  double loss_acc;
+  unsigned int done;  // CTAs that have added their part of the loss
+};
+
 struct SmoothParams {
   GridDev g;
   const float* table;
@@ -1659,94 +1681,194 @@ struct SmoothParams {
   double voxel, off[3], rnd[3];
   const float* rand_dev;  // DEVICE [6] overriding off/rnd (graph replay)
   double offmax[3], margin;
-  float* feat;    // [n^3, 32]
   float* d_table;
-  double* loss_acc;
-  float coef;     // grad_scale * weight / sample_points^3
+  SmoothHdr* hdr;
+  float* loss;
+  float coef;        // grad_scale * weight / sample_points^3
+  float loss_scale;  // weight / sample_points^3
+  int box_cap;       // entries of the shared-memory box this launch has room for
 };
 
-__device__ __forceinline__ void smooth_xn(const SmoothParams& p, int ix, int iy, int iz,
-                                          float xn[3]) {
-  const int c[3] = {ix, iy, iz};
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    // pts = (coords + rand) * voxel + bb_min + offset ; then (pts - bb_min)/(bb_max-bb_min), all f64
-    const double rnd = p.rand_dev ? (double)p.rand_dev[3 + d] : p.rnd[d];
-    const double off = p.rand_dev ? (double)p.rand_dev[d] * p.offmax[d] + p.margin : p.off[d];
-    double pt = ((double)(float)c[d] + rnd) * p.voxel + p.g.bmin[d] + off;
-    xn[d] = (float)((pt - p.g.bmin[d]) / (p.g.bmax[d] - p.g.bmin[d]));
+// normalised coordinate of lattice index i along axis d
+__device__ __forceinline__ float smooth_xn(const SmoothParams& p, int d, int i) {
+  // pts = (coords + rand) * voxel + bb_min + offset ; then (pts - bb_min)/(bb_max-bb_min), all f64
+  const double rnd = p.rand_dev ? (double)p.rand_dev[3 + d] : p.rnd[d];
+  const double off = p.rand_dev ? (double)p.rand_dev[d] * p.offmax[d] + p.margin : p.off[d];
+  const double pt = ((double)(float)i + rnd) * p.voxel + p.g.bmin[d] + off;
+  return (float)((pt - p.g.bmin[d]) / (p.g.bmax[d] - p.g.bmin[d]));
+}
+
+// first i in [0, n) with c[i] >= v, n if none (c nondecreasing)
+__device__ __forceinline__ int first_ge(const int* c, int n, int v) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int m = (lo + hi) >> 1;
+    if (c[m] < v) lo = m + 1; else hi = m;
   }
+  return lo;
 }
 
-__global__ void __launch_bounds__(256) k_smooth_fwd(SmoothParams p) {
-  const int n = p.n, N = n * n * n;
-  __shared__ Lv s_lv[kL];
-  load_levels(s_lv, p.g);
+// Features of one level over the lattice, the squared differences of neighbours (each counted
+// once, from its upper end) and, with d_table, their gradient added to the table.  The last CTA
+// to finish writes loss = loss_scale * sum.  Launched with kSmoothThreads threads and
+// (5 n^2 + 2 box_cap) float2 of dynamic shared memory.
+__global__ void __launch_bounds__(kSmoothThreads) k_smooth_bwd(SmoothParams p) {
+  extern __shared__ float2 s_win[];  // 4 slots of n^2 features | n^2 point gradients | box | box
+  __shared__ float s_xn[3][kSmoothMaxN], s_w[3][kSmoothMaxN];
+  __shared__ uint32_t s_cell[3][kSmoothMaxN];
+  __shared__ int s_c[3][kSmoothMaxN];  // cell relative to the box
+  __shared__ float s_part[kSmoothThreads / 32];
+  __shared__ bool s_last;
+  const int n = p.n, nn = n * n, l = blockIdx.y;
+  Lv L;
+  L.scale = p.g.scale[l]; L.res = p.g.res[l]; L.size = p.g.size[l]; L.offset = p.g.offset[l];
+  L.hashed = p.g.hashed[l]; L.magic = p.g.magic[l];
+  for (int i = threadIdx.x; i < 3 * n; i += blockDim.x) {
+    const int d = i / n, j = i % n;
+    const float xn = smooth_xn(p, d, j);
+    s_xn[d][j] = xn;
+    pos_fract(xn, L.scale, s_w[d][j], s_cell[d][j]);
+  }
   __syncthreads();
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;  // one thread per (point, level)
-  const int pt = q / kL, l = q % kL;
-  if (pt >= N || l >= p.g.n_levels) return;
-  const int iz = pt % n, iy = (pt / n) % n, ix = pt / (n * n);
-  float xn[3];
-  smooth_xn(p, ix, iy, iz, xn);
-  reinterpret_cast<float2*>(p.feat)[(size_t)pt * kL + l] = level_feature(p.table, s_lv[l], xn);
-}
-
-__global__ void __launch_bounds__(256) k_smooth_bwd(SmoothParams p) {
-  __shared__ Lv s_lv[kL];
-  load_levels(s_lv, p.g);
-  __syncthreads();
-  const int n = p.n, N = n * n * n;
-  const int q = blockIdx.x * blockDim.x + threadIdx.x;
-  const int pt = q / kL, l = q % kL;
+  const int x0 = blockIdx.x * kSmoothPlanes, x1 = min(x0 + kSmoothPlanes, n);
+  // the box: cells of planes x0 - 1 .. x1 and of all rows, plus their upper vertex; an even
+  // number of x vertices so that the box leaves in x pairs
+  const uint32_t org[3] = {s_cell[0][max(x0 - 1, 0)], s_cell[1][0], s_cell[2][0]};
+  const int B0 = ((int)(s_cell[0][min(x1, n - 1)] - org[0]) + 3) & ~1;
+  const int B1 = (int)(s_cell[1][n - 1] - org[1]) + 2, B2 = (int)(s_cell[2][n - 1] - org[2]) + 2;
+  const bool box = (long long)B0 * B1 * B2 <= p.box_cap;
+  const bool box_grad = box && p.d_table;
+  const float2* __restrict__ tab = reinterpret_cast<const float2*>(p.table);
+  float2* s_g = s_win + 4 * nn;
+  float2* s_tab = s_g + nn;
+  float2* s_acc = s_tab + p.box_cap;
+  if (box) {
+    for (int i = threadIdx.x; i < 3 * n; i += blockDim.x)
+      s_c[i / n][i % n] = (int)(s_cell[i / n][i % n] - org[i / n]);
+    for (int e = threadIdx.x; e < B0 * B1 * B2; e += blockDim.x) {
+      const int a = e % B0, b = (e / B0) % B1, c = e / (B0 * B1);
+      s_tab[e] = __ldg(&tab[grid_index(L, org[0] + a, org[1] + b, org[2] + c)]);
+      if (box_grad) s_acc[e] = make_float2(0.f, 0.f);
+    }
+    __syncthreads();
+  }
+  auto plane = [&](int x) {
+    float2* s = s_win + (x & 3) * nn;
+    for (int q = threadIdx.x; q < nn; q += blockDim.x) {
+      const int iy = q / n, iz = q % n;
+      if (box) {  // level_feature's arithmetic on the box
+        const float w[3] = {s_w[0][x], s_w[1][iy], s_w[2][iz]};
+        const float2* v = s_tab + s_c[0][x] + B0 * (s_c[1][iy] + B1 * s_c[2][iz]);
+        float f0 = 0.f, f1 = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const float wk = ((k & 1) ? w[0] : 1.f - w[0]) * ((k & 2) ? w[1] : 1.f - w[1]) *
+                           ((k & 4) ? w[2] : 1.f - w[2]);
+          const float2 vk = v[(k & 1) + ((k >> 1) & 1) * B0 + (k >> 2) * B0 * B1];
+          f0 = fmaf(wk, vk.x, f0);
+          f1 = fmaf(wk, vk.y, f1);
+        }
+        s[q] = make_float2(f0, f1);
+      } else {
+        const float xn[3] = {s_xn[0][x], s_xn[1][iy], s_xn[2][iz]};
+        s[q] = level_feature(p.table, L, xn);
+      }
+    }
+  };
+  if (x0 > 0) plane(x0 - 1);
+  plane(x0);
   float part = 0.f;
-  if (pt < N && l < p.g.n_levels) {
-    const int iz = pt % n, iy = (pt / n) % n, ix = pt / (n * n);
-    const float2* F = reinterpret_cast<const float2*>(p.feat);
-    const float2 f = F[(size_t)pt * kL + l];
-    float g0 = 0.f, g1 = 0.f;
-    const int stride[3] = {n * n, n, 1};
-    const int ci[3] = {ix, iy, iz};
+  for (int x = x0; x < x1; ++x) {
+    if (x + 1 < n) plane(x + 1);
+    __syncthreads();
+    const float2* F = s_win + (x & 3) * nn;
+    const float2* nb[3][2] = {{s_win + ((x - 1) & 3) * nn, s_win + ((x + 1) & 3) * nn},
+                              {F - n, F + n}, {F - 1, F + 1}};
+    for (int q = threadIdx.x; q < nn; q += blockDim.x) {
+      const int iy = q / n, iz = q % n;
+      const int ci[3] = {x, iy, iz};
+      const float2 f = F[q];
+      float g0 = 0.f, g1 = 0.f;
 #pragma unroll
-    for (int d = 0; d < 3; ++d) {
-      if (ci[d] > 0) {
-        float2 o = F[(size_t)(pt - stride[d]) * kL + l];
-        float a = f.x - o.x, b = f.y - o.y;
-        g0 += a; g1 += b;
-        part += a * a + b * b;  // each difference counted once (from its upper end)
+      for (int d = 0; d < 3; ++d) {
+        if (ci[d] > 0) {
+          const float2 o = nb[d][0][q];
+          const float a = f.x - o.x, b = f.y - o.y;
+          g0 += a; g1 += b;
+          part += a * a + b * b;
+        }
+        if (ci[d] < n - 1) {
+          const float2 o = nb[d][1][q];
+          g0 -= o.x - f.x; g1 -= o.y - f.y;
+        }
       }
-      if (ci[d] < n - 1) {
-        float2 o = F[(size_t)(pt + stride[d]) * kL + l];
-        g0 -= o.x - f.x; g1 -= o.y - f.y;
+      if (!p.d_table) continue;
+      g0 *= 2.f * p.coef; g1 *= 2.f * p.coef;
+      if (box) {
+        s_g[q] = make_float2(g0, g1);
+      } else {
+        const float xn[3] = {s_xn[0][x], s_xn[1][iy], s_xn[2][iz]};
+        float w[3];
+        uint32_t c[3], idx[8];
+        for (int d = 0; d < 3; ++d) pos_fract(xn[d], L.scale, w[d], c[d]);
+        corner_indices(L, c, idx);
+        scatter_corners(p.d_table, idx, w, g0, g1);
       }
     }
-    if (p.d_table) {
-      g0 *= 2.f * p.coef; g1 *= 2.f * p.coef;
-      float xn[3];
-      smooth_xn(p, ix, iy, iz, xn);
-      float w[3];
-      uint32_t c[3];
-      const Lv L = s_lv[l];
-      for (int d = 0; d < 3; ++d) pos_fract(xn[d], L.scale, w[d], c[d]);
-      uint32_t idx[8];
-      corner_indices(L, c, idx);
-      scatter_corners(p.d_table, idx, w, g0, g1);
+    if (box_grad) {
+      // (y, z) vertex (b, c) of plane x's two x vertices: the points of rows j with
+      // s_c[1][j] in {b - 1, b} and columns k with s_c[2][k] in {c - 1, c}
+      __syncthreads();
+      const float wx = s_w[0][x];
+      float2* t = s_acc + s_c[0][x];
+      for (int v = threadIdx.x; v < B1 * B2; v += blockDim.x) {
+        const int b = v % B1, c = v / B1;
+        const int j0 = first_ge(s_c[1], n, b - 1), j1 = first_ge(s_c[1], n, b + 1);
+        const int k0 = first_ge(s_c[2], n, c - 1), k1 = first_ge(s_c[2], n, c + 1);
+        float a0 = 0.f, a1 = 0.f;
+        for (int j = j0; j < j1; ++j) {
+          const float wy = s_c[1][j] == b ? 1.f - s_w[1][j] : s_w[1][j];
+          for (int k = k0; k < k1; ++k) {
+            const float wyz = wy * (s_c[2][k] == c ? 1.f - s_w[2][k] : s_w[2][k]);
+            const float2 g = s_g[j * n + k];
+            a0 = fmaf(wyz, g.x, a0);
+            a1 = fmaf(wyz, g.y, a1);
+          }
+        }
+        if (a0 != 0.f || a1 != 0.f) {
+          float2* e = t + B0 * v;
+          e[0].x += (1.f - wx) * a0; e[0].y += (1.f - wx) * a1;
+          e[1].x += wx * a0; e[1].y += wx * a1;
+        }
+      }
     }
   }
-  // one double atomic per CTA (per warp it was ~15 k serialised atomics on one address)
-  __shared__ float s_part[8];
+  if (box_grad) {
+    __syncthreads();
+    for (int e = 2 * threadIdx.x; e < B0 * B1 * B2; e += 2 * blockDim.x) {
+      const float2 lo = s_acc[e], hi = s_acc[e + 1];
+      if (lo.x == 0.f && lo.y == 0.f && hi.x == 0.f && hi.y == 0.f) continue;
+      const int a = e % B0, b = (e / B0) % B1, c = e / (B0 * B1);
+      scatter_corner_pair(p.d_table, grid_index(L, org[0] + a, org[1] + b, org[2] + c),
+                          grid_index(L, org[0] + a + 1, org[1] + b, org[2] + c), lo, hi);
+    }
+  }
+  // one double atomic per CTA; the last CTA (ticket after a fence) writes the loss
   part = warp_sum(part);
   if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = part;
   __syncthreads();
   if (threadIdx.x == 0) {
     double a = 0.0;
-    for (int i = 0; i < 8; ++i) a += (double)s_part[i];
-    if (a != 0.0) atomicAdd(p.loss_acc, a);
+    for (int i = 0; i < kSmoothThreads / 32; ++i) a += (double)s_part[i];
+    if (a != 0.0) atomicAdd(&p.hdr->loss_acc, a);
+    __threadfence();
+    s_last = atomicAdd(&p.hdr->done, 1u) == gridDim.x * gridDim.y - 1;
   }
-}
-
-__global__ void k_smooth_finalize(const double* acc, float* loss, float scale) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) loss[0] = (float)(acc[0] * (double)scale);
+  __syncthreads();
+  if (s_last && threadIdx.x == 0) {
+    __threadfence();
+    p.loss[0] = (float)(*(volatile double*)&p.hdr->loss_acc * (double)p.loss_scale);
+  }
 }
 
 // hash encode only
@@ -2067,16 +2189,15 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   return XRD_OK;
 }
 
-// loss_acc in a 256-byte header, then the features of the n^3 cells, n = sample_points - 1
+// the loss accumulator and the CTA counter of k_smooth_bwd
 struct SmoothWs : Carver {
-  SmoothWs(void* base, int sample_points) : Carver(base), n((size_t)(sample_points - 1)) {}
-  const size_t n;
-  double* loss_acc = take<double>(1);
-  float* feat = take_last<float>(n * n * n * 32);
+  explicit SmoothWs(void* base) : Carver(base) {}
+  SmoothHdr* hdr = take_last<SmoothHdr>(1);
 };
 
 extern "C" size_t xrd_coslam_smoothness_workspace_bytes(int sample_points) {
-  return SmoothWs(nullptr, sample_points).bytes();
+  (void)sample_points;
+  return SmoothWs(nullptr).bytes();
 }
 
 static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double voxel_size,
@@ -2084,9 +2205,9 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
                            float* loss, float* d_table, float grad_scale,
                            void* workspace, size_t workspace_bytes, void* stream_) {
   if (!grid || !grid->table || !smooth_rand || !loss || !workspace) return XRD_E_NULL;
-  if (sample_points < 3) return XRD_E_SHAPE;
+  if (sample_points < 3 || sample_points - 1 > kSmoothMaxN) return XRD_E_SHAPE;
   if (d_table && !aligned16(d_table)) return XRD_E_SHAPE;
-  const SmoothWs L(workspace, sample_points);
+  const SmoothWs L(workspace);
   if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
   SmoothParams p;
@@ -2106,19 +2227,31 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
   }
   p.margin = margin;
   p.rand_dev = rand_on_device ? smooth_rand : nullptr;
-  p.loss_acc = L.loss_acc;
-  p.feat = L.feat;
+  p.hdr = L.hdr;
+  p.loss = loss;
   p.d_table = d_table;
   const double sp3 = (double)sample_points * sample_points * sample_points;
   p.coef = (float)((double)grad_scale * (double)weight / sp3);
-  XRD_CUDA_TRY(cudaMemsetAsync(L.loss_acc, 0, 256, stream));
-  const int N = p.n * p.n * p.n;
-  const int blocks = (N * kL + 255) / 256;
-  k_smooth_fwd<<<blocks, 256, 0, stream>>>(p);
-  XRD_LAUNCH_CHECK();
-  k_smooth_bwd<<<blocks, 256, 0, stream>>>(p);
-  XRD_LAUNCH_CHECK();
-  k_smooth_finalize<<<1, 32, 0, stream>>>(p.loss_acc, loss, (float)((double)weight / sp3));
+  p.loss_scale = (float)((double)weight / sp3);
+  // the window and the point gradients, then as large a box as the rest of the SM's shared
+  // memory holds (up to kSmoothBox entries)
+  int dev = 0, smem_optin = 0;
+  cudaFuncAttributes fa;
+  XRD_CUDA_TRY(cudaGetDevice(&dev));
+  XRD_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  XRD_CUDA_TRY(cudaFuncGetAttributes(&fa, k_smooth_bwd));
+  const size_t win = 5 * sizeof(float2) * (size_t)p.n * p.n;
+  const long long room = ((long long)smem_optin - (long long)fa.sharedSizeBytes - (long long)win) /
+                         (2 * (long long)sizeof(float2));
+  if (room < 0) return XRD_E_SHAPE;
+  p.box_cap = (int)(room < kSmoothBox ? room : kSmoothBox);
+  const size_t smem = win + 2 * sizeof(float2) * (size_t)p.box_cap;
+  XRD_CUDA_TRY(cudaFuncSetAttribute(k_smooth_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)smem));
+  // the caller's workspace arrives uninitialised: zero the 16-byte header every call
+  XRD_CUDA_TRY(cudaMemsetAsync(L.hdr, 0, sizeof(SmoothHdr), stream));
+  const dim3 blocks((p.n + kSmoothPlanes - 1) / kSmoothPlanes, p.g.n_levels);
+  k_smooth_bwd<<<blocks, kSmoothThreads, smem, stream>>>(p);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
