@@ -279,6 +279,15 @@ __device__ __forceinline__ float normalise(float p, double bmin, double bmax) {
   return (float)(((double)p - bmin) / (bmax - bmin));
 }
 
+// normalised coordinate of the sample at depth z on ray r: pts = o + d z in f32, as the reference
+__device__ __forceinline__ void sample_xn(const Params& P, int r, float z, float xn[3]) {
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const float pt = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], z));
+    xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
+  }
+}
+
 // quartic kernel cdf / pdf in bin units t (|t| <= 1 inside the kernel support)
 __device__ __forceinline__ float qcdf(float t) {
   float t2 = t * t;
@@ -853,6 +862,164 @@ __device__ __forceinline__ void backward_h1(float* __restrict__ wrec, const floa
   store_c<MASK, L::N>(wrec, L::H1, c);
 }
 
+// Phase 2 of both fused kernels for ray rr, one warp: the composite of its S samples (raw: the RAW
+// slots of their records, stride N; zr: their z values), the per-ray outputs and, with BWD,
+// d loss / d raw in RAW[0..3].  Per sample the five sigmoids are evaluated once: colours overwrite
+// the rgb logits in RAW[0..2].  Lane owns samples kk = lane + 32 i, whose sigma(s/tr) and
+// unnormalised weight u are kept
+//   KPL > 0:  in registers, index i (the loops unroll over i < KPL; S <= 32 KPL);
+//   KPL == 0: in the caller's shared arrays sg_s, u_s of S floats, index kk, in loops that are
+//             not unrolled (the tile kernel: unrolled for its S <= 256 it is ~1400 instructions
+//             longer and slower).
+// Lane 0 hands the ray's loss partials to add_loss(term, v) (terms as in loss_acc: 0 rgb, 1 depth,
+// only for rays with valid depth, 2 sdf, 3 fs) as soon as each is known, so that none stays live
+// across the sample loops.
+// (The RAW-slot pointer, rather than the record base, keeps k_fused_g at 96 registers and an
+// 8-byte stack: with the record base, ptxas reloads a spilled address inside dw_tile's loop.)
+template <int N, bool BWD, int KPL, typename AddLoss>
+__device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& ln, float* raw,
+                                              const float* zr, float* sg_s, float* u_s, int rr,
+                                              int lane, AddLoss add_loss) {
+  constexpr int UNROLL = KPL > 0 ? KPL : 1;
+  const int S = P.S;
+  const int n = KPL > 0 ? KPL : (S + 31) / 32;  // samples per lane
+  const float tr = P.trunc;
+  float sg_reg[UNROLL], u_reg[UNROLL];
+  float* sg_r = KPL > 0 ? sg_reg : sg_s;
+  float* u_r = KPL > 0 ? u_reg : u_s;
+  int first = 0x7fffffff;
+#pragma unroll UNROLL
+  for (int i = 0; i < n; ++i) {
+    const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+    if (KPL > 0) {
+      sg_r[j] = 0.f;
+      u_r[j] = 0.f;
+    }
+    if (kk < S) {
+      float* rp = raw + kk * N;
+      const float s = rp[3];
+      const float sg = sigmoidf_acc(s / tr);
+      sg_r[j] = sg;
+      u_r[j] = sg * sigmoidf_acc((-s) / tr);
+      rp[0] = sigmoidf_acc(rp[0]);
+      rp[1] = sigmoidf_acc(rp[1]);
+      rp[2] = sigmoidf_acc(rp[2]);
+      if (kk < S - 1 && raw[(kk + 1) * N + 3] * s < 0.f) first = min(first, kk);
+    }
+  }
+  first = warp_min_i(first);
+  if (first == 0x7fffffff) first = 0;
+  __syncwarp();
+  const float zlim = zr[first] + P.trunc;
+  float usum = 0.f;
+#pragma unroll UNROLL
+  for (int i = 0; i < n; ++i) {
+    const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+    if (kk < S) {
+      const float u = (zr[kk] < zlim) ? u_r[j] : 0.f;
+      u_r[j] = u;
+      usum += u;
+    }
+  }
+  usum = warp_sum(usum);
+  const float W = usum + 1e-8f;
+  float o_r = 0.f, o_g = 0.f, o_b = 0.f, o_d = 0.f, o_acc = 0.f;
+#pragma unroll UNROLL
+  for (int i = 0; i < n; ++i) {
+    const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+    if (kk < S) {
+      const float* rp = raw + kk * N;
+      const float w = u_r[j] / W;
+      o_r = fmaf(w, rp[0], o_r);
+      o_g = fmaf(w, rp[1], o_g);
+      o_b = fmaf(w, rp[2], o_b);
+      o_d = fmaf(w, zr[kk], o_d);
+      o_acc += w;
+    }
+  }
+  o_r = warp_sum(o_r); o_g = warp_sum(o_g); o_b = warp_sum(o_b);
+  o_d = warp_sum(o_d); o_acc = warp_sum(o_acc);
+  if (P.depth_var) {
+    float v = 0.f;
+#pragma unroll UNROLL
+    for (int i = 0; i < n; ++i) {
+      const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+      if (kk < S) {
+        const float dz = zr[kk] - o_d;
+        v = fmaf(u_r[j] / W, dz * dz, v);
+      }
+    }
+    v = warp_sum(v);
+    if (lane == 0) P.depth_var[rr] = v;
+  }
+  if (lane == 0) {
+    if (P.rgb) { P.rgb[rr * 3] = o_r; P.rgb[rr * 3 + 1] = o_g; P.rgb[rr * 3 + 2] = o_b; }
+    if (P.depth) P.depth[rr] = o_d;
+    if (P.acc) P.acc[rr] = o_acc;
+    if (P.disp) P.disp[rr] = 1.0f / fmaxf(1e-10f, o_d / o_acc);
+  }
+  if (BWD) {
+    const float td = P.target_d[rr];
+    const float tr_ = P.target_s[rr * 3], tg_ = P.target_s[rr * 3 + 1],
+                tb_ = P.target_s[rr * 3 + 2];
+    const bool valid = (td > 0.f) && (td < P.depth_trunc);
+    const float RS = (float)P.Rg * (float)S;
+    const float c_rgb = P.ls[0] * P.w_rgb * 2.0f / (3.0f * (float)P.Rg);
+    const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
+    const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * ln.inv_nvalid : 0.f;
+    if (lane == 0) {
+      add_loss(0, (o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) + (o_b - tb_) * (o_b - tb_));
+      if (valid) add_loss(1, (o_d - td) * (o_d - td));
+    }
+    float qw = 0.f;
+#pragma unroll UNROLL
+    for (int i = 0; i < n; ++i) {
+      const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+      if (kk < S) {
+        const float* rp = raw + kk * N;
+        const float q_ = g_r * rp[0] + g_g * rp[1] + g_b * rp[2] + g_d * zr[kk];
+        qw = fmaf(q_, u_r[j] / W, qw);
+      }
+    }
+    qw = warp_sum(qw);
+    float a_fs = 0.f, a_sdf = 0.f;
+    const float c_fs = P.ls[3] * P.w_fs * ln.fs_w * 2.0f / RS;
+    const float c_sdf = P.ls[2] * P.w_sdf * ln.sdf_w * 2.0f / RS;
+#pragma unroll UNROLL
+    for (int i = 0; i < n; ++i) {
+      const int kk = lane + 32 * i, j = KPL > 0 ? i : kk;
+      if (kk >= S) continue;
+      float* rp = raw + kk * N;
+      const float z = zr[kk];
+      const float s = rp[3];
+      const float sg = sg_r[j];
+      const float u = u_r[j];  // a * mask
+      const float w = u / W;
+      const float c0 = rp[0], c1 = rp[1], c2 = rp[2];
+      const float q_ = g_r * c0 + g_g * c1 + g_b * c2 + g_d * z;
+      float ds = (q_ - qw) / W * u * (1.f - 2.f * sg) / tr;
+      const bool front = z < __fsub_rn(td, P.trunc);
+      const bool back = z > __fadd_rn(td, P.trunc);
+      if (front) {
+        ds += c_fs * (s - 1.f);
+        a_fs += (s - 1.f) * (s - 1.f);
+      }
+      if (!front && !back && td > 0.f) {
+        float e = (z + s * P.trunc) - td;
+        ds += c_sdf * e * P.trunc;
+        a_sdf += e * e;
+      }
+      rp[0] = g_r * w * c0 * (1.f - c0);
+      rp[1] = g_g * w * c1 * (1.f - c1);
+      rp[2] = g_b * w * c2 * (1.f - c2);
+      rp[3] = ds;
+    }
+    a_fs = warp_sum(a_fs);
+    a_sdf = warp_sum(a_sdf);
+    if (lane == 0) { add_loss(3, a_fs); add_loss(2, a_sdf); }
+  }
+}
+
 // ----------------------------------------------------------------- fused ---
 template <bool BWD, bool PREC3, bool BPREC3, int SLOTS>
 __global__ void __launch_bounds__(256) k_fused(const Params P) {
@@ -874,7 +1041,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
   // the 8 pad records after the tile stay zero for the whole kernel (k-step overrun of dw_tile)
   for (int q = tid; q < 8 * REC; q += blockDim.x) recs[blockDim.x * REC + q] = 0.f;
   const LossNorm ln = BWD ? loss_norm(P.counts) : LossNorm{};
-  double l_rgb = 0.0, l_depth = 0.0, l_sdf = 0.0, l_fs = 0.0;
+  double l_sum[4] = {0.0, 0.0, 0.0, 0.0};  // loss sums of this thread (lane 0 of each warp)
   float dwacc[SLOTS][4];
 #pragma unroll
   for (int j = 0; j < SLOTS; ++j)
@@ -902,12 +1069,9 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     if (active) {
       zv = P.z_vals[(size_t)r * S + k];
       zbuf[tid] = zv;
+      sample_xn(P, r, zv, xn);
 #pragma unroll
-      for (int d = 0; d < 3; ++d) {
-        float pt = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], zv));
-        xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
-        xnb[tid * 3 + d] = xn[d];
-      }
+      for (int d = 0; d < 3; ++d) xnb[tid * 3 + d] = xn[d];
       encode<1>(P.table, P.g.n_levels, s_lv, xn, rec, 0);
       blob_forward(xn, rec);
     } else {
@@ -927,121 +1091,10 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     }
     __syncthreads();
     // ---------------- phase 2: per-ray composite, loss, d loss / d raw ----
-    // per sample the five sigmoids are evaluated once: colours overwrite the rgb logits in
-    // RAW[0..2]; sigma(s/tr) and the unnormalised weight u live in sgb / ub.
-    for (int q = warp; q < nr; q += nwarps) {
-      const int rr = r0 + q;
-      const float* zr = zbuf + q * S;
-      float* sg_r = sgb + q * S;
-      float* u_r = ub + q * S;
-      float* rq = recs + (size_t)(q * S) * REC;
-      const float tr = P.trunc;
-      int first = 0x7fffffff;
-      for (int kk = lane; kk < S; kk += 32) {
-        float* rp = rq + kk * REC + R_RAW;
-        const float s = rp[3];
-        const float sg = sigmoidf_acc(s / tr);
-        sg_r[kk] = sg;
-        u_r[kk] = sg * sigmoidf_acc((-s) / tr);
-        rp[0] = sigmoidf_acc(rp[0]);
-        rp[1] = sigmoidf_acc(rp[1]);
-        rp[2] = sigmoidf_acc(rp[2]);
-        if (kk < S - 1 && rq[(kk + 1) * REC + R_RAW + 3] * s < 0.f) first = min(first, kk);
-      }
-      first = warp_min_i(first);
-      if (first == 0x7fffffff) first = 0;
-      __syncwarp();
-      const float zlim = zr[first] + P.trunc;
-      float usum = 0.f;
-      for (int kk = lane; kk < S; kk += 32) {
-        const float u = (zr[kk] < zlim) ? u_r[kk] : 0.f;
-        u_r[kk] = u;
-        usum += u;
-      }
-      usum = warp_sum(usum);
-      const float W = usum + 1e-8f;
-      float o_r = 0.f, o_g = 0.f, o_b = 0.f, o_d = 0.f, o_acc = 0.f;
-      for (int kk = lane; kk < S; kk += 32) {
-        const float* rp = rq + kk * REC + R_RAW;
-        const float w = u_r[kk] / W;
-        o_r = fmaf(w, rp[0], o_r);
-        o_g = fmaf(w, rp[1], o_g);
-        o_b = fmaf(w, rp[2], o_b);
-        o_d = fmaf(w, zr[kk], o_d);
-        o_acc += w;
-      }
-      o_r = warp_sum(o_r); o_g = warp_sum(o_g); o_b = warp_sum(o_b);
-      o_d = warp_sum(o_d); o_acc = warp_sum(o_acc);
-      if (P.depth_var) {
-        float v = 0.f;
-        for (int kk = lane; kk < S; kk += 32) {
-          const float dz = zr[kk] - o_d;
-          v = fmaf(u_r[kk] / W, dz * dz, v);
-        }
-        v = warp_sum(v);
-        if (lane == 0) P.depth_var[rr] = v;
-      }
-      if (lane == 0) {
-        if (P.rgb) { P.rgb[rr * 3] = o_r; P.rgb[rr * 3 + 1] = o_g; P.rgb[rr * 3 + 2] = o_b; }
-        if (P.depth) P.depth[rr] = o_d;
-        if (P.acc) P.acc[rr] = o_acc;
-        if (P.disp) P.disp[rr] = 1.0f / fmaxf(1e-10f, o_d / o_acc);
-      }
-      if (BWD) {
-        const float td = P.target_d[rr];
-        const float tr_ = P.target_s[rr * 3], tg_ = P.target_s[rr * 3 + 1],
-                    tb_ = P.target_s[rr * 3 + 2];
-        const bool valid = (td > 0.f) && (td < P.depth_trunc);
-        const float RS = (float)P.Rg * (float)S;
-        const float c_rgb = P.ls[0] * P.w_rgb * 2.0f / (3.0f * (float)P.Rg);
-        const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
-        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * ln.inv_nvalid : 0.f;
-        if (lane == 0) {
-          l_rgb += (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
-                            (o_b - tb_) * (o_b - tb_));
-          if (valid) l_depth += (double)((o_d - td) * (o_d - td));
-        }
-        float qw = 0.f;
-        for (int kk = lane; kk < S; kk += 32) {
-          const float* rp = rq + kk * REC + R_RAW;
-          const float q_ = g_r * rp[0] + g_g * rp[1] + g_b * rp[2] + g_d * zr[kk];
-          qw = fmaf(q_, u_r[kk] / W, qw);
-        }
-        qw = warp_sum(qw);
-        float a_fs = 0.f, a_sdf = 0.f;
-        const float c_fs = P.ls[3] * P.w_fs * ln.fs_w * 2.0f / RS;
-        const float c_sdf = P.ls[2] * P.w_sdf * ln.sdf_w * 2.0f / RS;
-        for (int kk = lane; kk < S; kk += 32) {
-          float* rp = rq + kk * REC + R_RAW;
-          const float z = zr[kk];
-          const float s = rp[3];
-          const float sg = sg_r[kk];
-          const float u = u_r[kk];  // a * mask
-          const float w = u / W;
-          const float c0 = rp[0], c1 = rp[1], c2 = rp[2];
-          const float q_ = g_r * c0 + g_g * c1 + g_b * c2 + g_d * z;
-          float ds = (q_ - qw) / W * u * (1.f - 2.f * sg) / tr;
-          const bool front = z < __fsub_rn(td, P.trunc);
-          const bool back = z > __fadd_rn(td, P.trunc);
-          if (front) {
-            ds += c_fs * (s - 1.f);
-            a_fs += (s - 1.f) * (s - 1.f);
-          }
-          if (!front && !back && td > 0.f) {
-            float e = (z + s * P.trunc) - td;
-            ds += c_sdf * e * P.trunc;
-            a_sdf += e * e;
-          }
-          rp[0] = g_r * w * c0 * (1.f - c0);
-          rp[1] = g_g * w * c1 * (1.f - c1);
-          rp[2] = g_b * w * c2 * (1.f - c2);
-          rp[3] = ds;
-        }
-        a_fs = warp_sum(a_fs);
-        a_sdf = warp_sum(a_sdf);
-        if (lane == 0) { l_fs += (double)a_fs; l_sdf += (double)a_sdf; }
-      }
-    }
+    for (int q = warp; q < nr; q += nwarps)
+      composite_ray<REC, BWD, 0>(P, ln, recs + (size_t)(q * S) * REC + R_RAW, zbuf + q * S,
+                                 sgb + q * S, ub + q * S, r0 + q, lane,
+                                 [&](int i, float v) { l_sum[i] += (double)v; });
     __syncthreads();
     if (!BWD) continue;
     // ---------------- phase 3: backward ----------------------------------
@@ -1170,10 +1223,9 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
 
   if (BWD) {
     if (lane == 0) {
-      if (l_rgb != 0.0) atomicAdd(&P.loss_acc[0], l_rgb);
-      if (l_depth != 0.0) atomicAdd(&P.loss_acc[1], l_depth);
-      if (l_sdf != 0.0) atomicAdd(&P.loss_acc[2], l_sdf);
-      if (l_fs != 0.0) atomicAdd(&P.loss_acc[3], l_fs);
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if (l_sum[i] != 0.0) atomicAdd(&P.loss_acc[i], l_sum[i]);
     }
     if (map_grads) {
 #pragma unroll
@@ -1294,11 +1346,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     // ---------------- phase 1: forward -------------------------------------
     if (active) {
       zv = P.z_vals[(size_t)r * S + k];
-#pragma unroll
-      for (int d = 0; d < 3; ++d) {
-        float pt = __fadd_rn(P.rays_o[r * 3 + d], __fmul_rn(P.rays_d[r * 3 + d], zv));
-        xn[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
-      }
+      sample_xn(P, r, zv, xn);
       if (half == 0) zbuf[p] = zv;
       encode<2>(P.table, P.g.n_levels, s_lv, xn, rec, half);
       // OneBlob dims 0, 1 (half 0) and 2 (half 1); constant indices keep xn in registers
@@ -1326,145 +1374,10 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
     }
     group_sync(grp);
     // ---------------- phase 2: per-ray composite, loss, d loss / d raw ----
-    // lane owns samples lane + 32 i (i < G_KPL): sigma(s/tr) and the unnormalised weight u stay
-    // in registers
-    for (int q = gw; q < nr; q += GW) {
-      const int rr = r0 + q;
-      const float* zr = zbuf + q * S;
-      float* rq = recs + (size_t)(q * S) * GREC;
-      const float tr = P.trunc;
-      float sg_r[G_KPL], u_r[G_KPL];
-      int first = 0x7fffffff;
-#pragma unroll
-      for (int i = 0; i < G_KPL; ++i) {
-        const int kk = lane + 32 * i;
-        sg_r[i] = 0.f;
-        u_r[i] = 0.f;
-        if (kk < S) {
-          float* rp = rq + kk * GREC + G_RAW;
-          const float s = rp[3];
-          const float sg = sigmoidf_acc(s / tr);
-          sg_r[i] = sg;
-          u_r[i] = sg * sigmoidf_acc((-s) / tr);
-          rp[0] = sigmoidf_acc(rp[0]);
-          rp[1] = sigmoidf_acc(rp[1]);
-          rp[2] = sigmoidf_acc(rp[2]);
-          if (kk < S - 1 && rq[(kk + 1) * GREC + G_RAW + 3] * s < 0.f) first = min(first, kk);
-        }
-      }
-      first = warp_min_i(first);
-      if (first == 0x7fffffff) first = 0;
-      __syncwarp();
-      const float zlim = zr[first] + P.trunc;
-      float usum = 0.f;
-#pragma unroll
-      for (int i = 0; i < G_KPL; ++i) {
-        const int kk = lane + 32 * i;
-        if (kk < S) {
-          const float u = (zr[kk] < zlim) ? u_r[i] : 0.f;
-          u_r[i] = u;
-          usum += u;
-        }
-      }
-      usum = warp_sum(usum);
-      const float W = usum + 1e-8f;
-      float o_r = 0.f, o_g = 0.f, o_b = 0.f, o_d = 0.f, o_acc = 0.f;
-#pragma unroll
-      for (int i = 0; i < G_KPL; ++i) {
-        const int kk = lane + 32 * i;
-        if (kk < S) {
-          const float* rp = rq + kk * GREC + G_RAW;
-          const float w = u_r[i] / W;
-          o_r = fmaf(w, rp[0], o_r);
-          o_g = fmaf(w, rp[1], o_g);
-          o_b = fmaf(w, rp[2], o_b);
-          o_d = fmaf(w, zr[kk], o_d);
-          o_acc += w;
-        }
-      }
-      o_r = warp_sum(o_r); o_g = warp_sum(o_g); o_b = warp_sum(o_b);
-      o_d = warp_sum(o_d); o_acc = warp_sum(o_acc);
-      if (P.depth_var) {
-        float v = 0.f;
-#pragma unroll
-        for (int i = 0; i < G_KPL; ++i) {
-          const int kk = lane + 32 * i;
-          if (kk < S) {
-            const float dz = zr[kk] - o_d;
-            v = fmaf(u_r[i] / W, dz * dz, v);
-          }
-        }
-        v = warp_sum(v);
-        if (lane == 0) P.depth_var[rr] = v;
-      }
-      if (lane == 0) {
-        if (P.rgb) { P.rgb[rr * 3] = o_r; P.rgb[rr * 3 + 1] = o_g; P.rgb[rr * 3 + 2] = o_b; }
-        if (P.depth) P.depth[rr] = o_d;
-        if (P.acc) P.acc[rr] = o_acc;
-        if (P.disp) P.disp[rr] = 1.0f / fmaxf(1e-10f, o_d / o_acc);
-      }
-      if (BWD) {
-        const float td = P.target_d[rr];
-        const float tr_ = P.target_s[rr * 3], tg_ = P.target_s[rr * 3 + 1],
-                    tb_ = P.target_s[rr * 3 + 2];
-        const bool valid = (td > 0.f) && (td < P.depth_trunc);
-        const float RS = (float)P.Rg * (float)S;
-        const float c_rgb = P.ls[0] * P.w_rgb * 2.0f / (3.0f * (float)P.Rg);
-        const float g_r = c_rgb * (o_r - tr_), g_g = c_rgb * (o_g - tg_), g_b = c_rgb * (o_b - tb_);
-        const float g_d = valid ? P.ls[1] * P.w_depth * 2.0f * (o_d - td) * ln.inv_nvalid : 0.f;
-        if (lane == 0) {
-          atomicAdd(&s_loss[0], (double)((o_r - tr_) * (o_r - tr_) + (o_g - tg_) * (o_g - tg_) +
-                                         (o_b - tb_) * (o_b - tb_)));
-          if (valid) atomicAdd(&s_loss[1], (double)((o_d - td) * (o_d - td)));
-        }
-        float qw = 0.f;
-#pragma unroll
-        for (int i = 0; i < G_KPL; ++i) {
-          const int kk = lane + 32 * i;
-          if (kk < S) {
-            const float* rp = rq + kk * GREC + G_RAW;
-            const float q_ = g_r * rp[0] + g_g * rp[1] + g_b * rp[2] + g_d * zr[kk];
-            qw = fmaf(q_, u_r[i] / W, qw);
-          }
-        }
-        qw = warp_sum(qw);
-        float a_fs = 0.f, a_sdf = 0.f;
-        const float c_fs = P.ls[3] * P.w_fs * ln.fs_w * 2.0f / RS;
-        const float c_sdf = P.ls[2] * P.w_sdf * ln.sdf_w * 2.0f / RS;
-#pragma unroll
-        for (int i = 0; i < G_KPL; ++i) {
-          const int kk = lane + 32 * i;
-          if (kk >= S) continue;
-          float* rp = rq + kk * GREC + G_RAW;
-          const float z = zr[kk];
-          const float s = rp[3];
-          const float sg = sg_r[i];
-          const float u = u_r[i];  // a * mask
-          const float w = u / W;
-          const float c0 = rp[0], c1 = rp[1], c2 = rp[2];
-          const float q_ = g_r * c0 + g_g * c1 + g_b * c2 + g_d * z;
-          float ds = (q_ - qw) / W * u * (1.f - 2.f * sg) / tr;
-          const bool front = z < __fsub_rn(td, P.trunc);
-          const bool back = z > __fadd_rn(td, P.trunc);
-          if (front) {
-            ds += c_fs * (s - 1.f);
-            a_fs += (s - 1.f) * (s - 1.f);
-          }
-          if (!front && !back && td > 0.f) {
-            float e = (z + s * P.trunc) - td;
-            ds += c_sdf * e * P.trunc;
-            a_sdf += e * e;
-          }
-          rp[0] = g_r * w * c0 * (1.f - c0);
-          rp[1] = g_g * w * c1 * (1.f - c1);
-          rp[2] = g_b * w * c2 * (1.f - c2);
-          rp[3] = ds;
-        }
-        a_fs = warp_sum(a_fs);
-        a_sdf = warp_sum(a_sdf);
-        if (lane == 0) { atomicAdd(&s_loss[3], (double)a_fs); atomicAdd(&s_loss[2], (double)a_sdf); }
-      }
-    }
+    for (int q = gw; q < nr; q += GW)
+      composite_ray<GREC, BWD, G_KPL>(P, ln, recs + (size_t)(q * S) * GREC + G_RAW, zbuf + q * S,
+                                      nullptr, nullptr, r0 + q, lane,
+                                      [&](int i, float v) { atomicAdd(&s_loss[i], (double)v); });
     if (!BWD) continue;  // the barrier at the top of the loop orders the next unit
     group_sync(grp);
     // ---------------- phase 3: backward ----------------------------------
@@ -1544,15 +1457,7 @@ __global__ void __launch_bounds__(GT * NGROUPS, 1) k_fused_g(const Params P, int
       float dxh[3] = {0.f, 0.f, 0.f};
       float xq[3] = {0.f, 0.f, 0.f};
       const float zq = act2 ? zbuf[pp] : 0.f;
-      if (act2) {
-        // xn of point pp, recomputed exactly as in the forward
-        const int rq = r0 + pp / S;
-#pragma unroll
-        for (int d = 0; d < 3; ++d) {
-          const float pt = __fadd_rn(P.rays_o[rq * 3 + d], __fmul_rn(P.rays_d[rq * 3 + d], zq));
-          xq[d] = normalise(pt, P.g.bmin[d], P.g.bmax[d]);
-        }
-      }
+      if (act2) sample_xn(P, r0 + pp / S, zq, xq);  // xn of point pp, exactly as in the forward
       if (act2 && (map_grads || need_dx)) {
 #pragma unroll 1
         for (int i2 = 0; i2 < kL / 2; i2 += 2) {  // two levels per call: half + 2 i2, half + 2 i2 + 2
