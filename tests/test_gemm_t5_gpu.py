@@ -1,4 +1,4 @@
-"""The Hopper-native GEMM (csrc/gemm_t5.cuh: wgmma.mma_async tf32 + TMA + mbarrier, 3xTF32)
+"""The Hopper-native GEMM (csrc/mlp.cu: wgmma.mma_async tf32 + TMA + mbarrier, 3xTF32)
 against float64 matmul and against the mma.sync path, on the shapes of the Vox-Fusion decoder and
 the Point-SLAM colour trunk (forward and transposed-weight backward GEMMs, ragged N, masks)."""
 import pytest

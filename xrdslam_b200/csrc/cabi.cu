@@ -7,9 +7,7 @@
 
 namespace xrd {
 thread_local int g_last_cuda_error = 0;
-thread_local int g_gemm_mode = 1;  // gemm.cuh: arithmetic of the wide-MLP GEMMs (per calling thread)
 thread_local cudaEvent_t g_ev_start = nullptr, g_ev_stop = nullptr;
-namespace t5 { thread_local int g_t5_variant = 0; }
 
 int num_sms() {
   static int cached[64] = {0};
@@ -39,17 +37,6 @@ int copy_totals(int32_t* counts, const int* a, const int* b, cudaStream_t stream
 extern "C" int xrd_abi_version(void) { return XRD_ABI_VERSION; }
 
 extern "C" int xrd_last_cuda_error(void) { return xrd::g_last_cuda_error; }
-
-extern "C" int xrd_debug_gemm_mode(int mode) {
-  if (mode < 0 || mode > 3) return XRD_E_SHAPE;
-  xrd::g_gemm_mode = mode;
-  return XRD_OK;
-}
-
-extern "C" int xrd_debug_gemm_variant(int variant) {
-  xrd::t5::g_t5_variant = variant;
-  return XRD_OK;
-}
 
 extern "C" int xrd_debug_kernel_events(void* start_event, void* stop_event) {
   xrd::g_ev_start = (cudaEvent_t)start_event;

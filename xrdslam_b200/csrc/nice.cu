@@ -26,8 +26,8 @@
 //   k_rayreduce     d loss / d rays_o, d rays_d
 #include <math.h>
 
-#include "common.cuh"
-#include "dw.cuh"
+#include "mlp.cuh"
+#include "nice.cuh"
 
 namespace xrd {
 namespace nice {
@@ -60,35 +60,6 @@ __host__ __device__ inline WOff woff(int c_dim) {
   o.total = q;
   return o;
 }
-
-struct Grid {
-  const float* data;
-  float* grad;
-  int nx, ny, nz;
-};
-
-struct DecParams {
-  int P, S;
-  const double* z;
-  const float *rays_o, *rays_d;
-  double bmin[3], bmax[3];
-  Grid ga;          // own grid
-  Grid gb;          // fine decoder: the middle grid (no gradient); data == NULL otherwise
-  XrdNiceDecoder dec;
-  // outputs / inputs per point (SoA)
-  float* out[4];        // fwd: out[k][p] (n_out rows)
-  const float* dout[4]; // bwd: d loss / d out[k][p]
-  uint32_t* masks;      // [5][P]
-  float* acts;          // trainable: rows of Pp floats: e[93] h0..h4[160] c[c_dim] | bwd: dh[160] gm[93] pf[3]
-  int Pp;
-  float* dp;            // [3][P] d loss / d point, accumulated across the decoder passes
-  int need_dp;
-  // Point-SLAM reuses this decoder with a kNN-interpolated feature instead of a grid:
-  const float* zf;      // float32 sample depths (z == NULL)
-  const float* ext_c;   // [c_dim][P] feature rows (ga.data == NULL)
-  float* ext_dc;        // [c_dim][P] gradient w.r.t. the feature rows
-  float embed_scale;    // 1 (NICE: sin(p B)) or 2*pi (Point-SLAM: sin(2 pi p B))
-};
 
 // rows of the activation workspace (trainable decoder)
 __host__ __device__ inline int row_e() { return 0; }
@@ -556,6 +527,16 @@ static __global__ void __launch_bounds__(T) k_decoder_bwd(const DecParams P) {
   }
 }
 
+cudaError_t launch_decoder(const DecParams& D, bool bwd, cudaStream_t stream) {
+  const size_t smem = sizeof(float) * ((size_t)woff(D.dec.c_dim).total + (size_t)(E + CMAX) * T);
+  void (*k)(const DecParams) = bwd ? k_decoder_bwd : k_decoder_fwd;
+  const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  const int n_tiles = (D.P + T - 1) / T, sms = num_sms();
+  k<<<n_tiles < sms ? n_tiles : sms, T, smem, stream>>>(D);
+  return cudaGetLastError();
+}
+
 // --------------------------------------------------- coarse level (N6) ---
 // MLP_no_xyz (decoder_nice.py:237-320): h = c; 5 x [h = relu(W h + b)], [c, h] re-concatenated
 // after block 2, occupancy = w_out h + b_out.  The grid feature c is sampled with the COARSE
@@ -924,7 +905,6 @@ static __global__ void __launch_bounds__(128) k_rayreduce(int R, int S, int P, c
 }  // namespace nice
 }  // namespace xrd
 
-#ifndef XRD_NICE_KERNELS_ONLY
 using namespace xrd;
 using namespace xrd::nice;
 
@@ -992,40 +972,28 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   k_sample<<<(R + 3) / 4, 128, 0, stream>>>(sp);
   XRD_LAUNCH_CHECK();
 
-  const int sms = num_sms();
+  const bool train_color = grads && grads->d_color && stage == XRD_NICE_COLOR;
   auto dec_params = [&](int d) {
     DecParams D;
     D.P = P; D.S = S; D.z = z; D.rays_o = rays->rays_o; D.rays_d = rays->rays_d;
     for (int k = 0; k < 3; ++k) { D.bmin[k] = cfg->bound_min[k]; D.bmax[k] = cfg->bound_max[k]; }
-    D.ga.data = grids[d].data; D.ga.nx = grids[d].nx; D.ga.ny = grids[d].ny; D.ga.nz = grids[d].nz;
-    D.ga.grad = (grads && grads->d_grid[d]) ? grads->d_grid[d] : nullptr;
-    D.gb.data = nullptr; D.gb.grad = nullptr; D.gb.nx = D.gb.ny = D.gb.nz = 1;
-    if (d == 1) { D.gb.data = grids[0].data; D.gb.nx = grids[0].nx; D.gb.ny = grids[0].ny; D.gb.nz = grids[0].nz; }
+    D.ga = {grids[d].data, grads ? grads->d_grid[d] : nullptr, grids[d].nx, grids[d].ny, grids[d].nz};
+    if (d == 1) D.gb = {grids[0].data, nullptr, grids[0].nx, grids[0].ny, grids[0].nz};
     D.dec = decoders[d];
-    for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
     D.masks = grads ? L.masks + (size_t)d * 5 * P : nullptr;
-    D.acts = nullptr; D.Pp = Pp;
+    if (d == 2 && train_color) { D.acts = L.acts; D.Pp = Pp; }
     D.dp = L.dp;
     D.need_dp = grads && (grads->d_rays_o || grads->d_rays_d);
-    D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
     return D;
   };
-  auto dec_smem = [&](int c_dim) { return sizeof(float) * ((size_t)woff(c_dim).total + (size_t)(E + CMAX) * T); };
-  const int n_tiles = (P + T - 1) / T;
-  const int gridx = n_tiles < sms ? n_tiles : sms;
-  const bool train_color = grads && grads->d_color && stage == XRD_NICE_COLOR;
 
   for (int d = 0; d <= stage; ++d) {
     DecParams D = dec_params(d);
     if (d == 0) D.out[0] = occ_mid;
     if (d == 1) D.out[0] = occ_fine;
-    if (d == 2) { D.out[0] = rgb; D.out[1] = rgb + P; D.out[2] = rgb + 2 * (size_t)P; D.out[3] = nullptr; }
-    if (d == 2 && train_color) D.acts = L.acts;
-    const size_t smem = dec_smem(decoders[d].c_dim);
-    XRD_CUDA_TRY(cudaFuncSetAttribute(k_decoder_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (d == 2) { D.out[0] = rgb; D.out[1] = rgb + P; D.out[2] = rgb + 2 * (size_t)P; }
     KernelTimer kt(stream);
-    k_decoder_fwd<<<gridx, T, smem, stream>>>(D);
-    XRD_LAUNCH_CHECK();
+    XRD_CUDA_TRY(launch_decoder(D, false, stream));
   }
 
   CompParams C;
@@ -1061,12 +1029,8 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   for (int d = 0; d <= stage; ++d) {
     DecParams D = dec_params(d);
     if (d < 2) D.dout[0] = C.d_occ;
-    else { D.dout[0] = C.d_rgb[0]; D.dout[1] = C.d_rgb[1]; D.dout[2] = C.d_rgb[2]; D.dout[3] = nullptr; }
-    if (d == 2 && train_color) D.acts = L.acts;
-    const size_t smem = dec_smem(decoders[d].c_dim);
-    XRD_CUDA_TRY(cudaFuncSetAttribute(k_decoder_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_decoder_bwd<<<gridx, T, smem, stream>>>(D);
-    XRD_LAUNCH_CHECK();
+    else { D.dout[0] = C.d_rgb[0]; D.dout[1] = C.d_rgb[1]; D.dout[2] = C.d_rgb[2]; }
+    XRD_CUDA_TRY(launch_decoder(D, true, stream));
   }
 
   if (train_color) {
@@ -1145,28 +1109,17 @@ extern "C" int xrd_nice_query(const float* points, int n_points, const XrdNiceGr
   // point = rays_o + rays_d * z with rays_o = the query point, rays_d = 0, z = 0 (exact)
   XRD_CUDA_TRY(cudaMemsetAsync(L.z, 0, (size_t)P * 8, stream));
   XRD_CUDA_TRY(cudaMemsetAsync(L.zero_d, 0, (size_t)P * 12, stream));
-  const int sms = num_sms();
-  const int n_tiles = (P + T - 1) / T;
-  const int gridx = n_tiles < sms ? n_tiles : sms;
   for (int d = 0; d <= stage; ++d) {
     DecParams D;
     D.P = P; D.S = 1; D.z = L.z; D.rays_o = points; D.rays_d = L.zero_d;
     for (int k = 0; k < 3; ++k) { D.bmin[k] = bound_min[k]; D.bmax[k] = bound_max[k]; }
-    D.ga.data = grids[d].data; D.ga.nx = grids[d].nx; D.ga.ny = grids[d].ny; D.ga.nz = grids[d].nz;
-    D.ga.grad = nullptr;
-    D.gb.data = nullptr; D.gb.grad = nullptr; D.gb.nx = D.gb.ny = D.gb.nz = 1;
-    if (d == 1) { D.gb.data = grids[0].data; D.gb.nx = grids[0].nx; D.gb.ny = grids[0].ny; D.gb.nz = grids[0].nz; }
+    D.ga = {grids[d].data, nullptr, grids[d].nx, grids[d].ny, grids[d].nz};
+    if (d == 1) D.gb = {grids[0].data, nullptr, grids[0].nx, grids[0].ny, grids[0].nz};
     D.dec = decoders[d];
-    for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
     if (d == 0) D.out[0] = L.occ_mid;
     if (d == 1) D.out[0] = L.occ_fine;
     if (d == 2) { D.out[0] = L.rgb; D.out[1] = L.rgb + P; D.out[2] = L.rgb + 2 * (size_t)P; }
-    D.masks = nullptr; D.acts = nullptr; D.Pp = (int)align_up((size_t)P, 64); D.dp = nullptr; D.need_dp = 0;
-    D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
-    const size_t smem = sizeof(float) * ((size_t)woff(decoders[d].c_dim).total + (size_t)(E + CMAX) * T);
-    XRD_CUDA_TRY(cudaFuncSetAttribute(k_decoder_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k_decoder_fwd<<<gridx, T, smem, stream>>>(D);
-    XRD_LAUNCH_CHECK();
+    XRD_CUDA_TRY(launch_decoder(D, false, stream));
   }
   k_query_pack<<<(P + 255) / 256, 256, 0, stream>>>(P, L.occ_mid,
                                                     stage >= XRD_NICE_FINE ? L.occ_fine : nullptr,
@@ -1197,7 +1150,7 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   const Ws L(workspace, R, S, with_grads);
   if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
-  const int P = R * S, Pp = (int)align_up((size_t)P, 64);
+  const int P = R * S;
   double* z = out->z_vals ? out->z_vals : L.z;
   float* occ = L.occ_mid;
 
@@ -1212,17 +1165,11 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   DecParams D;
   D.P = P; D.S = S; D.z = z; D.rays_o = rays->rays_o; D.rays_d = rays->rays_d;
   for (int k = 0; k < 3; ++k) { D.bmin[k] = cfg->coarse_bound_min[k]; D.bmax[k] = cfg->coarse_bound_max[k]; }
-  D.ga.data = grid->data; D.ga.nx = grid->nx; D.ga.ny = grid->ny; D.ga.nz = grid->nz;
-  D.ga.grad = with_grads ? d_grid : nullptr;
-  D.gb.data = nullptr; D.gb.grad = nullptr; D.gb.nx = D.gb.ny = D.gb.nz = 1;
-  for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
+  D.ga = {grid->data, with_grads ? d_grid : nullptr, grid->nx, grid->ny, grid->nz};
   D.out[0] = occ;
   D.masks = L.masks;
-  D.acts = nullptr; D.Pp = Pp;
   D.dp = L.dp;
   D.need_dp = with_grads && (d_rays_o || d_rays_d);
-  D.zf = nullptr; D.ext_c = nullptr; D.ext_dc = nullptr; D.embed_scale = 1.0f;
-  D.dec = XrdNiceDecoder{};
   CoarseW W;
   for (int l = 0; l < 5; ++l) { W.pts_w[l] = dec->pts_w[l]; W.pts_b[l] = dec->pts_b[l]; }
   W.out_w = dec->out_w; W.out_b = dec->out_b;
@@ -1272,5 +1219,3 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   }
   return XRD_OK;
 }
-
-#endif  // XRD_NICE_KERNELS_ONLY

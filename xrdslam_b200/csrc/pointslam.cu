@@ -9,13 +9,12 @@
 //   slam/models/conv_onet_pointslam.py:311-461 render_batch_ray, :144-195 get_loss_dict
 //   slam/model_components/utils.py:247-295 raw2outputs_nerf_color2
 // The 5x32 Fourier MLP is the NICE decoder with sin(2 pi p B) and an externally supplied
-// feature: its kernels are shared (nice.cu, compiled in here as static functions).
+// feature (nice::launch_decoder).
 #include <float.h>
 #include <math.h>
 
-#define XRD_NICE_KERNELS_ONLY
-#include "nice.cu"
-#include "gemm_t5.cuh"
+#include "mlp.cuh"
+#include "nice.cuh"
 
 namespace xrd {
 namespace point {
@@ -942,27 +941,15 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   XRD_LAUNCH_CHECK();
 
   xrd::nice::DecParams D;
-  D.P = P; D.S = S; D.z = nullptr; D.zf = z; D.rays_o = rays->rays_o; D.rays_d = rays->rays_d;
-  for (int k = 0; k < 3; ++k) { D.bmin[k] = 0.0; D.bmax[k] = 1.0; }
-  D.ga.data = nullptr; D.ga.grad = nullptr; D.ga.nx = D.ga.ny = D.ga.nz = 1;
-  D.gb = D.ga;
+  D.P = P; D.S = S; D.zf = z; D.rays_o = rays->rays_o; D.rays_d = rays->rays_d;
   D.dec = *dec;
-  for (int k = 0; k < 4; ++k) { D.out[k] = nullptr; D.dout[k] = nullptr; }
   D.out[0] = L.occ;
   D.masks = L.masks;
-  D.acts = nullptr; D.Pp = P;
   D.dp = L.dp;
   D.need_dp = grads && (grads->d_rays_o || grads->d_rays_d);
   D.ext_c = Q.c; D.ext_dc = L.dc;
   D.embed_scale = 6.283185307179586f;  // 2 * math.pi, float32
-  const size_t smem = sizeof(float) * ((size_t)xrd::nice::woff(CD).total +
-                                       (size_t)(xrd::nice::E + xrd::nice::CMAX) * xrd::nice::T);
-  const int tiles = (P + xrd::nice::T - 1) / xrd::nice::T, sms = num_sms();
-  const int gridx = tiles < sms ? tiles : sms;
-  XRD_CUDA_TRY(cudaFuncSetAttribute(xrd::nice::k_decoder_fwd,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  xrd::nice::k_decoder_fwd<<<gridx, xrd::nice::T, smem, stream>>>(D);
-  XRD_LAUNCH_CHECK();
+  XRD_CUDA_TRY(xrd::nice::launch_decoder(D, false, stream));
   ColorP C{};
   if (stage == 1) {
     C.K = Q.K; C.Pp = L.Pp; C.min_nn = cfg->min_nn_num; C.col_feats = feats->col_feats;
@@ -987,10 +974,7 @@ extern "C" int xrd_pointslam_step(const XrdRays* rays, const XrdPointIndex* inde
   XRD_LAUNCH_CHECK();
   XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   D.dout[0] = Y.d_occ;
-  XRD_CUDA_TRY(cudaFuncSetAttribute(xrd::nice::k_decoder_bwd,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  xrd::nice::k_decoder_bwd<<<gridx, xrd::nice::T, smem, stream>>>(D);
-  XRD_LAUNCH_CHECK();
+  XRD_CUDA_TRY(xrd::nice::launch_decoder(D, true, stream));
   Q.dc = D.ext_dc; Q.d_feats = grads->d_geo_feats; Q.dp = D.dp; Q.need_dp = D.need_dp;
   k_interp_bwd<<<(P + 127) / 128, 128, 0, stream>>>(Q);
   XRD_LAUNCH_CHECK();

@@ -13,8 +13,7 @@
 #include <math.h>
 
 #include "common.cuh"
-#include "dw.cuh"
-#include "gemm_t5.cuh"
+#include "mlp.cuh"
 
 namespace xrd {
 namespace vox {
@@ -386,7 +385,7 @@ __device__ __forceinline__ void trilerp_emb(const float* __restrict__ emb, const
   }
 }
 
-// ---- GEMM decoder path: gather / head / scatter kernels around gemm.cuh -------------------
+// ---- GEMM decoder path: gather / head / scatter kernels around launch_gemm ----------------
 // x = trilinear embedding of the sample point -> activation rows ra_x
 __global__ void __launch_bounds__(T) k_vox_gather(const PointParams P) {
   const int p = blockIdx.x * T + threadIdx.x;
@@ -983,62 +982,5 @@ extern "C" int xrd_voxfusion_render(const XrdRays* rays, const XrdVoxMap* map,
                                                  grads->d_rays_o, grads->d_rays_d);
     XRD_LAUNCH_CHECK();
   }
-  return XRD_OK;
-}
-
-
-// Direct entry to the wide-MLP GEMM (gemm.cuh / gemm_t5.cuh) for the unit tests:
-//   C[m][n] = act( sum_k A(m,k) B[k][n] + bias[m] ), optional relu mask / addend, under the
-//   calling thread's xrd_debug_gemm_mode.  All pointers DEVICE.
-extern "C" int xrd_debug_gemm(int M, int N, int K, const float* A, int lda, int transA, const float* B,
-                              int ldb, float* C, int ldc, const float* bias, int act,
-                              const float* relu_mask, int ldmask, const float* addend, int ldadd,
-                              void* stream) {
-  if (!A || !B || !C) return XRD_E_NULL;
-  if (M <= 0 || N <= 0 || K <= 0) return XRD_E_SHAPE;
-  xrd::GemmArgs g{};
-  g.M = M; g.N = N; g.K = K; g.A = A; g.lda = lda; g.transA = transA; g.B = B; g.ldb = ldb;
-  g.C = C; g.ldc = ldc; g.bias = bias; g.act = act; g.relu_mask = relu_mask; g.ldmask = ldmask;
-  g.addend = addend; g.ldadd = ldadd;
-  XRD_CUDA_TRY(xrd::launch_gemm(g, (cudaStream_t)stream));
-  return XRD_OK;
-}
-
-// ... with the remaining epilogue options: act_out[m][n] receives the masked activation before
-// the addend, accumulate != 0 adds the result to C.
-extern "C" int xrd_debug_gemm_ex(int M, int N, int K, const float* A, int lda, int transA, const float* B,
-                                 int ldb, float* C, int ldc, const float* bias, int act,
-                                 const float* relu_mask, int ldmask, const float* addend, int ldadd,
-                                 float* act_out, int ldact, int accumulate, void* stream) {
-  if (!A || !B || !C) return XRD_E_NULL;
-  if (M <= 0 || N <= 0 || K <= 0) return XRD_E_SHAPE;
-  xrd::GemmArgs g{};
-  g.M = M; g.N = N; g.K = K; g.A = A; g.lda = lda; g.transA = transA; g.B = B; g.ldb = ldb;
-  g.C = C; g.ldc = ldc; g.bias = bias; g.act = act; g.relu_mask = relu_mask; g.ldmask = ldmask;
-  g.addend = addend; g.ldadd = ldadd; g.act_out = act_out; g.ldact = ldact; g.accumulate = accumulate;
-  XRD_CUDA_TRY(xrd::launch_gemm(g, (cudaStream_t)stream));
-  return XRD_OK;
-}
-
-// Direct entry to the weight-gradient kernels (dw.cuh) for the unit tests:
-//   out[j][i] += sum_p B[j][p] (where bit (j & 31) of mask[j / 32][p] is set) * A[i][p],
-//   bias[j] += sum_p B[j][p] (masked)
-// A [nA][Pp], B [nB][Pp] rows of P valid points; the rows of B are cut into 32-row jobs exactly
-// as the model kernels do, under the calling thread's xrd_debug_gemm_mode.  DEVICE pointers.
-extern "C" int xrd_debug_dw(int nA, int nB, int P, int Pp, const float* A, const float* B,
-                            const uint32_t* mask, float* out, float* bias, void* stream) {
-  if (!A || !B || !out) return XRD_E_NULL;
-  if (nA <= 0 || nB <= 0 || P <= 0 || Pp < P) return XRD_E_SHAPE;
-  xrd::DwParams D;
-  D.n_jobs = 0; D.P = P; D.Pp = Pp; D.chunk = 512;
-  for (int c = 0; c < nB; c += 32) {
-    if (D.n_jobs >= xrd::DW_MAX_JOBS) return XRD_E_SHAPE;
-    xrd::DwJob& J = D.jobs[D.n_jobs++];
-    J.A = A; J.nA = nA; J.B = B + (size_t)c * Pp; J.nB = nB - c < 32 ? nB - c : 32;
-    J.mask = mask ? mask + (size_t)(c / 32) * P : nullptr;
-    J.out = out + (size_t)c * nA; J.sj = nA; J.si = 1;
-    J.bias = bias ? bias + c : nullptr;
-  }
-  XRD_CUDA_TRY(xrd::launch_dw(D, (cudaStream_t)stream));
   return XRD_OK;
 }
