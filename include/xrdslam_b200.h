@@ -279,6 +279,11 @@ int xrd_coslam_smoothness_dev(const XrdHashGrid* grid, int sample_points,
                           const float* smooth_rand, float* loss, float* d_table,
                           float grad_scale, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* Test hook of both smoothness entry points: cap >= 0 limits the shared-memory box of table
+ * entries a CTA may interpolate from to min(cap, what the device has room for), so cap = 0
+ * sends every level through the 8-corner gather; cap < 0 restores the automatic size (the
+ * default).  Thread-local; returns the previous value. */
+int xrd_debug_smooth_box_cap(int cap);
 
 /* Point queries of the mesher path (slam/models/joint_encoding.py:408-481 query_fn /
  * color_func / query_sdf / query_color_sdf; slam/common/mesher.py:138-263 calls them on

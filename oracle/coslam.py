@@ -186,21 +186,25 @@ class CoslamOracle(torch.nn.Module):
             d['smooth_loss'] = self.smoothness(smooth_rand) * c.smooth_weight
         return d
 
-    def smooth_points(self, smooth_rand):
+    def smooth_points(self, smooth_rand, sample_points=None, voxel=None, margin=None):
         """pts (f64, normalised) of the smoothness lattice; smooth_rand[0] is
-        torch.rand(3) of :176, smooth_rand[1] the torch.rand((1,1,1,3)) of :179."""
+        torch.rand(3) of :176, smooth_rand[1] the torch.rand((1,1,1,3)) of :179.
+        sample_points / voxel / margin default to the config's."""
         c = self.cfg
+        sp = c.smooth_pts if sample_points is None else sample_points
+        vox = c.smooth_vox if voxel is None else voxel
+        margin = c.smooth_margin if margin is None else margin
         bb = self.bounding_box.to(self.embed_fn.params.device)
         smooth_rand = smooth_rand.to(bb.device)
-        n = c.smooth_pts - 1
-        grid_size = (c.smooth_pts - 1) * c.smooth_vox
-        offset_max = bb[:, 1] - bb[:, 0] - grid_size - 2 * c.smooth_margin
-        offset = smooth_rand[0].to(offset_max) * offset_max + c.smooth_margin
+        n = sp - 1
+        grid_size = (sp - 1) * vox
+        offset_max = bb[:, 1] - bb[:, 0] - grid_size - 2 * margin
+        offset = smooth_rand[0].to(offset_max) * offset_max + margin
         ar = torch.arange(0, n, dtype=torch.long, device=bb.device)
         x, y, z = torch.meshgrid(ar, ar, ar, indexing='ij')
         coords = torch.stack([x, y, z], -1).float().to(bb)
         pts = (coords + smooth_rand[1].reshape(1, 1, 1, 3).to(bb)
-               ) * c.smooth_vox + bb[:, 0] + offset
+               ) * vox + bb[:, 0] + offset
         return (pts - bb[:, 0]) / (bb[:, 1] - bb[:, 0])
 
     def smoothness(self, smooth_rand):

@@ -447,36 +447,59 @@ def failures(rep, gates):
 
 
 # ------------------------------------------------------------- smoothness ---
-def smoothness_replay(ora, smooth_rand, weight=1.0, device='cpu'):
+def _one_level(lay, l):
+    """The layout of level l alone, its entries counted from 0."""
+    out = {k: (v[l:l + 1] if isinstance(v, np.ndarray) else v) for k, v in lay.items()}
+    out['offset'] = np.zeros(1, dtype=np.uint32)
+    return out
+
+
+def smoothness_replay(ora, smooth_rand, weight=1.0, device='cpu', sample_points=None,
+                      voxel=None, margin=None, with_terms=False):
     """Float64 total-variation term of oracle/coslam.py ``smoothness`` times ``weight``, on the
-    fp32 lattice coordinates and their fp32 hash indices / weights.  Returns (loss, d_table,
-    A_table, layout) with A_table the |w_c| * |dfeat| bound (dfeat = 2 coef sum of neighbour
-    differences, bounded by 2 coef sum (|f| + |f_nb|))."""
+    fp32 lattice coordinates and their fp32 hash indices / weights.  sample_points / voxel /
+    margin default to ``ora.cfg``.  Returns (loss, d_table, A_table, layout) with A_table the
+    |w_c| * |dfeat| bound (dfeat = 2 coef sum of neighbour differences, bounded by
+    2 coef sum (|f| + |f_nb|)).  with_terms appends, per level, the largest number of
+    (point, corner) terms that land on one table entry.
+
+    The levels are independent (the TV term sums over feature channels), so they run one at a
+    time: at 75^3 points the peak stays at a few hundred MB."""
     c = ora.cfg
+    sp = c.smooth_pts if sample_points is None else int(sample_points)
     lay = ora.embed_fn.table
     dev = torch.device(device)
-    x32 = ora.smooth_points(smooth_rand).reshape(-1, 3).float().to(dev)
-    n = c.smooth_pts - 1
-    idx, w32 = hashgrid_indices(x32, lay)
-    P, L = idx.shape[:2]
-    table = ora.embed_fn.params.detach().to(device=dev, dtype=F64).requires_grad_(True)
-    wc = corner_weights(w32.double())
-    tab = table.view(-1, 2)
-    feat = 0
-    for k in range(8):
-        feat = feat + wc[..., k, None] * tab[idx[..., k]]
-    f = feat.reshape(n, n, n, L * 2)
-    coef = float(weight) / c.smooth_pts ** 3
-    tv = sum(((torch.diff(f, dim=d)) ** 2).sum() for d in range(3))
-    loss = tv * coef
-    loss.backward()
-    fa = f.detach().abs()
-    B = torch.zeros_like(fa)
-    for d in range(3):
-        s = fa.narrow(d, 0, n - 1) + fa.narrow(d, 1, n - 1)
-        B.narrow(d, 1, n - 1).add_(s)
-        B.narrow(d, 0, n - 1).add_(s)
-    B = (2.0 * coef * B).reshape(P, L, 1, 2) * wc.abs()[..., None]
-    A = torch.zeros(table.numel() // 2, 2, dtype=F64, device=dev)
-    A.index_add_(0, idx.reshape(-1), B.reshape(-1, 2))
-    return loss.detach(), table.grad, A.reshape(-1), lay
+    x32 = ora.smooth_points(smooth_rand, sp, voxel, margin).reshape(-1, 3).float().to(dev)
+    n = sp - 1
+    coef = float(weight) / sp ** 3
+    params = ora.embed_fn.params.detach().to(device=dev, dtype=F64)
+    grad, A = torch.zeros_like(params), torch.zeros_like(params)
+    loss = torch.zeros((), dtype=F64, device=dev)
+    terms = []
+    for l, (a, b) in enumerate(level_slices(lay)):
+        idx, w32 = hashgrid_indices(x32, _one_level(lay, l))     # [P,1,8] level-local, [P,1,3]
+        idx, wc = idx[:, 0], corner_weights(w32[:, 0].double())    # [P,8]
+        tab = params[a:b].clone().requires_grad_(True)
+        tv2 = tab.view(-1, 2)
+        feat = 0
+        for k in range(8):
+            feat = feat + wc[:, k, None] * tv2[idx[:, k]]
+        f = feat.reshape(n, n, n, 2)
+        tv = sum(((torch.diff(f, dim=d)) ** 2).sum() for d in range(3))
+        lv = tv * coef
+        lv.backward()
+        loss += lv.detach()
+        grad[a:b] = tab.grad
+        fa = f.detach().abs()
+        B = torch.zeros_like(fa)
+        for d in range(3):
+            s = fa.narrow(d, 0, n - 1) + fa.narrow(d, 1, n - 1)
+            B.narrow(d, 1, n - 1).add_(s)
+            B.narrow(d, 0, n - 1).add_(s)
+        B = (2.0 * coef * B).reshape(-1, 1, 2) * wc.abs()[..., None]
+        A[a:b].view(-1, 2).index_add_(0, idx.reshape(-1), B.reshape(-1, 2))
+        if with_terms:
+            terms.append(int(torch.bincount(idx.reshape(-1)).max()))
+        del idx, wc, feat, f, tv, lv, fa, B, tab, tv2
+    out = (loss, grad, A, lay)
+    return out + (terms,) if with_terms else out

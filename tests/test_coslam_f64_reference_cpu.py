@@ -173,3 +173,29 @@ def test_mutation_drop_last_ray_col1(step4097):
     assert bool((contrib != 0).any())
     mut = dict(cand, d_w_col1=cand['d_w_col1'] - contrib)
     assert 0 not in _flagged(ref, mut, sdf, modes=(0,))
+
+
+@pytest.mark.parametrize('sp, voxel', [(3, 0.1), (6, 0.1), (40, 0.15)])
+def test_smoothness_replay_lattice_arguments(sp, voxel):
+    """smoothness_replay on a lattice other than the config's agrees with the fp32 oracle's
+    autograd of the same lattice to fp32 rounding within the entry bound A, and with no
+    arguments it replays the config's lattice."""
+    ora = _oracle(0.1)
+    rnd = torch.tensor([0.3, 0.7, 0.1, 0.9, 0.2, 0.5]).reshape(2, 3)
+    loss64, g64, A, _, terms = F.smoothness_replay(ora, rnd, sample_points=sp, voxel=voxel,
+                                                   margin=0.05, with_terms=True)
+    assert len(terms) == 16 and min(terms) >= 1
+    p = ora.smooth_points(rnd, sp, voxel, 0.05)
+    assert p.shape == (sp - 1,) * 3 + (3,)
+    f = ora.embed_fn(p.reshape(-1, 3)).reshape(*p.shape[:-1], -1)
+    tv = sum((torch.diff(f, dim=d) ** 2).sum() for d in range(3)) / sp ** 3
+    tv.backward()
+    err = (ora.embed_fn.params.grad.double() - g64).abs()
+    assert not bool(((A == 0) & (err > 0)).any())
+    assert float((err[A > 0] / A[A > 0]).max()) < 1e-5
+    assert abs(float(tv.detach()) - float(loss64)) <= 1e-6 * float(loss64)
+    c = ora.cfg
+    dflt = F.smoothness_replay(ora, rnd)
+    expl = F.smoothness_replay(ora, rnd, sample_points=c.smooth_pts, voxel=c.smooth_vox,
+                               margin=c.smooth_margin)
+    assert all(torch.equal(a, b) for a, b in zip(dflt[:3], expl[:3]))

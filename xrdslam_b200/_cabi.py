@@ -310,6 +310,7 @@ SYMBOLS = {
         C.POINTER(XrdHashGrid), C.c_int, C.c_double, C.c_double, C.c_float, vp,
         vp, vp, C.c_float, vp, C.c_size_t, vp
     ]),
+    'xrd_debug_smooth_box_cap': (C.c_int, [C.c_int]),
     'xrd_hashgrid_encode':
     (C.c_int, [C.POINTER(XrdHashGrid), vp, C.c_int, vp, vp, vp]),
     'xrd_octree_create': (vp, [C.c_int]),

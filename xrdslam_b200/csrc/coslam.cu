@@ -2094,6 +2094,9 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   return XRD_OK;
 }
 
+// xrd_debug_smooth_box_cap: an upper limit on the box capacity, per calling thread (< 0: none)
+thread_local int g_smooth_box_cap = -1;
+
 // the loss accumulator and the CTA counter of k_smooth_bwd
 struct SmoothWs : Carver {
   explicit SmoothWs(void* base) : Carver(base) {}
@@ -2150,6 +2153,7 @@ static int smoothness_impl(const XrdHashGrid* grid, int sample_points, double vo
                          (2 * (long long)sizeof(float2));
   if (room < 0) return XRD_E_SHAPE;
   p.box_cap = (int)(room < kSmoothBox ? room : kSmoothBox);
+  if (g_smooth_box_cap >= 0 && g_smooth_box_cap < p.box_cap) p.box_cap = g_smooth_box_cap;
   const size_t smem = win + 2 * sizeof(float2) * (size_t)p.box_cap;
   XRD_CUDA_TRY(cudaFuncSetAttribute(k_smooth_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)smem));
@@ -2175,6 +2179,12 @@ extern "C" int xrd_coslam_smoothness_dev(const XrdHashGrid* grid, int sample_poi
                                          void* workspace, size_t workspace_bytes, void* stream_) {
   return smoothness_impl(grid, sample_points, voxel_size, margin, weight, smooth_rand, true, loss,
                          d_table, grad_scale, workspace, workspace_bytes, stream_);
+}
+
+extern "C" int xrd_debug_smooth_box_cap(int cap) {
+  const int prev = g_smooth_box_cap;
+  g_smooth_box_cap = cap < 0 ? -1 : cap;
+  return prev;
 }
 
 extern "C" int xrd_coslam_query(const XrdHashGrid* grid, const XrdCoslamMlp* mlp, const float* pts,
