@@ -176,12 +176,23 @@ typedef struct {
 int xrd_hashgrid_layout(XrdHashGrid* g, int n_levels, int log2_hashmap_size,
                         int base_resolution, float per_level_scale);
 
-/* ColorSDFNet_v2 weights, torch nn.Linear layout [out,in], no bias. DEVICE. */
+/* ColorSDFNet_v2 weights, torch nn.Linear layout [out,in], no bias. DEVICE.
+ * grid_color != NULL selects ColorSDFNet (JointEncodingConfig.oneGrid = False,
+ * slam/models/joint_encoding.py:199-234, decoder_coslam.py:113-136): a second hash
+ * grid, embed_fn_color, feeds the colour branch, whose input becomes
+ * oneblob48 ++ colour-hash32 ++ geo15, so w_col0 is [32,95].  Its layout fields and
+ * table are read like `grid`'s; the points are normalised with `grid`'s bound.
+ * NULL keeps ColorSDFNet_v2 (one grid).  xrd_coslam_step runs a colour-grid pass on the
+ * tile kernel only (rays_per_tile = -2 returns XRD_E_SHAPE).  Its shared memory bounds the
+ * points per tile: forward-only passes take every n_samples the one-grid path takes (<= 256,
+ * render without depth included); a gradient pass takes n_samples <= 224 (XRD_E_SHAPE
+ * otherwise; with depth the samples are n_sample_d + n_range_d = 43). */
 typedef struct {
   const float* w_sdf0; /* [32,80]  in = hash32 ++ oneblob48                  */
   const float* w_sdf1; /* [16,32]  out = sdf ++ geo15                        */
-  const float* w_col0; /* [32,63]  in = oneblob48 ++ geo15                   */
+  const float* w_col0; /* [32,63]  in = oneblob48 ++ geo15; [32,95] with grid_color */
   const float* w_col1; /* [3,32]                                             */
+  const XrdHashGrid* grid_color; /* HOST pointer, or NULL                    */
 } XrdCoslamMlp;
 
 typedef struct {
@@ -232,11 +243,11 @@ typedef struct {
 
 /* Gradients of (rgb+depth+sdf+fs) loss scaled by loss_scale[4] per term.
  * d_table and d_w_* are ACCUMULATED into (caller zeroes them: mapping-pose Adam
- * uses accum_step, Q11); d_rays_* are overwritten.  The five map gradients are
- * all-or-nothing: all NULL selects the pose-only pass used by tracking (no
- * scatter, no weight-gradient tiles).  d_table must be 16-byte aligned: two
- * x-adjacent trilinear corners that share a 16-byte chunk are added with one
- * vector reduction (XRD_E_SHAPE otherwise). */
+ * uses accum_step, Q11); d_rays_* are overwritten.  The five map gradients (six
+ * with a colour grid: d_table_color too) are all-or-nothing: all NULL selects the
+ * pose-only pass used by tracking (no scatter, no weight-gradient tiles).  d_table and
+ * d_table_color must be 16-byte aligned: two x-adjacent trilinear corners that share a
+ * 16-byte chunk are added with one vector reduction (XRD_E_SHAPE otherwise). */
 typedef struct {
   float* d_table;  /* [n_entries*2] */
   float* d_w_sdf0; /* [32,80] */
@@ -246,6 +257,9 @@ typedef struct {
   float* d_rays_o; /* [R,3] or NULL */
   float* d_rays_d; /* [R,3] or NULL */
   float loss_scale[4]; /* upstream d total / d term (normally 1,1,1,1) */
+  float* d_table_color; /* [grid_color->n_entries*2]; NULL without a colour grid.
+                         * Only the rgb term reaches it (embed_fn_color feeds the colour
+                         * branch only); its spatial derivative adds to d_rays_*. */
 } XrdCoslamGrads;
 
 size_t xrd_coslam_workspace_bytes(int n_rays, int n_samples);
@@ -286,7 +300,8 @@ int xrd_coslam_smoothness_dev(const XrdHashGrid* grid, int sample_points,
 int xrd_debug_smooth_box_cap(int cap);
 
 /* Point queries of the mesher path (slam/models/joint_encoding.py:408-481 query_fn /
- * color_func / query_sdf / query_color_sdf; slam/common/mesher.py:138-263 calls them on
+ * color_func / query_sdf / query_color_sdf, with mlp->grid_color the colour grid of
+ * query_color_sdf :463-481 too; slam/common/mesher.py:138-263 calls them on
  * marching-cubes lattice points): pts DEVICE [P,3], world coordinates (normalised = 0: the
  * kernel applies (p - bbox_min) / (bbox_max - bbox_min) in float64 like the reference) or
  * already normalised (1).  Any of raw [P,4] (rgb logits ++ sdf), geo [P,15], feat [P,32]

@@ -56,7 +56,8 @@ class XrdHashGrid(C.Structure):
 
 
 class XrdCoslamMlp(C.Structure):
-    _fields_ = [('w_sdf0', vp), ('w_sdf1', vp), ('w_col0', vp), ('w_col1', vp)]
+    _fields_ = [('w_sdf0', vp), ('w_sdf1', vp), ('w_col0', vp), ('w_col1', vp),
+                ('grid_color', C.POINTER(XrdHashGrid))]
 
 
 class XrdCoslamCfg(C.Structure):
@@ -80,7 +81,7 @@ class XrdCoslamOut(C.Structure):
 class XrdCoslamGrads(C.Structure):
     _fields_ = [('d_table', vp), ('d_w_sdf0', vp), ('d_w_sdf1', vp),
                 ('d_w_col0', vp), ('d_w_col1', vp), ('d_rays_o', vp),
-                ('d_rays_d', vp), ('loss_scale', C.c_float * 4)]
+                ('d_rays_d', vp), ('loss_scale', C.c_float * 4), ('d_table_color', vp)]
 
 
 class XrdNiceDecoder(C.Structure):

@@ -281,9 +281,8 @@ class CoSLAM(Algorithm):
         cache = self.__dict__.setdefault('_graph_sessions', {})
         for k in [k for k in cache if k != key]:
             cache.pop(k).release()
-        if key in cache and (cache[key].stale() or
-                             cache[key].opt_groups[0][0] is not self.model_optimizers.optimizers['embed_fn']):
-            cache.pop(key).release()  # optimiser state / parameters were replaced: re-capture
+        if key in cache and cache[key].stale():
+            cache.pop(key).release()  # optimisers / their state / parameters were replaced: re-capture
         if key not in cache:
             cache[key] = MappingGraphSession(self, n_bank, n_cur, len(optimize_frames), first, ba)
         return cache[key]

@@ -89,14 +89,17 @@ class MappingGraphSession:
         self.ws, self.ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
         self.ws_s, self.ws_s_bytes = _cabi.workspace(dev, 'coslam_smoothness',
                                                      cfg.trainging_smooth_pts)
-        # per-iteration scalars: [seed u64 | smooth_rand f32 x6 | (lr, bc1, bc2) per group]
+        # per-iteration scalars: [seed u64 | smooth_rand f32 x6 | (lr, bc1, bc2) per group (<= 3)]
         self._scalars = _ScalarRing(128, dev)
         self.dyn = self._scalars.dyn
         # ---- model parameters, their persistent gradient buffers and Adam state
         self.table = model.embed_fn.params
         self.weights = list(model._weights())
+        # oneGrid=False: the colour grid's table, one more Adam group in the same bucket
+        self.table_c = None if cfg.oneGrid else model.embed_fn_color.params
+        self.group_names = ('embed_fn', 'decoder') + (() if cfg.oneGrid else ('embed_fn_color',))
         self.opt_groups = []  # (FusedAdam, [params])
-        for name in ('embed_fn', 'decoder'):
+        for name in self.group_names:
             opt = algo.model_optimizers.optimizers[name]
             if not isinstance(opt, FusedAdam) or len(opt.param_groups) != 1:
                 raise RuntimeError('graph mapping needs FusedAdam model optimizers')
@@ -173,7 +176,8 @@ class MappingGraphSession:
         gs = XrdCoslamGrads(ptr(G[self.table]), *(ptr(G[t]) for t in self.weights),
                             ptr(self.d_rays_o) if self.ba else None,
                             ptr(self.d_rays_d) if self.ba else None,
-                            (C.c_float * 4)(1.0, 1.0, 1.0, 1.0))
+                            (C.c_float * 4)(1.0, 1.0, 1.0, 1.0),
+                            ptr(G[self.table_c]) if self.table_c is not None else None)
         sharded = dict(phase=2, n_rays_global=self.R * self.world, counts_global=self.counts)
         _fused_step(self, stream, gs, **(sharded if self.world > 1 else {}))
         if smooth:
@@ -311,7 +315,11 @@ class MappingGraphSession:
     # ------------------------------------------------------------------ running ---
     def stale(self):
         """True when a captured pointer no longer belongs to the live model / optimiser state
-        (optimiser state replaced, parameter re-allocated): the session must be rebuilt."""
+        (optimiser replaced, optimiser state replaced, parameter re-allocated): the session must
+        be rebuilt."""
+        live = self.algo.model_optimizers.optimizers
+        if any(opt is not live.get(name) for name, (opt, _) in zip(self.group_names, self.opt_groups)):
+            return True
         for opt, params in self.opt_groups:
             for p in params:
                 st = opt.state.get(p)

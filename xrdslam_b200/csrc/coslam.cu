@@ -29,6 +29,10 @@
 //              independent groups of warps with named barriers, one m-tile per warp, a
 //              132-float record with OneBlob in compact form and a balanced
 //              point-parallel hash backward (see its comment).
+//   k_fused_c  the tile kernel for a separate colour hash grid (Co-SLAM oneGrid=False,
+//              decoder_coslam.py:113-136 ColorSDFNet): a second 16-level gather into the record,
+//              the 95-input colour decoder, and the colour grid's hash backward (scatter into
+//              d_table_c, d loss / d xn).
 //   k_finalize loss accumulators -> the 4 weighted loss terms.
 #include <math.h>
 
@@ -50,12 +54,27 @@ constexpr int R_FEAT = 0, R_BLOB = 32, R_GEO = 80, R_SDF = 95, R_H1 = 96, R_C1 =
 // slower (DESIGN.md section 4.1).
 constexpr int G_FEAT = 0, G_BLOB = 32, G_GEO = 48, G_SDF = 63, G_H1 = 64, G_C1 = 96, G_RAW = 128,
               GREC = 132;
-// per-layout offsets for the code both kernels share
-template <bool COMPACT>
+// Colour grid (k_fused_c, k_query_c), stride 196: the colour grid's features sit between OneBlob
+// and geo, so that the 95 colour-decoder inputs [blob48 | cfeat32 | geo15] and the zero-weight
+// sdf column are one contiguous block of 12 k-steps:
+//   [feat32 | blob48 | cfeat32 | geo15 | sdf | h1 32 | c1 32 | raw4]
+constexpr int C_CFEAT = 80, C_GEO = 112, C_SDF = 127, C_H1 = 128, C_C1 = 160, C_RAW = 192,
+              CREC = 196;
+// Colour grid, forward only (CGF), stride 132: h1 overwrites the hash features once the first
+// GEMM has read them, and c1 overwrites h1 once the second has; nothing needs them afterwards.
+// [feat32 -> h1 -> c1 | blob48 | cfeat32 | geo15 | sdf | raw4].  This is what lets a render
+// pass without depth (256 samples: one ray of 256 points per tile) fit in shared memory.
+constexpr int F_H = 0, F_RAW = 128, FREC = 132;
+// per-layout offsets for the code the kernels share (CG: colour-grid record, CGF: its
+// forward-only form)
+template <bool COMPACT, bool CG = false, bool CGF = false>
 struct Rec {
-  static constexpr int N = COMPACT ? GREC : REC, GEO = COMPACT ? G_GEO : R_GEO,
-                       H1 = COMPACT ? G_H1 : R_H1, C1 = COMPACT ? G_C1 : R_C1,
-                       RAW = COMPACT ? G_RAW : R_RAW;
+  static constexpr int N = COMPACT ? GREC : CGF ? FREC : CG ? CREC : REC,
+                       GEO = COMPACT ? G_GEO : CG ? C_GEO : R_GEO,
+                       SDF = COMPACT ? G_SDF : CG ? C_SDF : R_SDF,
+                       H1 = COMPACT ? G_H1 : CGF ? F_H : CG ? C_H1 : R_H1,
+                       C1 = COMPACT ? G_C1 : CGF ? F_H : CG ? C_C1 : R_C1,
+                       RAW = COMPACT ? G_RAW : CGF ? F_RAW : CG ? C_RAW : R_RAW;
 };
 struct GridDev {
   float scale[kL];
@@ -87,6 +106,12 @@ struct Params {
   double* loss_acc;   // 4 sums
   int NR;             // rays per tile
   int n_tiles;
+};
+// k_fused_c: the colour grid on top (normalised coordinates come from g's bound)
+struct ParamsC : Params {
+  GridDev gc;
+  const float* table_c;
+  float* d_table_c;
 };
 
 // ------------------------------------------------------------------ sample ---
@@ -644,6 +669,19 @@ constexpr int SW_TOTAL = SWC1 + 32 * LDC1; // 6784 floats
 //   [0,2) d w_col1   [2,18) d w_col0   [18,22) d w_sdf1   [22,42) d w_sdf0
 constexpr int DW_TILES = 42;
 
+// Decoder shapes that differ with a colour grid: w_col0 has NC = 95 inputs instead of 63 (KC
+// k-steps of the colour GEMM, its transpose [96][40] with row 95 = 0 in shared memory), so
+// w_col1 and the end of the weight area move, and d w_col0 takes 24 weight-gradient tiles:
+//   [0,2) d w_col1   [2,26) d w_col0   [26,30) d w_sdf1   [30,50) d w_sdf0
+template <bool CG>
+struct Wts {
+  static constexpr int NC = CG ? 95 : 63, KC = CG ? 12 : 8, SWC1 = SWC0 + 8 * KC * LDC0,
+                       TOTAL = SWC1 + 32 * LDC1, COL0_TILES = CG ? 24 : 16,
+                       SDF1_LO = 2 + COL0_TILES, SDF0_LO = SDF1_LO + 4, DW = SDF0_LO + 20;
+};
+static_assert(Wts<false>::SWC1 == SWC1 && Wts<false>::TOTAL == SW_TOTAL &&
+              Wts<false>::DW == DW_TILES, "one-grid decoder layout");
+
 // A fragment values of the dense OneBlob bins (g, g + 8) of dimension bd for points p0 (k-slot t)
 // and p1 (k-slot t + 4), expanded from the compact form: both bins live in slot g & 3, with
 // quarters g >> 2 and (g >> 2) + 2.
@@ -689,15 +727,16 @@ __device__ __forceinline__ void dw_tile(const float* __restrict__ recs, int npts
 // The decoders for MT m-tiles of 16 records at wrec: h1, [geo, sdf], c1 and the rgb logits
 // (RAW[0..2]; RAW[3] = sdf is the caller's).  Caller: one warp.
 // COMPACT: the OneBlob A fragments are expanded from compact records.
-template <bool PREC3, int MT, bool COMPACT>
+template <bool PREC3, int MT, bool COMPACT, bool CG = false, bool CGF = false>
 __device__ __forceinline__ void decoder_forward(float* __restrict__ wrec, const float* __restrict__ sw) {
-  using L = Rec<COMPACT>;
+  using L = Rec<COMPACT, CG, CGF>;
   constexpr int N = L::N;
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   {  // h1 = relu([feat, blob] W0^T)
     float c[MT][4][4];
     zero_c(c);
     warp_gemm<10, 4, false, PREC3, N, COMPACT ? 4 : -1>(wrec, R_FEAT, sw + SW0, LD0, 0, 0, c);
+    if (CGF) __syncwarp();  // h1 replaces feat: every lane has read its A fragments
     store_c<RELU, N>(wrec, L::H1, c);
   }
   __syncwarp();
@@ -708,17 +747,17 @@ __device__ __forceinline__ void decoder_forward(float* __restrict__ wrec, const 
     store_c<PLAIN, N>(wrec, L::GEO, c);
   }
   __syncwarp();
-  {  // c1 = relu([blob, geo, (sdf: zero weight row)] Wc0^T)
+  {  // c1 = relu([blob, (cfeat,) geo, (sdf: zero weight row)] Wc0^T)
     float c[MT][4][4];
     zero_c(c);
-    warp_gemm<8, 4, false, PREC3, N, COMPACT ? 0 : -1>(wrec, COMPACT ? 0 : R_BLOB, sw + SWC0, LDC0, 0, 0, c);
+    warp_gemm<Wts<CG>::KC, 4, false, PREC3, N, COMPACT ? 0 : -1>(wrec, COMPACT ? 0 : R_BLOB, sw + SWC0, LDC0, 0, 0, c);
     store_c<RELU, N>(wrec, L::C1, c);
   }
   __syncwarp();
   {  // rgb logits = c1 Wc1^T (cols 0..2 of an 8-wide tile)
     float c[MT][1][4];
     zero_c(c);
-    warp_gemm<4, 1, false, PREC3, N>(wrec, L::C1, sw + SWC1, LDC1, 0, 0, c);
+    warp_gemm<4, 1, false, PREC3, N>(wrec, L::C1, sw + Wts<CG>::SWC1, LDC1, 0, 0, c);
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
       float* q0 = wrec + (mt * 16 + g) * N + L::RAW;
@@ -736,8 +775,10 @@ __device__ __forceinline__ void decoder_forward(float* __restrict__ wrec, const 
 
 // Zeroes the weight area, then stages the transposed decoder weights (zero padding included).
 // Whole CTA; the caller synchronises before the first read.
+template <bool CG = false>
 __device__ __forceinline__ void stage_weights(float* __restrict__ sw, const Params& P) {
-  for (int q = threadIdx.x; q < SW_TOTAL; q += blockDim.x) sw[q] = 0.f;
+  using W = Wts<CG>;
+  for (int q = threadIdx.x; q < W::TOTAL; q += blockDim.x) sw[q] = 0.f;
   __syncthreads();
   for (int q = threadIdx.x; q < 80 * 32; q += blockDim.x) {
     int i = q / 32, j = q % 32;
@@ -748,13 +789,13 @@ __device__ __forceinline__ void stage_weights(float* __restrict__ sw, const Para
     int jt = (jp + 1) & 15;
     sw[SW1 + i * LD1 + jp] = P.w_sdf1[jt * 32 + i];
   }
-  for (int q = threadIdx.x; q < 63 * 32; q += blockDim.x) {
+  for (int q = threadIdx.x; q < W::NC * 32; q += blockDim.x) {
     int i = q / 32, j = q % 32;
-    sw[SWC0 + i * LDC0 + j] = P.w_col0[j * 63 + i];
+    sw[SWC0 + i * LDC0 + j] = P.w_col0[j * W::NC + i];
   }
   for (int q = threadIdx.x; q < 32 * 3; q += blockDim.x) {
     int i = q / 3, k = q % 3;
-    sw[SWC1 + i * LDC1 + k] = P.w_col1[k * 32 + i];
+    sw[W::SWC1 + i * LDC1 + k] = P.w_col1[k * 32 + i];
   }
 }
 
@@ -775,17 +816,17 @@ __device__ __forceinline__ LossNorm loss_norm(const int* __restrict__ counts) {
 // Tile id of a weight-gradient layer whose tiles are [lo, hi) of the 42.  m-tile mt of the layer
 // input covers its columns 16 mt .. 16 mt + 15 at record offset aoff; m-tiles
 // [blob_mt, blob_mt + 3) are the OneBlob dimensions, read from the compact form.
-template <bool PREC3, bool COMPACT>
+template <bool PREC3, bool COMPACT, bool CG = false>
 __device__ __forceinline__ void dw_layer_tile(const float* __restrict__ recs, int npts, int id,
                                               int lo, int aoff, int boff, int n_tiles_n,
                                               int blob_mt, float (&acc)[4]) {
   const int loc = id - lo, mt = loc / n_tiles_n, nt = loc % n_tiles_n;
   const int bd = (blob_mt >= 0 && mt >= blob_mt && mt < blob_mt + 3) ? mt - blob_mt : -1;
-  dw_tile<PREC3, Rec<COMPACT>::N, COMPACT>(recs, npts, aoff + 16 * mt, boff + 8 * nt, acc, bd);
+  dw_tile<PREC3, Rec<COMPACT, CG>::N, COMPACT>(recs, npts, aoff + 16 * mt, boff + 8 * nt, acc, bd);
 }
 
 // This warp's share of one weight-gradient layer: slot j holds tile w + j * nw.
-template <bool PREC3, bool COMPACT, int SLOTS>
+template <bool PREC3, bool COMPACT, bool CG = false, int SLOTS>
 __device__ __forceinline__ void dw_layer(const float* __restrict__ recs, int npts, int w, int nw,
                                          float (&acc)[SLOTS][4], int lo, int hi, int aoff,
                                          int boff, int n_tiles_n, int blob_mt) {
@@ -793,13 +834,15 @@ __device__ __forceinline__ void dw_layer(const float* __restrict__ recs, int npt
   for (int j = 0; j < SLOTS; ++j) {
     const int id = w + j * nw;
     if (id >= lo && id < hi)
-      dw_layer_tile<PREC3, COMPACT>(recs, npts, id, lo, aoff, boff, n_tiles_n, blob_mt, acc[j]);
+      dw_layer_tile<PREC3, COMPACT, CG>(recs, npts, id, lo, aoff, boff, n_tiles_n, blob_mt, acc[j]);
   }
 }
 
 // Adds weight-gradient tile id (this lane's C fragment v; rows = in-feature, cols = out-unit) to
 // the weight gradients in global memory.
+template <bool CG = false>
 __device__ __forceinline__ void dw_store(const Params& P, int id, const float (&v)[4]) {
+  using W = Wts<CG>;
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -807,14 +850,14 @@ __device__ __forceinline__ void dw_store(const Params& P, int id, const float (&
     if (id < 2) {  // d w_col1 [3][32]
       const int in = 16 * id + rloc, out = cloc;
       if (out < 3) red_add(P.d_w_col1 + out * 32 + in, v[i]);
-    } else if (id < 18) {  // d w_col0 [32][63]
+    } else if (id < W::SDF1_LO) {  // d w_col0 [32][NC]
       const int loc = id - 2, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
-      if (in < 63) red_add(P.d_w_col0 + out * 63 + in, v[i]);
-    } else if (id < 22) {  // d w_sdf1 [16][32], stored column jp -> torch row (jp+1)&15
-      const int loc = id - 18, in = 16 * (loc / 2) + rloc, jp = 8 * (loc % 2) + cloc;
+      if (in < W::NC) red_add(P.d_w_col0 + out * W::NC + in, v[i]);
+    } else if (id < W::SDF0_LO) {  // d w_sdf1 [16][32], stored column jp -> torch row (jp+1)&15
+      const int loc = id - W::SDF1_LO, in = 16 * (loc / 2) + rloc, jp = 8 * (loc % 2) + cloc;
       red_add(P.d_w_sdf1 + ((jp + 1) & 15) * 32 + in, v[i]);
     } else {  // d w_sdf0 [32][80]
-      const int loc = id - 22, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
+      const int loc = id - W::SDF0_LO, in = 16 * (loc / 4) + rloc, out = 8 * (loc % 4) + cloc;
       red_add(P.d_w_sdf0 + out * 80 + in, v[i]);
     }
   }
@@ -822,12 +865,12 @@ __device__ __forceinline__ void dw_store(const Params& P, int id, const float (&
 
 // d_rays_o / d_rays_d of ray rr (one warp): sums over its S records (rq) of d loss / d pts and
 // z * d loss / d pts, parked in C1 slots 0..5
-template <bool COMPACT>
+template <bool COMPACT, bool CG = false>
 __device__ __forceinline__ void ray_grads(const Params& P, const float* __restrict__ rq, int rr,
                                           int lane) {
   float a[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int kk = lane; kk < P.S; kk += 32) {
-    const float* rp = rq + (size_t)kk * Rec<COMPACT>::N + Rec<COMPACT>::C1;
+    const float* rp = rq + (size_t)kk * Rec<COMPACT, CG>::N + Rec<COMPACT, CG>::C1;
 #pragma unroll
     for (int d = 0; d < 6; ++d) a[d] += rp[d];
   }
@@ -842,20 +885,20 @@ __device__ __forceinline__ void ray_grads(const Params& P, const float* __restri
   }
 }
 
-// dgeo = dc1pre Wc0[:, 48:64] -> dH = [dgeo(15), dsdf] in the GEO slots (SDF is the caller's),
-// then dh1pre = (h1 > 0) * (dH W1) in place of h1; the caller's barrier and dW layer run between
-// the two.  One warp, MT m-tiles.
-template <bool PREC3, int MT, bool COMPACT>
+// dgeo = dc1pre Wc0[:, 48:64] (colour grid: Wc0[:, 80:96]) -> dH = [dgeo(15), dsdf] in the GEO
+// slots (SDF is the caller's), then dh1pre = (h1 > 0) * (dH W1) in place of h1; the caller's
+// barrier and dW layer run between the two.  One warp, MT m-tiles.
+template <bool PREC3, int MT, bool COMPACT, bool CG = false>
 __device__ __forceinline__ void backward_geo(float* __restrict__ wrec, const float* __restrict__ sw) {
-  using L = Rec<COMPACT>;
+  using L = Rec<COMPACT, CG>;
   float c[MT][2][4];
   zero_c(c);
-  warp_gemm<4, 2, true, PREC3, L::N>(wrec, L::C1, sw + SWC0, LDC0, 0, 48, c);
+  warp_gemm<4, 2, true, PREC3, L::N>(wrec, L::C1, sw + SWC0, LDC0, 0, CG ? 80 : 48, c);
   store_c<PLAIN, L::N>(wrec, L::GEO, c);
 }
-template <bool PREC3, int MT, bool COMPACT>
+template <bool PREC3, int MT, bool COMPACT, bool CG = false>
 __device__ __forceinline__ void backward_h1(float* __restrict__ wrec, const float* __restrict__ sw) {
-  using L = Rec<COMPACT>;
+  using L = Rec<COMPACT, CG>;
   float c[MT][4][4];
   zero_c(c);
   warp_gemm<2, 4, true, PREC3, L::N>(wrec, L::GEO, sw + SW1, LD1, 0, 0, c);
@@ -1021,11 +1064,16 @@ __device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& l
 }
 
 // ----------------------------------------------------------------- fused ---
-template <bool BWD, bool PREC3, bool BPREC3, int SLOTS>
-__global__ void __launch_bounds__(256) k_fused(const Params P) {
+// The tile kernel's body; CG: with the colour grid (k_fused_c).
+template <bool CG, bool BWD, bool PREC3, bool BPREC3, int SLOTS, typename PT>
+__device__ __forceinline__ void fused_tile(const PT& P) {
+  constexpr bool CGF = CG && !BWD;  // forward-only colour-grid pass: the compact record
+  using L = Rec<false, CG, CGF>;
+  using W = Wts<CG>;
+  constexpr int REC = L::N;
   extern __shared__ __align__(16) float smem[];
-  float* sw = smem;                            // SW_TOTAL
-  float* recs = sw + SW_TOTAL;                 // (blockDim.x + 8) * REC
+  float* sw = smem;                            // W::TOTAL
+  float* recs = sw + W::TOTAL;                 // (blockDim.x + 8) * REC
   float* zbuf = recs + (blockDim.x + 8) * REC; // NR*S z values
   float* sgb = zbuf + P.NR * P.S;              // NR*S sigma(sdf/trunc)
   float* ub = sgb + P.NR * P.S;                // NR*S unnormalised weights
@@ -1035,9 +1083,10 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
   const int nwarps = blockDim.x >> 5;
   const int S = P.S;
 
-  __shared__ Lv s_lv[kL];
+  __shared__ Lv s_lv[CG ? 2 * kL : kL];  // the colour grid's levels at kL
   load_levels(s_lv, P.g);
-  stage_weights(sw, P);
+  if constexpr (CG) load_levels(s_lv + kL, P.gc);
+  stage_weights<CG>(sw, P);
   // the 8 pad records after the tile stay zero for the whole kernel (k-step overrun of dw_tile)
   for (int q = tid; q < 8 * REC; q += blockDim.x) recs[blockDim.x * REC + q] = 0.f;
   const LossNorm ln = BWD ? loss_norm(P.counts) : LossNorm{};
@@ -1073,6 +1122,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
 #pragma unroll
       for (int d = 0; d < 3; ++d) xnb[tid * 3 + d] = xn[d];
       encode<1>(P.table, P.g.n_levels, s_lv, xn, rec, 0);
+      if constexpr (CG) encode<1>(P.table_c, P.gc.n_levels, s_lv + kL, xn, rec + C_CFEAT, 0);
       blob_forward(xn, rec);
     } else {
       // inactive rows must read as zero in every GEMM (k-dimension of the dW tiles)
@@ -1081,18 +1131,18 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         *reinterpret_cast<float4*>(rec + q) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     __syncwarp();
-    if (warp_active) decoder_forward<PREC3, 2, false>(wrec, sw);
+    if (warp_active) decoder_forward<PREC3, 2, false, CG, CGF>(wrec, sw);
     if (active) {
-      rec[R_RAW + 3] = rec[R_SDF];
+      rec[L::RAW + 3] = rec[L::SDF];
       if (P.raw) {
-        float4 rw = *reinterpret_cast<const float4*>(rec + R_RAW);
+        float4 rw = *reinterpret_cast<const float4*>(rec + L::RAW);
         *reinterpret_cast<float4*>(P.raw + ((size_t)r * S + k) * 4) = rw;
       }
     }
     __syncthreads();
     // ---------------- phase 2: per-ray composite, loss, d loss / d raw ----
     for (int q = warp; q < nr; q += nwarps)
-      composite_ray<REC, BWD, 0>(P, ln, recs + (size_t)(q * S) * REC + R_RAW, zbuf + q * S,
+      composite_ray<REC, BWD, 0>(P, ln, recs + (size_t)(q * S) * REC + L::RAW, zbuf + q * S,
                                  sgb + q * S, ub + q * S, r0 + q, lane,
                                  [&](int i, float v) { l_sum[i] += (double)v; });
     __syncthreads();
@@ -1101,37 +1151,45 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
     // weight-gradient tiles owned by this warp: tile id = warp + j * nwarps
     auto dw_phase = [&](int lo, int hi, int aoff, int boff, int n_tiles_n, int blob_mt) {
       if (map_grads)
-        dw_layer<BPREC3, false>(recs, npts, warp, nwarps, dwacc, lo, hi, aoff, boff, n_tiles_n, blob_mt);
+        dw_layer<BPREC3, false, CG>(recs, npts, warp, nwarps, dwacc, lo, hi, aoff, boff, n_tiles_n, blob_mt);
     };
     // d w_col1 += c1^T draw        (8-wide n tile over raw[4] + 4 floats of the next record:
-    dw_phase(0, 2, R_C1, R_RAW, 1, -1);  //  columns 3..7 are never written out)
+    dw_phase(0, 2, L::C1, L::RAW, 1, -1);  //  columns 3..7 are never written out)
     __syncthreads();
     float draw3 = 0.f;
     if (active) {
-      const float4 dr = *reinterpret_cast<const float4*>(rec + R_RAW);
+      const float4 dr = *reinterpret_cast<const float4*>(rec + L::RAW);
       draw3 = dr.w;
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
-        const float* w = sw + SWC1 + j * LDC1;
-        const float c1 = rec[R_C1 + j];
-        rec[R_C1 + j] = (c1 > 0.f) ? (dr.x * w[0] + dr.y * w[1] + dr.z * w[2]) : 0.f;
+        const float* w = sw + W::SWC1 + j * LDC1;
+        const float c1 = rec[L::C1 + j];
+        rec[L::C1 + j] = (c1 > 0.f) ? (dr.x * w[0] + dr.y * w[1] + dr.z * w[2]) : 0.f;
       }
     }
     __syncthreads();
-    // d w_col0 += [blob, geo, sdf]^T dc1pre   (row 63 is discarded at write-out)
-    dw_phase(2, 18, R_BLOB, R_C1, 4, -1);
+    // d w_col0 += [blob, (cfeat,) geo, sdf]^T dc1pre   (row NC is discarded at write-out)
+    dw_phase(2, W::SDF1_LO, R_BLOB, L::C1, 4, -1);
     __syncthreads();
-    if (warp_active) backward_geo<BPREC3, 2, false>(wrec, sw);
+    if (warp_active) backward_geo<BPREC3, 2, false, CG>(wrec, sw);
+    if (CG && warp_active && (map_grads || need_dx)) {
+      // dcfeat = dc1pre Wc0[:, 48:80] into the CFEAT slots (their last reader, the d w_col0
+      // tiles, finished before the barrier above)
+      float c[2][4][4];
+      zero_c(c);
+      warp_gemm<4, 4, true, BPREC3, REC>(wrec, L::C1, sw + SWC0, LDC0, 0, 48, c);
+      store_c<PLAIN, REC>(wrec, C_CFEAT, c);
+    }
     __syncwarp();
-    if (active) rec[R_SDF] = draw3;
+    if (active) rec[L::SDF] = draw3;
     __syncthreads();
     // d w_sdf1 += h1^T dH
-    dw_phase(18, 22, R_H1, R_GEO, 2, -1);
+    dw_phase(W::SDF1_LO, W::SDF0_LO, L::H1, L::GEO, 2, -1);
     __syncthreads();
-    if (warp_active) backward_h1<BPREC3, 2, false>(wrec, sw);
+    if (warp_active) backward_h1<BPREC3, 2, false, CG>(wrec, sw);
     __syncthreads();
     // d w_sdf0 += x^T dh1pre
-    dw_phase(22, 42, R_FEAT, R_H1, 4, -1);
+    dw_phase(W::SDF0_LO, W::DW, R_FEAT, L::H1, 4, -1);
     // (readers of C1 / GEO slots are done: dW phases 2 and 3 finished before the last barrier)
     float hdx[2][2][3];  // hash-path d loss / d x for rows (mt, g / g+8), fragment layout
 #pragma unroll
@@ -1143,15 +1201,15 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         // dblob = dc1pre Wc0[:, 0:48] + dh1pre W0[:, 32:80]  -> scratch (C1 slots 0..31, GEO 32..47)
         float c[2][6][4];
         zero_c(c);
-        warp_gemm<4, 6, true, BPREC3, REC>(wrec, R_C1, sw + SWC0, LDC0, 0, 0, c);
-        warp_gemm<4, 6, true, BPREC3, REC>(wrec, R_H1, sw + SW0, LD0, 0, 32, c);
+        warp_gemm<4, 6, true, BPREC3, REC>(wrec, L::C1, sw + SWC0, LDC0, 0, 0, c);
+        warp_gemm<4, 6, true, BPREC3, REC>(wrec, L::H1, sw + SW0, LD0, 0, 32, c);
         __syncwarp();
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
           for (int nt = 0; nt < 6; ++nt) {
             const int col = nt * 8 + 2 * t;
-            const int off = (col < 32) ? (R_C1 + col) : (R_GEO + col - 32);
+            const int off = (col < 32) ? (L::C1 + col) : (L::GEO + col - 32);
             float* q0 = wrec + (mt * 16 + g) * REC + off;
             *reinterpret_cast<float2*>(q0) = make_float2(c[mt][nt][0], c[mt][nt][1]);
             *reinterpret_cast<float2*>(q0 + 8 * REC) = make_float2(c[mt][nt][2], c[mt][nt][3]);
@@ -1161,7 +1219,7 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
         // dfeat = dh1pre W0[:, 0:32]; lane (g,t) holds (f0,f1) of level 4*nt+t for rows g, g+8
         float c[2][4][4];
         zero_c(c);
-        warp_gemm<4, 4, true, BPREC3, REC>(wrec, R_H1, sw + SW0, LD0, 0, 0, c);
+        warp_gemm<4, 4, true, BPREC3, REC>(wrec, L::H1, sw + SW0, LD0, 0, 0, c);
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -1184,6 +1242,24 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
                   hdx[mt][h][0] += d3.x; hdx[mt][h][1] += d3.y; hdx[mt][h][2] += d3.z;
                 }
               }
+              if constexpr (CG) {  // the colour grid: d loss / d cfeat of the same levels from CFEAT
+                const float* cf = recs + row * REC + C_CFEAT;
+                LevelItems<4> it;
+                bool any = false;
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt) {
+                  const float2 gv = *reinterpret_cast<const float2*>(cf + 2 * (4 * nt + t));
+                  it.g[nt][0] = gv.x; it.g[nt][1] = gv.y;
+                  it.on[nt] = (4 * nt + t) < P.gc.n_levels && (gv.x != 0.f || gv.y != 0.f);
+                  any |= it.on[nt];
+                }
+                if (any) {
+                  const float3 d3 = hash_backward_multi<4>(P.table_c, P.d_table_c, s_lv + kL, t,
+                                                           it, x3[0], x3[1], x3[2], need_dx,
+                                                           map_grads);
+                  hdx[mt][h][0] += d3.x; hdx[mt][h][1] += d3.y; hdx[mt][h][2] += d3.z;
+                }
+              }
             }
           }
       }
@@ -1198,25 +1274,25 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
               float v = hdx[mt][h][d];
               v += __shfl_xor_sync(0xffffffffu, v, 1);
               v += __shfl_xor_sync(0xffffffffu, v, 2);
-              if (t == 0) wrec[(mt * 16 + g + 8 * h) * REC + R_RAW + d] = v;
+              if (t == 0) wrec[(mt * 16 + g + 8 * h) * REC + L::RAW + d] = v;
             }
         __syncwarp();
         if (active) {
-          float dxn[3] = {rec[R_RAW], rec[R_RAW + 1], rec[R_RAW + 2]};
-          blob_backward(xn, [&](int i) { return (i < 32) ? rec[R_C1 + i] : rec[R_GEO + i - 32]; }, dxn);
+          float dxn[3] = {rec[L::RAW], rec[L::RAW + 1], rec[L::RAW + 2]};
+          blob_backward(xn, [&](int i) { return (i < 32) ? rec[L::C1 + i] : rec[L::GEO + i - 32]; }, dxn);
           // park d loss / d pts and z * d loss / d pts in the (dead) C1 slots 0..5
           float dp[3];
 #pragma unroll
           for (int d = 0; d < 3; ++d)
             dp[d] = (float)((double)dxn[d] * P.g.binv[d]);
-          rec[R_C1 + 0] = dp[0]; rec[R_C1 + 1] = dp[1]; rec[R_C1 + 2] = dp[2];
-          rec[R_C1 + 3] = dp[0] * zv; rec[R_C1 + 4] = dp[1] * zv; rec[R_C1 + 5] = dp[2] * zv;
+          rec[L::C1 + 0] = dp[0]; rec[L::C1 + 1] = dp[1]; rec[L::C1 + 2] = dp[2];
+          rec[L::C1 + 3] = dp[0] * zv; rec[L::C1 + 4] = dp[1] * zv; rec[L::C1 + 5] = dp[2] * zv;
         }
       }
     }
     __syncthreads();
     if (need_dx) {
-      for (int q = warp; q < nr; q += nwarps) ray_grads<false>(P, recs + (size_t)(q * S) * REC, r0 + q, lane);
+      for (int q = warp; q < nr; q += nwarps) ray_grads<false, CG>(P, recs + (size_t)(q * S) * REC, r0 + q, lane);
       __syncthreads();
     }
   }
@@ -1231,11 +1307,21 @@ __global__ void __launch_bounds__(256) k_fused(const Params P) {
 #pragma unroll
       for (int j = 0; j < SLOTS; ++j) {
         const int id = warp + j * nwarps;
-        if (id < DW_TILES) dw_store(P, id, dwacc[j]);
+        if (id < W::DW) dw_store<CG>(P, id, dwacc[j]);
       }
     }
   }
 }
+
+template <bool BWD, bool PREC3, bool BPREC3, int SLOTS>
+__global__ void __launch_bounds__(256) k_fused(const Params P) {
+  fused_tile<false, BWD, PREC3, BPREC3, SLOTS>(P);
+}
+template <bool BWD, bool PREC3, bool BPREC3, int SLOTS>
+__global__ void __launch_bounds__(256) k_fused_c(const ParamsC P) {
+  fused_tile<true, BWD, PREC3, BPREC3, SLOTS>(P);
+}
+
 
 // ----------------------------------------------------------- fused, grouped ---
 // v5: the same record-based algorithm, re-organised for latency hiding.  One persistent CTA
@@ -1816,15 +1902,24 @@ struct QueryParams {
   float* geo;         // [P,15] or NULL
   float* feat;        // [P,32] hash features (query_sdf(embed=True)) or NULL
 };
+// k_query_c: the colour grid on top (normalised coordinates come from g's bound)
+struct QueryParamsC : QueryParams {
+  GridDev gc;
+  const float* table_c;
+};
 
-__global__ void __launch_bounds__(128) k_query(const QueryParams Q) {
+// The query kernel's body; CG: with the colour grid (k_query_c, ColorSDFNet).
+template <bool CG, typename QT>
+__device__ __forceinline__ void query_points(const QT& Q) {
+  constexpr int NC = Wts<CG>::NC;
   extern __shared__ __align__(16) float qrec[];  // 128 records
-  __shared__ Lv s_lv[kL];
+  __shared__ Lv s_lv[CG ? 2 * kL : kL];  // the colour grid's levels at kL
   load_levels(s_lv, Q.g);
+  if constexpr (CG) load_levels(s_lv + kL, Q.gc);
   __syncthreads();
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= Q.P) return;
-  float* rec = qrec + threadIdx.x * REC;
+  float* rec = qrec + threadIdx.x * Rec<false, CG>::N;
   float xn[3];
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
@@ -1832,6 +1927,7 @@ __global__ void __launch_bounds__(128) k_query(const QueryParams Q) {
     xn[d] = Q.normalised ? v : normalise(v, Q.g.bmin[d], Q.g.bmax[d]);
   }
   encode<1>(Q.table, Q.g.n_levels, s_lv, xn, rec, 0);
+  if constexpr (CG) encode<1>(Q.table_c, Q.gc.n_levels, s_lv + kL, xn, rec + C_CFEAT, 0);
   blob_forward(xn, rec);
   if (Q.feat)
 #pragma unroll 4
@@ -1858,14 +1954,16 @@ __global__ void __launch_bounds__(128) k_query(const QueryParams Q) {
   if (Q.geo)
     for (int j = 0; j < 15; ++j) Q.geo[(size_t)p * 15 + j] = so[1 + j];
   if (!Q.raw) return;
-  // colour: c1 = relu(Wc0 [blob, geo]);  rgb logits = Wc1 c1
+  // colour: c1 = relu(Wc0 [blob, (cfeat,) geo]);  rgb logits = Wc1 c1
   float c1[32];
 #pragma unroll 1
   for (int j = 0; j < 32; ++j) {
     float a = 0.f;
-    const float* w = Q.w_col0 + j * 63;
+    const float* w = Q.w_col0 + j * NC;
     for (int i = 0; i < 48; ++i) a = fmaf(__ldg(w + i), rec[R_BLOB + i], a);
-    for (int i = 0; i < 15; ++i) a = fmaf(__ldg(w + 48 + i), so[1 + i], a);
+    if constexpr (CG)
+      for (int i = 0; i < 32; ++i) a = fmaf(__ldg(w + 48 + i), rec[C_CFEAT + i], a);
+    for (int i = 0; i < 15; ++i) a = fmaf(__ldg(w + NC - 15 + i), so[1 + i], a);
     c1[j] = fmaxf(a, 0.f);
   }
   float o3[3];
@@ -1878,6 +1976,9 @@ __global__ void __launch_bounds__(128) k_query(const QueryParams Q) {
   }
   *reinterpret_cast<float4*>(Q.raw + (size_t)p * 4) = make_float4(o3[0], o3[1], o3[2], so[0]);
 }
+
+__global__ void __launch_bounds__(128) k_query(const QueryParams Q) { query_points<false>(Q); }
+__global__ void __launch_bounds__(128) k_query_c(const QueryParamsC Q) { query_points<true>(Q); }
 
 static int fill_grid(GridDev& g, const XrdHashGrid* h) {
   if (h->n_levels < 1 || h->n_levels > kL) return XRD_E_SHAPE;
@@ -1926,6 +2027,10 @@ static int pick_rays_per_tile(int S, int requested) {
 template <bool BWD, bool PREC3, bool BPREC3>
 struct TileKernel {
   static constexpr auto fn = &k_fused<BWD, PREC3, BPREC3, BWD ? 6 : 1>;
+};
+template <bool BWD, bool PREC3, bool BPREC3>
+struct TileKernelC {
+  static constexpr auto fn = &k_fused_c<BWD, PREC3, BPREC3, BWD ? 8 : 1>;
 };
 template <bool BWD, bool PREC3, bool BPREC3>
 struct GroupedKernel {
@@ -1981,14 +2086,18 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   if (has_depth && (!cfg->lin_uniform || !cfg->lin_range || !cfg->lin_nodepth)) return XRD_E_NULL;
   if (!has_depth && !cfg->lin_full) return XRD_E_NULL;
   if (grads && (!has_depth || !rays->target_s || !out->losses)) return XRD_E_NULL;
+  const XrdHashGrid* grid_c = mlp->grid_color;  // NULL: one grid (ColorSDFNet_v2)
+  if (grid_c && !grid_c->table) return XRD_E_NULL;
   if (grads) {
     // map gradients are all-or-nothing; d_table == NULL selects the pose-only (tracking) pass
     const int n_map = (grads->d_table != nullptr) + (grads->d_w_sdf0 != nullptr) +
                       (grads->d_w_sdf1 != nullptr) + (grads->d_w_col0 != nullptr) +
-                      (grads->d_w_col1 != nullptr);
-    if (n_map != 0 && n_map != 5) return XRD_E_NULL;
+                      (grads->d_w_col1 != nullptr) +
+                      (grid_c ? (grads->d_table_color != nullptr) : 0);
+    if (n_map != 0 && n_map != (grid_c ? 6 : 5)) return XRD_E_NULL;
     if (n_map == 0 && !grads->d_rays_o && !grads->d_rays_d) return XRD_E_NULL;
     if (grads->d_table && !aligned16(grads->d_table)) return XRD_E_SHAPE;
+    if (grid_c && grads->d_table_color && !aligned16(grads->d_table_color)) return XRD_E_SHAPE;
   }
   const StepWs L(workspace, R, S);
   if (int st = L.check(workspace_bytes)) return st;
@@ -2019,7 +2128,7 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   }
   if (phase == 1) return XRD_OK;
 
-  Params P;
+  ParamsC P;  // k_fused and k_fused_g take its Params part
   int st = fill_grid(P.g, grid);
   if (st != XRD_OK) return st;
   P.R = R; P.S = S;
@@ -2040,6 +2149,14 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   } else {
     P.d_table = P.d_w_sdf0 = P.d_w_sdf1 = P.d_w_col0 = P.d_w_col1 = P.d_rays_o = P.d_rays_d = nullptr;
   }
+  P.table_c = nullptr;
+  P.d_table_c = nullptr;
+  if (grid_c) {
+    st = fill_grid(P.gc, grid_c);
+    if (st != XRD_OK) return st;
+    P.table_c = grid_c->table;
+    P.d_table_c = grads ? grads->d_table_color : nullptr;
+  }
   const int sms = num_sms();
   // Kernel choice (rays_per_tile: 0 = automatic, -1 = tile kernel, -2 = grouped kernel, > 0 = tile
   // kernel with that many rays per tile).  Automatic: the grouped kernel runs the gradient pass
@@ -2048,8 +2165,12 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   // 0.433 ms of the benchmark's 4096-ray mapping step.  On scripts/quick_time_coslam.py's
   // random rays (mode 1) the two are close: tile / grouped fwd+bwd R = 1024: 214 / 195 us,
   // 4096: 462 / 468, 16384: 1470 / 1520, 65536: 5463 / 5818 us; the rule is unchanged.
+  // A colour-grid pass runs on the tile kernel: the grouped kernel's three groups of 96 records
+  // would need 32 more floats each, which with its weight-gradient buffer outgrows the 227 KB a
+  // CTA may opt in to.
+  if (grid_c && cfg->rays_per_tile == -2) return XRD_E_SHAPE;
   bool grouped = false;
-  if (S <= GP) {
+  if (S <= GP && !grid_c) {
     const int units = (R + GP / S - 1) / (GP / S);
     grouped = cfg->rays_per_tile == -2 || (cfg->rays_per_tile == 0 && grads && units >= 4 * sms);
   }
@@ -2071,21 +2192,37 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
     XRD_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     XRD_CUDA_TRY(cudaFuncGetAttributes(&fa, kernel));
     if (smem_g + fa.sharedSizeBytes > (size_t)smem_optin) return XRD_E_SHAPE;
-    st = launch_fused(kernel, (P.n_tiles + NGROUPS - 1) / NGROUPS, GT * NGROUPS, smem_g, stream, P,
-                      queue);
+    st = launch_fused(kernel, (P.n_tiles + NGROUPS - 1) / NGROUPS, GT * NGROUPS, smem_g, stream,
+                      static_cast<const Params&>(P), queue);
   } else {
     // tile kernel (k_fused): rays_per_tile > 0 selects its tile size, < 0 its default
     const int NR = pick_rays_per_tile(S, cfg->rays_per_tile);
     if (NR < 1 || NR * S > 256) return XRD_E_SHAPE;
     int threads = (NR * S + 31) / 32 * 32;
     if (grads && threads < 224) threads = 224;  // 7+ warps own the 42 weight-gradient tiles (6 each)
-    if (grads && (DW_TILES + threads / 32 - 1) / (threads / 32) != 6) return XRD_E_SHAPE;
     P.NR = NR;
     P.n_tiles = (R + NR - 1) / NR;
-    // weights + (threads + 8) records + per point z and xn
-    const size_t smem = sizeof(float) * ((size_t)SW_TOTAL + (size_t)(threads + 8) * REC + 6 * (size_t)NR * S);
-    st = launch_fused(fused_kernel<TileKernel>(grads != nullptr, cfg->precision), P.n_tiles, threads,
-                      smem, stream, P);
+    if (!grid_c) {
+      if (grads && (DW_TILES + threads / 32 - 1) / (threads / 32) != 6) return XRD_E_SHAPE;
+      // weights + (threads + 8) records + per point z and xn
+      const size_t smem = sizeof(float) * ((size_t)SW_TOTAL + (size_t)(threads + 8) * REC + 6 * (size_t)NR * S);
+      st = launch_fused(fused_kernel<TileKernel>(grads != nullptr, cfg->precision), P.n_tiles,
+                        threads, smem, stream, static_cast<const Params&>(P));
+    } else {
+      // 50 weight-gradient tiles: 8 slots per warp cover them from 7 warps on
+      if (grads && (Wts<true>::DW + threads / 32 - 1) / (threads / 32) > 8) return XRD_E_SHAPE;
+      // gradient pass, 224 threads (S = 43): 219 304 B of the 227 KB opt-in (NR * S above 224
+      // does not fit); forward only, compact record: 177 792 B at 256 threads
+      const size_t smem = sizeof(float) * ((size_t)Wts<true>::TOTAL +
+                                           (size_t)(threads + 8) * (grads ? CREC : FREC) +
+                                           6 * (size_t)NR * S);
+      int dev = 0, smem_optin = 0;
+      XRD_CUDA_TRY(cudaGetDevice(&dev));
+      XRD_CUDA_TRY(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+      if (smem + 2 * kL * sizeof(Lv) > (size_t)smem_optin) return XRD_E_SHAPE;
+      st = launch_fused(fused_kernel<TileKernelC>(grads != nullptr, cfg->precision), P.n_tiles,
+                        threads, smem, stream, P);
+    }
   }
   if (st != XRD_OK || !grads) return st;
   FinalizeParams fp{loss_acc, P.counts, out->losses, P.Rg, S, cfg->w_rgb, cfg->w_depth, cfg->w_sdf, cfg->w_fs};
@@ -2193,17 +2330,30 @@ extern "C" int xrd_coslam_query(const XrdHashGrid* grid, const XrdCoslamMlp* mlp
   if (!grid || !grid->table || !pts) return XRD_E_NULL;
   if ((raw || geo) && (!mlp || !mlp->w_sdf0 || !mlp->w_sdf1)) return XRD_E_NULL;
   if (raw && (!mlp->w_col0 || !mlp->w_col1)) return XRD_E_NULL;
+  const XrdHashGrid* grid_c = mlp ? mlp->grid_color : nullptr;
+  if (grid_c && !grid_c->table) return XRD_E_NULL;
   if (n_points <= 0) return XRD_OK;
-  QueryParams Q;
+  QueryParamsC Q;  // k_query takes its QueryParams part
   int st = fill_grid(Q.g, grid);
   if (st != XRD_OK) return st;
   Q.table = grid->table;
   Q.w_sdf0 = mlp ? mlp->w_sdf0 : nullptr; Q.w_sdf1 = mlp ? mlp->w_sdf1 : nullptr;
   Q.w_col0 = mlp ? mlp->w_col0 : nullptr; Q.w_col1 = mlp ? mlp->w_col1 : nullptr;
   Q.pts = pts; Q.P = n_points; Q.normalised = normalised; Q.raw = raw; Q.geo = geo; Q.feat = feat;
-  const size_t smem = 128 * REC * sizeof(float);
-  XRD_CUDA_TRY(cudaFuncSetAttribute(k_query, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_query<<<(n_points + 127) / 128, 128, smem, (cudaStream_t)stream_>>>(Q);
+  Q.table_c = nullptr;
+  if (grid_c) {
+    st = fill_grid(Q.gc, grid_c);
+    if (st != XRD_OK) return st;
+    Q.table_c = grid_c->table;
+  }
+  const size_t smem = 128 * (grid_c ? CREC : REC) * sizeof(float);
+  if (grid_c) {
+    XRD_CUDA_TRY(cudaFuncSetAttribute(k_query_c, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_query_c<<<(n_points + 127) / 128, 128, smem, (cudaStream_t)stream_>>>(Q);
+  } else {
+    XRD_CUDA_TRY(cudaFuncSetAttribute(k_query, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_query<<<(n_points + 127) / 128, 128, smem, (cudaStream_t)stream_>>>(Q);
+  }
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }

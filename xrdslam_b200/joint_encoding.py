@@ -3,8 +3,9 @@
 Host-side mirror of slam/models/joint_encoding.py (reference @ f0366f20): same
 class name, same config fields, same ``forward / get_outputs / get_loss_dict /
 get_param_groups / smoothness / query_sdf / query_color / query_fn / color_func``
-signatures, same parameter-group names (``decoder``, ``embed_fn``) and the same
-state_dict keys (``embed_fn.params``, ``decoder.sdf_net.model.{0,2}.weight``,
+signatures, same parameter-group names (``decoder``, ``embed_fn``, and
+``embed_fn_color`` with ``oneGrid=False``) and the same state_dict keys
+(``embed_fn.params``, ``embed_fn_color.params``, ``decoder.sdf_net.model.{0,2}.weight``,
 ``decoder.color_net.model.{0,2}.weight``).
 
 Nothing is computed in PyTorch: ``forward`` enqueues the fused sm_90a kernels of
@@ -120,26 +121,37 @@ class ColorSDFNet_v2(nn.Module):
                             1 + config.geo_feat_dim)
 
 
+class ColorSDFNet(nn.Module):
+    """Parameter container of decoder_coslam.py:113-136 (colour grid + SDF grid): the
+    colour branch reads [oneblob48, colour_hash32, geo15]."""
+    def __init__(self, config, input_ch, input_ch_color, input_ch_pos):
+        super().__init__()
+        self.color_net = _Seq(input_ch_pos + input_ch_color + config.geo_feat_dim,
+                              config.hidden_dim_color, 3)
+        self.sdf_net = _Seq(input_ch + input_ch_pos, config.hidden_dim,
+                            1 + config.geo_feat_dim)
+
+
 class _CoslamStep(torch.autograd.Function):
-    """losses[4] = fused(rays, table, weights); backward hands out the gradients
-    the kernel already produced."""
+    """losses[4] = fused(rays, table, weights[, colour table]); backward hands out the
+    gradients the kernel already produced."""
     @staticmethod
     def forward(ctx, rays_o, rays_d, table, w0, w1, wc0, wc1, model, target_s,
-                target_d, noise):
-        need = any(ctx.needs_input_grad[:7])
+                target_d, noise, table_c=None):
+        need = any(ctx.needs_input_grad[:7]) or ctx.needs_input_grad[11]
         need_rays = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         # tracking: only the pose is optimised -> skip scatter / weight-gradient tiles
-        map_grads = any(ctx.needs_input_grad[2:7]) and not (
+        map_grads = (any(ctx.needs_input_grad[2:7]) or ctx.needs_input_grad[11]) and not (
             model.freeze_map_grads and need_rays)
         outs, grads = model._launch(rays_o, rays_d, table, w0, w1, wc0, wc1,
                                     target_s, target_d, noise, with_grads=need,
                                     need_ray_grads=need_rays,
-                                    map_grads=map_grads)
+                                    map_grads=map_grads, table_c=table_c)
         ctx.grads = grads
         ctx.model = model
         ctx.strict = model.config.strict_loss_grad
         ctx.inputs = (rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
-                      target_d, noise, model._last_seed)
+                      target_d, noise, model._last_seed, table_c)
         ret = (outs['losses'], outs['rgb'], outs['depth'], outs['disp_map'],
                outs['acc_map'], outs['depth_var'], outs['z_vals'], outs['raw'])
         ctx.mark_non_differentiable(*ret[1:])
@@ -156,21 +168,21 @@ class _CoslamStep(torch.autograd.Function):
                 # non-unit upstream gradient: re-run the fused pass with the
                 # per-term scales (the kernel is linear in them)
                 (rays_o, rays_d, table, w0, w1, wc0, wc1, ts, td, noise,
-                 seed) = ctx.inputs
+                 seed, table_c) = ctx.inputs
                 _, grads = ctx.model._launch(
                     rays_o, rays_d, table, w0, w1, wc0, wc1, ts, td, noise,
                     with_grads=True, need_ray_grads=True,
-                    loss_scale=[float(v) for v in g], seed=seed)
+                    loss_scale=[float(v) for v in g], seed=seed, table_c=table_c)
         else:
             # sync-free: total-loss scaling is honoured, unequal per-term scales poison
             # the gradients with NaN (base_model.upstream_scale)
             s = upstream_scale(g_losses)
             keys = ('d_rays_o', 'd_rays_d', 'd_table', 'd_w_sdf0', 'd_w_sdf1', 'd_w_col0',
-                    'd_w_col1')
+                    'd_w_col1', 'd_table_color')
             grads = dict(zip(keys, scale_grads([grads[k] for k in keys], s)))
         return (grads['d_rays_o'], grads['d_rays_d'], grads['d_table'],
                 grads['d_w_sdf0'], grads['d_w_sdf1'], grads['d_w_col0'],
-                grads['d_w_col1'], None, None, None, None)
+                grads['d_w_col1'], None, None, None, None, grads['d_table_color'])
 
 
 class JointEncoding(Model):
@@ -187,10 +199,10 @@ class JointEncoding(Model):
     def populate_modules(self):
         super().populate_modules()
         cfg = self.config
-        if not cfg.oneGrid or cfg.tcnn_network or cfg.training_n_importance:
+        if cfg.tcnn_network or cfg.training_n_importance:
             raise NotImplementedError(
-                'CUDA path covers the reference defaults: oneGrid=True, '
-                'tcnn_network=False, n_importance=0 (input_config.py:253-254)')
+                'CUDA path covers tcnn_network=False, n_importance=0 (the reference '
+                'defaults, input_config.py:253-254)')
         if not cfg.tcnn_encoding:
             raise NotImplementedError('tcnn_encoding=True is the co-slam '
                                       'default (input_config.py:254)')
@@ -198,7 +210,7 @@ class JointEncoding(Model):
                 cfg.pos_nbins, cfg.num_layers, cfg.num_layers_color) != (
                     32, 32, 15, 16, 2, 2):
             raise NotImplementedError('decoder shape fixed to the reference '
-                                      'default 80-32-16 / 63-32-3')
+                                      'default 80-32-16 / 63-32-3 (95-32-3 with oneGrid=False)')
         self.bounding_box = torch.as_tensor(np.asarray(self.bounding_box),
                                             dtype=torch.float64)
         self.get_resolution()
@@ -245,15 +257,27 @@ class JointEncoding(Model):
                                        per_level_scale)
         self.input_ch = self.embed_fn.n_output_dims
         self.input_ch_pos = 3 * self.config.pos_nbins  # OneBlob, no params
+        if not self.config.oneGrid:
+            # the colour grid: the same HashGrid config at resolution_color
+            pls_color = np.exp2(np.log2(self.resolution_color / base) / (n_levels - 1))
+            self.embed_fn_color = HashGridParams(n_levels, self.config.hashsize, base,
+                                                 pls_color, seed=1338)
+            self.input_ch_color = self.embed_fn_color.n_output_dims
 
     def get_decoder(self):
-        self.decoder = ColorSDFNet_v2(self.config, input_ch=self.input_ch,
-                                      input_ch_pos=self.input_ch_pos)
+        if not self.config.oneGrid:
+            self.decoder = ColorSDFNet(self.config, input_ch=self.input_ch,
+                                       input_ch_color=self.input_ch_color,
+                                       input_ch_pos=self.input_ch_pos)
+        else:
+            self.decoder = ColorSDFNet_v2(self.config, input_ch=self.input_ch,
+                                          input_ch_pos=self.input_ch_pos)
 
     # ------------------------------------------------------ C-ABI plumbing ---
-    def _grid_struct(self, table):
+    def _grid_struct(self, table, enc=None):
+        """XrdHashGrid of `table` in the layout of `enc` (default: embed_fn)."""
         g = XrdHashGrid()
-        C.memmove(C.byref(g), C.byref(self.embed_fn.layout), C.sizeof(g))
+        C.memmove(C.byref(g), C.byref((enc or self.embed_fn).layout), C.sizeof(g))
         bb = self.bounding_box
         for d in range(3):
             g.bbox_min[d] = float(bb[d, 0])
@@ -271,8 +295,14 @@ class JointEncoding(Model):
         return (cfg.training_n_sample_d +
                 cfg.training_n_range_d) if with_depth else cfg.training_n_samples
 
-    def _mlp_struct(self, weights):
-        return XrdCoslamMlp(*(ptr(w.detach()) for w in weights))
+    def _mlp_struct(self, weights, table_c=None):
+        """XrdCoslamMlp of the four weights; with oneGrid=False also the colour grid
+        (`table_c`, default embed_fn_color.params)."""
+        m = XrdCoslamMlp(*(ptr(w.detach()) for w in weights))
+        if not self.config.oneGrid:
+            tc = self.embed_fn_color.params if table_c is None else table_c
+            m.grid_color = C.pointer(self._grid_struct(tc.detach(), self.embed_fn_color))
+        return m
 
     def _cfg_struct(self, S, seed=0, seed_dev=None, phase=0, n_rays_global=0,
                     counts_global=None, counts_out=None):
@@ -311,8 +341,11 @@ class JointEncoding(Model):
 
     def _launch(self, rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
                 target_d, noise, with_grads, need_ray_grads=True,
-                loss_scale=None, seed=None, map_grads=True):
+                loss_scale=None, seed=None, map_grads=True, table_c=None):
+        """table_c: the colour grid's table (oneGrid=False; default embed_fn_color.params)."""
         cfg = self.config
+        if not cfg.oneGrid and table_c is None:
+            table_c = self.embed_fn_color.params
         dev = table.device
         _cabi.require_cuda(dev, 'model')
         f32 = dict(dtype=torch.float32, device=dev)
@@ -333,7 +366,7 @@ class JointEncoding(Model):
         o, out = self._outputs(R, S, dev)
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), ptr(ts), ptr(td))
         grid = self._grid_struct(table.detach())
-        mlp = self._mlp_struct((w0, w1, wc0, wc1))
+        mlp = self._mlp_struct((w0, w1, wc0, wc1), table_c)
         if seed is None:
             seed = self._next_seed()
         # sharding applies to mapping only (tracking is per-frame sequential, single GPU)
@@ -352,12 +385,15 @@ class JointEncoding(Model):
                      d_w_col0=z(wc0) if map_grads else None,
                      d_w_col1=z(wc1) if map_grads else None,
                      d_rays_o=torch.empty(R, 3, **f32) if need_ray_grads else None,
-                     d_rays_d=torch.empty(R, 3, **f32) if need_ray_grads else None)
+                     d_rays_d=torch.empty(R, 3, **f32) if need_ray_grads else None,
+                     d_table_color=z(table_c, **f32) if (map_grads and table_c is not None)
+                     else None)
             sc = loss_scale or [1.0, 1.0, 1.0, 1.0]
             gs = XrdCoslamGrads(ptr(g['d_table']), ptr(g['d_w_sdf0']),
                                 ptr(g['d_w_sdf1']), ptr(g['d_w_col0']),
                                 ptr(g['d_w_col1']), ptr(g['d_rays_o']),
-                                ptr(g['d_rays_d']), (C.c_float * 4)(*sc))
+                                ptr(g['d_rays_d']), (C.c_float * 4)(*sc),
+                                ptr(g['d_table_color']))
         ws, ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
 
         def step(grads):
@@ -404,16 +440,17 @@ class JointEncoding(Model):
         w0, w1, wc0, wc1 = self._weights()
         fused = (torch.is_grad_enabled() and target_d is not None
                  and target_s is not None)
+        table_c = None if self.config.oneGrid else self.embed_fn_color.params
         if fused:
             (losses, rgb, depth, disp, acc, var, z_vals,
              raw) = _CoslamStep.apply(rays_o, rays_d, table, w0, w1, wc0, wc1,
-                                      self, target_s, target_d, noise)
+                                      self, target_s, target_d, noise, table_c)
             ret = dict(rgb=rgb, depth=depth, disp_map=disp, acc_map=acc,
                        depth_var=var, z_vals=z_vals, raw=raw)
             ret['_losses'] = losses
             return ret
         o, _ = self._launch(rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
-                            target_d, noise, with_grads=False)
+                            target_d, noise, with_grads=False, table_c=table_c)
         o.pop('losses')
         return o
 
@@ -442,10 +479,13 @@ class JointEncoding(Model):
         return loss_dict
 
     def get_param_groups(self) -> Dict[str, List[Parameter]]:
-        return {
+        groups = {
             'decoder': list(self.decoder.parameters()),
             'embed_fn': list(self.embed_fn.parameters()),
         }
+        if not self.config.oneGrid:
+            groups['embed_fn_color'] = list(self.embed_fn_color.parameters())
+        return groups
 
     def smoothness(self, sample_points=256, voxel_size=0.1, margin=0.05,
                    rand=None, weight=None):
