@@ -226,6 +226,9 @@ typedef struct {
   int* counts_out;           /* DEVICE [4], written in phase 1                  */
   const uint64_t* seed_dev;  /* DEVICE scalar overriding `seed` (read by the kernel:
                               * a captured CUDA graph replays with a fresh seed)  */
+  int n_importance;          /* phase 2 only: the z_vals are a fine pass's
+                              * (xrd_coslam_importance), so with depth n_samples =
+                              * n_sample_d + n_range_d + n_importance; 0 otherwise */
 } XrdCoslamCfg;
 
 /* Per-ray / per-sample outputs (DEVICE, any may be NULL except losses when
@@ -272,6 +275,43 @@ int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
                     const float* noise, XrdCoslamOut* out,
                     XrdCoslamGrads* grads, void* workspace,
                     size_t workspace_bytes, void* stream);
+
+/* Hierarchical (importance) sampling of Co-SLAM's fine pass, training_n_importance > 0
+ * (slam/models/joint_encoding.py:301-315, sample_pdf in slam/model_components/utils.py:31-76).
+ * From a coarse pass of xrd_coslam_step (its z_vals and raw), per ray:
+ *   weights = that pass's composite weights, recomputed by the same device code (bit-identical)
+ *   pdf     = (weights[1:-1] + 1e-5) / sum, cdf = [0, cumsum(pdf)] over the S0-1 bin midpoints
+ *   z_samples = inverse-cdf samples at u: searchsorted(cdf, u, right=True), clamped, linear
+ *               interpolation, denominators < 1e-5 replaced by 1
+ *   z_fine  = sort(z_vals ++ z_samples)                                           [R, S0+N]
+ * u is `u` [R,N] when given, else lin_u [N] for every ray when det (torch.linspace(0.5/N,
+ * 1-0.5/N, N), training_perturb == 0), else Philox uniforms from seed / *seed_dev (a stream
+ * disjoint from the coarse pass's jitter under the same seed).  The fine pass is then
+ * xrd_coslam_step with phase = 2, out->z_vals = z_fine, n_samples = S0+N, cfg.n_importance =
+ * N and counts_global = counts_out (n_fs, n_sdf, n_valid of z_fine, as in phase 1; summed over
+ * the ranks first when mapping rays are sharded).  No workspace.  XRD_E_SHAPE unless
+ * S0 >= 3, N >= 1 and S0 + N <= 256. */
+typedef struct {
+  int n_rays;
+  int n_samples;           /* S0: samples per ray of the coarse pass                */
+  int n_importance;        /* N                                                     */
+  int det;                 /* 1: u = lin_u (when u is NULL)                         */
+  float trunc;             /* as XrdCoslamCfg.trunc, depth_trunc                    */
+  float depth_trunc;
+  const float* z_vals;     /* DEVICE [R,S0]   the coarse pass's z_vals              */
+  const float* raw;        /* DEVICE [R,S0,4] the coarse pass's raw (sdf in [..,3]) */
+  const float* target_d;   /* DEVICE [R], needed with counts_out                    */
+  const float* u;          /* DEVICE [R,N] or NULL                                  */
+  const float* lin_u;      /* DEVICE [N] or NULL                                    */
+  uint64_t seed;
+  const uint64_t* seed_dev;/* DEVICE scalar overriding seed, or NULL                */
+  float* z_fine;           /* DEVICE [R,S0+N]                                       */
+  float* z_samples;        /* DEVICE [R,N] in draw order, or NULL                   */
+  float* z_std;            /* DEVICE [R] std(z_samples, unbiased=False), or NULL    */
+  int* counts_out;         /* DEVICE [4] (zeroed here), or NULL                     */
+} XrdCoslamImportance;
+
+int xrd_coslam_importance(const XrdCoslamImportance* q, void* stream);
 
 size_t xrd_coslam_smoothness_workspace_bytes(int sample_points);
 

@@ -70,7 +70,16 @@ class XrdCoslamCfg(C.Structure):
                 ('lin_full', vp), ('seed', C.c_uint64),
                 ('rays_per_tile', C.c_int), ('precision', C.c_int),
                 ('phase', C.c_int), ('n_rays_global', C.c_int),
-                ('counts_global', vp), ('counts_out', vp), ('seed_dev', vp)]
+                ('counts_global', vp), ('counts_out', vp), ('seed_dev', vp),
+                ('n_importance', C.c_int)]
+
+
+class XrdCoslamImportance(C.Structure):
+    _fields_ = [('n_rays', C.c_int), ('n_samples', C.c_int), ('n_importance', C.c_int),
+                ('det', C.c_int), ('trunc', C.c_float), ('depth_trunc', C.c_float),
+                ('z_vals', vp), ('raw', vp), ('target_d', vp), ('u', vp), ('lin_u', vp),
+                ('seed', C.c_uint64), ('seed_dev', vp), ('z_fine', vp), ('z_samples', vp),
+                ('z_std', vp), ('counts_out', vp)]
 
 
 class XrdCoslamOut(C.Structure):
@@ -302,6 +311,7 @@ SYMBOLS = {
         C.POINTER(XrdCoslamOut),
         C.POINTER(XrdCoslamGrads), vp, C.c_size_t, vp
     ]),
+    'xrd_coslam_importance': (C.c_int, [C.POINTER(XrdCoslamImportance), vp]),
     'xrd_coslam_smoothness_workspace_bytes': (C.c_size_t, [C.c_int]),
     'xrd_coslam_smoothness': (C.c_int, [
         C.POINTER(XrdHashGrid), C.c_int, C.c_double, C.c_double, C.c_float, fp,

@@ -34,6 +34,8 @@
 //              the 95-input colour decoder, and the colour grid's hash backward (scatter into
 //              d_table_c, d loss / d xn).
 //   k_finalize loss accumulators -> the 4 weighted loss terms.
+//   k_importance  hierarchical sampling between a coarse and a fine pass (training_n_importance
+//              > 0): the coarse weights, sample_pdf, the sorted merge and the fine pass's counts.
 #include <math.h>
 
 #include "common.cuh"
@@ -125,6 +127,25 @@ struct SampleParams {
   int* counts;
 };
 
+// The loss normalisers' counts (SURVEY Q9) of one sample at depth zv on a ray of target depth d:
+// free-space samples (c_fs) and samples inside the truncation band (c_sdf).
+__device__ __forceinline__ void count_sample(float zv, float d, float trunc, int& c_fs, int& c_sdf) {
+  const bool front = zv < __fsub_rn(d, trunc);
+  const bool back = zv > __fadd_rn(d, trunc);
+  c_fs += front;
+  c_sdf += (!front && !back && d > 0.f);
+}
+// One warp's counts into counts[0..2] = n_fs, n_sdf, n_valid (c_valid: lane 0's).
+__device__ __forceinline__ void add_counts(int* counts, int c_fs, int c_sdf, int c_valid, int lane) {
+  c_fs = warp_sum_i(c_fs);
+  c_sdf = warp_sum_i(c_sdf);
+  if (lane == 0) {
+    if (c_fs) atomicAdd(&counts[0], c_fs);
+    if (c_sdf) atomicAdd(&counts[1], c_sdf);
+    if (c_valid) atomicAdd(&counts[2], c_valid);
+  }
+}
+
 __global__ void __launch_bounds__(128) k_sample(SampleParams p) {
   __shared__ float zs[4][260];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -178,24 +199,11 @@ __global__ void __launch_bounds__(128) k_sample(SampleParams p) {
         zv = __fadd_rn(lo, __fmul_rn(__fsub_rn(hi, lo), u));
       }
       p.z_vals[(size_t)r * S + k] = zv;
-      if (p.has_depth) {
-        const bool front = zv < __fsub_rn(d, p.trunc);
-        const bool back = zv > __fadd_rn(d, p.trunc);
-        c_fs += front;
-        c_sdf += (!front && !back && d > 0.f);
-      }
+      if (p.has_depth) count_sample(zv, d, p.trunc, c_fs, c_sdf);
     }
     if (p.has_depth && lane == 0) c_valid = (d > 0.f && d < p.depth_trunc);
   }
-  if (p.has_depth) {
-    c_fs = warp_sum_i(c_fs);
-    c_sdf = warp_sum_i(c_sdf);
-    if (lane == 0) {
-      if (c_fs) atomicAdd(&p.counts[0], c_fs);
-      if (c_sdf) atomicAdd(&p.counts[1], c_sdf);
-      if (c_valid) atomicAdd(&p.counts[2], c_valid);
-    }
-  }
+  if (p.has_depth) add_counts(p.counts, c_fs, c_sdf, c_valid, lane);
 }
 
 // --------------------------------------------------------------- encoding ---
@@ -919,17 +927,16 @@ __device__ __forceinline__ void backward_h1(float* __restrict__ wrec, const floa
 // across the sample loops.
 // (The RAW-slot pointer, rather than the record base, keeps k_fused_g at 96 registers and an
 // 8-byte stack: with the record base, ptxas reloads a spilled address inside dw_tile's loop.)
-template <int N, bool BWD, int KPL, typename AddLoss>
-__device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& ln, float* raw,
-                                              const float* zr, float* sg_s, float* u_s, int rr,
-                                              int lane, AddLoss add_loss) {
+// sdf2weights of one ray (one warp; samples, KPL and sg_r / u_r as in composite_ray): sg_r[j] =
+// sigma(s/tr), u_r[j] = the unnormalised, truncated weight; returns the normaliser W (the weight
+// of sample kk is u_r[j] / W).  COLOURS: also replace the rgb logits raw[kk*N + 0..2] by their
+// sigmoids.  xrd_coslam_importance recomputes the coarse pass's weights through this function,
+// so the pdf it samples comes from the weights that pass composited, bit for bit.
+template <int N, int KPL, bool COLOURS>
+__device__ __forceinline__ float composite_weights(float* raw, const float* zr, int S, float tr,
+                                                   float* sg_r, float* u_r, int lane) {
   constexpr int UNROLL = KPL > 0 ? KPL : 1;
-  const int S = P.S;
   const int n = KPL > 0 ? KPL : (S + 31) / 32;  // samples per lane
-  const float tr = P.trunc;
-  float sg_reg[UNROLL], u_reg[UNROLL];
-  float* sg_r = KPL > 0 ? sg_reg : sg_s;
-  float* u_r = KPL > 0 ? u_reg : u_s;
   int first = 0x7fffffff;
 #pragma unroll UNROLL
   for (int i = 0; i < n; ++i) {
@@ -944,16 +951,18 @@ __device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& l
       const float sg = sigmoidf_acc(s / tr);
       sg_r[j] = sg;
       u_r[j] = sg * sigmoidf_acc((-s) / tr);
-      rp[0] = sigmoidf_acc(rp[0]);
-      rp[1] = sigmoidf_acc(rp[1]);
-      rp[2] = sigmoidf_acc(rp[2]);
+      if (COLOURS) {
+        rp[0] = sigmoidf_acc(rp[0]);
+        rp[1] = sigmoidf_acc(rp[1]);
+        rp[2] = sigmoidf_acc(rp[2]);
+      }
       if (kk < S - 1 && raw[(kk + 1) * N + 3] * s < 0.f) first = min(first, kk);
     }
   }
   first = warp_min_i(first);
   if (first == 0x7fffffff) first = 0;
   __syncwarp();
-  const float zlim = zr[first] + P.trunc;
+  const float zlim = zr[first] + tr;
   float usum = 0.f;
 #pragma unroll UNROLL
   for (int i = 0; i < n; ++i) {
@@ -965,7 +974,21 @@ __device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& l
     }
   }
   usum = warp_sum(usum);
-  const float W = usum + 1e-8f;
+  return usum + 1e-8f;
+}
+
+template <int N, bool BWD, int KPL, typename AddLoss>
+__device__ __forceinline__ void composite_ray(const Params& P, const LossNorm& ln, float* raw,
+                                              const float* zr, float* sg_s, float* u_s, int rr,
+                                              int lane, AddLoss add_loss) {
+  constexpr int UNROLL = KPL > 0 ? KPL : 1;
+  const int S = P.S;
+  const int n = KPL > 0 ? KPL : (S + 31) / 32;  // samples per lane
+  const float tr = P.trunc;
+  float sg_reg[UNROLL], u_reg[UNROLL];
+  float* sg_r = KPL > 0 ? sg_reg : sg_s;
+  float* u_r = KPL > 0 ? u_reg : u_s;
+  const float W = composite_weights<N, KPL, true>(raw, zr, S, tr, sg_r, u_r, lane);
   float o_r = 0.f, o_g = 0.f, o_b = 0.f, o_d = 0.f, o_acc = 0.f;
 #pragma unroll UNROLL
   for (int i = 0; i < n; ++i) {
@@ -1995,6 +2018,140 @@ static int fill_grid(GridDev& g, const XrdHashGrid* h) {
   return XRD_OK;
 }
 
+// -------------------------------------------------------------- importance ---
+// Hierarchical sampling between the coarse and the fine pass (joint_encoding.py:301-315 and
+// sample_pdf, slam/model_components/utils.py:31-76), one warp per ray:
+//   the coarse pass's weights (composite_weights on its raw sdf and z_vals)
+//   -> pdf of weights[1:-1] + 1e-5 -> cdf = [0, cumsum(pdf)], the prefix sums in float64 and each
+//      rounded to float, as torch.cumsum does on float32
+//   -> inverse-cdf samples at u over the S0-1 bin midpoints
+//   -> z_fine = sort(z_vals ++ z_samples), each value written at its rank
+//   -> the fine pass's counts n_fs, n_sdf, n_valid over z_fine.
+struct ImportanceParams {
+  int R, S, N, det;
+  float trunc, depth_trunc;
+  const float *z_vals, *raw, *target_d, *u, *lin_u;
+  uint64_t seed;
+  const uint64_t* seed_dev;
+  float *z_fine, *z_samples, *z_std;
+  int* counts;
+};
+constexpr int kImpWarps = 4;
+// shared floats per warp: sigma / pdf, weights, cdf, bin midpoints (S each), merged values (S + N)
+__host__ __device__ constexpr int imp_floats(int S, int N) { return 4 * S + S + N; }
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(kImpWarps * 32) k_importance(ImportanceParams p) {
+  extern __shared__ float ism[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.x * kImpWarps + warp;
+  const int S = p.S, N = p.N, T = S + N, M = S - 2;  // M inner weights; bins and cdf: M + 1
+  float* pdf = ism + (size_t)warp * imp_floats(S, N);
+  float* wu = pdf + S;
+  float* cdf = wu + S;
+  float* mid = cdf + S;
+  float* zall = mid + S;
+  int c_fs = 0, c_sdf = 0, c_valid = 0;
+  if (r < p.R) {  // warp-uniform
+    const float* zr = p.z_vals + (size_t)r * S;
+    // (COLOURS = false: raw is only read)
+    const float W = composite_weights<4, 0, false>(const_cast<float*>(p.raw) + (size_t)r * S * 4,
+                                                   zr, S, p.trunc, pdf, wu, lane);
+    __syncwarp();  // the weights other lanes wrote in composite_weights are read below
+    double part = 0.0;
+    for (int j = lane; j < M; j += 32) {
+      const float w = __fadd_rn(wu[j + 1] / W, 1e-5f);
+      pdf[j] = w;
+      part += (double)w;
+    }
+    const float sum = (float)warp_sum_d(part);
+    for (int j = lane; j < S - 1; j += 32) mid[j] = __fmul_rn(0.5f, __fadd_rn(zr[j + 1], zr[j]));
+    for (int k = lane; k < S; k += 32) zall[k] = zr[k];
+    __syncwarp();
+    // cdf: lane owns the contiguous run [j0, j1) of the pdf; exclusive scan of the run totals
+    const int C = (M + 31) / 32, j0 = min(M, lane * C), j1 = min(M, j0 + C);
+    double run = 0.0;
+    for (int j = j0; j < j1; ++j) {
+      const float q = __fdiv_rn(pdf[j], sum);
+      pdf[j] = q;
+      run += (double)q;
+    }
+    double pre = run;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const double v = __shfl_up_sync(0xffffffffu, pre, o);
+      if (lane >= o) pre += v;
+    }
+    pre -= run;
+    for (int j = j0; j < j1; ++j) {
+      pre += (double)pdf[j];
+      cdf[j + 1] = (float)pre;
+    }
+    if (lane == 0) cdf[0] = 0.f;
+    __syncwarp();
+    const uint64_t seed = p.seed_dev ? *p.seed_dev : p.seed;
+    double zsum = 0.0;
+    for (int j = lane; j < N; j += 32) {
+      float u;
+      if (p.u) {
+        u = p.u[(size_t)r * N + j];
+      } else if (p.det) {
+        u = p.lin_u[j];
+      } else {
+        // counters above 2^63: disjoint from the coarse pass's jitter stream (k_sample)
+        float q[4];
+        philox4(seed, (1ull << 63) | ((uint64_t)r * N + j), q);
+        u = q[0];
+      }
+      // searchsorted(cdf, u, right=True): the first index whose cdf exceeds u, in [0, M + 1]
+      int lo = 0, hi = M + 1;
+      while (lo < hi) {
+        const int m = (lo + hi) >> 1;
+        if (cdf[m] <= u) lo = m + 1; else hi = m;
+      }
+      const int below = max(lo - 1, 0), above = min(lo, M);
+      const float c0 = cdf[below];
+      float den = __fsub_rn(cdf[above], c0);
+      if (den < 1e-5f) den = 1.f;
+      const float t = __fdiv_rn(__fsub_rn(u, c0), den);
+      const float b0 = mid[below];
+      const float z = __fadd_rn(b0, __fmul_rn(t, __fsub_rn(mid[above], b0)));
+      zall[S + j] = z;
+      zsum += (double)z;
+      if (p.z_samples) p.z_samples[(size_t)r * N + j] = z;
+    }
+    __syncwarp();
+    if (p.z_std) {  // std(z_samples, unbiased=False), two passes in float64
+      const double mean = warp_sum_d(zsum) / N;
+      double v = 0.0;
+      for (int j = lane; j < N; j += 32) {
+        const double dz = (double)zall[S + j] - mean;
+        v += dz * dz;
+      }
+      v = warp_sum_d(v);
+      if (lane == 0) p.z_std[r] = (float)sqrt(v / N);
+    }
+    const float d = p.counts ? p.target_d[r] : 0.f;
+    for (int e = lane; e < T; e += 32) {
+      const float v = zall[e];
+      int rank = 0;
+      for (int q = 0; q < T; ++q) {
+        const float w = zall[q];
+        rank += (w < v) || (w == v && q < e);
+      }
+      p.z_fine[(size_t)r * T + rank] = v;
+      if (p.counts) count_sample(v, d, p.trunc, c_fs, c_sdf);
+    }
+    if (p.counts && lane == 0) c_valid = (d > 0.f && d < p.depth_trunc);
+  }
+  if (p.counts) add_counts(p.counts, c_fs, c_sdf, c_valid, lane);
+}
+
 // the corner-pair scatter adds to the table gradient in 16-byte chunks
 static bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
 
@@ -2082,7 +2239,10 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   if (R <= 0) return XRD_OK;
   if (S < 2 || S > 256) return XRD_E_SHAPE;
   const bool has_depth = rays->target_d != nullptr;
-  if (has_depth && S != cfg->n_sample_d + cfg->n_range_d) return XRD_E_SHAPE;
+  // a fine pass (phase 2 on the z_vals of xrd_coslam_importance) marches n_importance more
+  if (cfg->n_importance < 0) return XRD_E_SHAPE;
+  const int n_fine = cfg->phase == 2 ? cfg->n_importance : 0;
+  if (has_depth && S != cfg->n_sample_d + cfg->n_range_d + n_fine) return XRD_E_SHAPE;
   if (has_depth && (!cfg->lin_uniform || !cfg->lin_range || !cfg->lin_nodepth)) return XRD_E_NULL;
   if (!has_depth && !cfg->lin_full) return XRD_E_NULL;
   if (grads && (!has_depth || !rays->target_s || !out->losses)) return XRD_E_NULL;
@@ -2227,6 +2387,28 @@ extern "C" int xrd_coslam_step(const XrdRays* rays, const XrdHashGrid* grid,
   if (st != XRD_OK || !grads) return st;
   FinalizeParams fp{loss_acc, P.counts, out->losses, P.Rg, S, cfg->w_rgb, cfg->w_depth, cfg->w_sdf, cfg->w_fs};
   k_finalize<<<1, 32, 0, stream>>>(fp);
+  XRD_LAUNCH_CHECK();
+  return XRD_OK;
+}
+
+extern "C" int xrd_coslam_importance(const XrdCoslamImportance* q, void* stream_) {
+  if (!q || !q->z_vals || !q->raw || !q->z_fine) return XRD_E_NULL;
+  const int R = q->n_rays, S = q->n_samples, N = q->n_importance;
+  // the fine pass marches S + N samples per ray: at most 256 (xrd_coslam_step)
+  if (R < 0 || S < 3 || N < 1 || S + N > 256) return XRD_E_SHAPE;
+  if (!q->u && q->det && !q->lin_u) return XRD_E_NULL;
+  if (q->counts_out && !q->target_d) return XRD_E_NULL;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (q->counts_out) XRD_CUDA_TRY(cudaMemsetAsync(q->counts_out, 0, 4 * sizeof(int), stream));
+  if (R == 0) return XRD_OK;
+  ImportanceParams p;
+  p.R = R; p.S = S; p.N = N; p.det = q->det;
+  p.trunc = q->trunc; p.depth_trunc = q->depth_trunc;
+  p.z_vals = q->z_vals; p.raw = q->raw; p.target_d = q->target_d; p.u = q->u; p.lin_u = q->lin_u;
+  p.seed = q->seed; p.seed_dev = q->seed_dev;
+  p.z_fine = q->z_fine; p.z_samples = q->z_samples; p.z_std = q->z_std; p.counts = q->counts_out;
+  const size_t smem = sizeof(float) * kImpWarps * (size_t)imp_floats(S, N);  // <= 20 KB
+  k_importance<<<(R + kImpWarps - 1) / kImpWarps, kImpWarps * 32, smem, stream>>>(p);
   XRD_LAUNCH_CHECK();
   return XRD_OK;
 }

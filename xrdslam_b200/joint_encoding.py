@@ -28,8 +28,8 @@ from torch import nn
 from torch.nn import Parameter
 
 from . import _cabi
-from ._cabi import (XrdCoslamCfg, XrdCoslamGrads, XrdCoslamMlp, XrdCoslamOut,
-                    XrdHashGrid, XrdRays, ptr)
+from ._cabi import (XrdCoslamCfg, XrdCoslamGrads, XrdCoslamImportance, XrdCoslamMlp,
+                    XrdCoslamOut, XrdHashGrid, XrdRays, ptr)
 from .base_model import Model, ModelConfig, scale_grads, upstream_scale
 
 
@@ -132,12 +132,21 @@ class ColorSDFNet(nn.Module):
                             1 + config.geo_feat_dim)
 
 
+# render_rays outputs (joint_encoding.py:317-341); the second tuple only with
+# training_n_importance > 0 (the coarse pass's maps and the spread of the fine samples)
+OUT_KEYS = ('rgb', 'depth', 'disp_map', 'acc_map', 'depth_var', 'z_vals', 'raw')
+IMPORTANCE_KEYS = ('rgb0', 'disp0', 'acc0', 'depth0', 'depth_var0', 'z_std')
+# samples per ray the fused kernels march at most (xrd_coslam_step); a gradient pass with a
+# colour grid (oneGrid=False) at most 224
+MAX_SAMPLES, MAX_SAMPLES_COLOR_GRID = 256, 224
+
+
 class _CoslamStep(torch.autograd.Function):
     """losses[4] = fused(rays, table, weights[, colour table]); backward hands out the
     gradients the kernel already produced."""
     @staticmethod
     def forward(ctx, rays_o, rays_d, table, w0, w1, wc0, wc1, model, target_s,
-                target_d, noise, table_c=None):
+                target_d, noise, table_c=None, importance_u=None):
         need = any(ctx.needs_input_grad[:7]) or ctx.needs_input_grad[11]
         need_rays = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         # tracking: only the pose is optimised -> skip scatter / weight-gradient tiles
@@ -146,14 +155,14 @@ class _CoslamStep(torch.autograd.Function):
         outs, grads = model._launch(rays_o, rays_d, table, w0, w1, wc0, wc1,
                                     target_s, target_d, noise, with_grads=need,
                                     need_ray_grads=need_rays,
-                                    map_grads=map_grads, table_c=table_c)
+                                    map_grads=map_grads, table_c=table_c,
+                                    importance_u=importance_u)
         ctx.grads = grads
         ctx.model = model
         ctx.strict = model.config.strict_loss_grad
         ctx.inputs = (rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
-                      target_d, noise, model._last_seed, table_c)
-        ret = (outs['losses'], outs['rgb'], outs['depth'], outs['disp_map'],
-               outs['acc_map'], outs['depth_var'], outs['z_vals'], outs['raw'])
+                      target_d, noise, model._last_seed, table_c, importance_u)
+        ret = (outs['losses'],) + tuple(outs[k] for k in model._out_keys())
         ctx.mark_non_differentiable(*ret[1:])
         return ret
 
@@ -168,11 +177,12 @@ class _CoslamStep(torch.autograd.Function):
                 # non-unit upstream gradient: re-run the fused pass with the
                 # per-term scales (the kernel is linear in them)
                 (rays_o, rays_d, table, w0, w1, wc0, wc1, ts, td, noise,
-                 seed, table_c) = ctx.inputs
+                 seed, table_c, importance_u) = ctx.inputs
                 _, grads = ctx.model._launch(
                     rays_o, rays_d, table, w0, w1, wc0, wc1, ts, td, noise,
                     with_grads=True, need_ray_grads=True,
-                    loss_scale=[float(v) for v in g], seed=seed, table_c=table_c)
+                    loss_scale=[float(v) for v in g], seed=seed, table_c=table_c,
+                    importance_u=importance_u)
         else:
             # sync-free: total-loss scaling is honoured, unequal per-term scales poison
             # the gradients with NaN (base_model.upstream_scale)
@@ -182,7 +192,7 @@ class _CoslamStep(torch.autograd.Function):
             grads = dict(zip(keys, scale_grads([grads[k] for k in keys], s)))
         return (grads['d_rays_o'], grads['d_rays_d'], grads['d_table'],
                 grads['d_w_sdf0'], grads['d_w_sdf1'], grads['d_w_col0'],
-                grads['d_w_col1'], None, None, None, None, grads['d_table_color'])
+                grads['d_w_col1'], None, None, None, None, grads['d_table_color'], None)
 
 
 class JointEncoding(Model):
@@ -199,10 +209,23 @@ class JointEncoding(Model):
     def populate_modules(self):
         super().populate_modules()
         cfg = self.config
-        if cfg.tcnn_network or cfg.training_n_importance:
+        if cfg.tcnn_network:
             raise NotImplementedError(
-                'CUDA path covers tcnn_network=False, n_importance=0 (the reference '
-                'defaults, input_config.py:253-254)')
+                'CUDA path covers tcnn_network=False (the reference default, '
+                'input_config.py:253-254)')
+        N = cfg.training_n_importance
+        if N < 0:
+            raise ValueError(f'training_n_importance must be >= 0, got {N}')
+        if N:
+            # the fine pass of every training step marches the depth-guided samples plus N
+            limit = MAX_SAMPLES if cfg.oneGrid else MAX_SAMPLES_COLOR_GRID
+            S = cfg.training_n_sample_d + cfg.training_n_range_d + N
+            if S > limit:
+                raise ValueError(
+                    f'training_n_importance={N}: the fine pass would march training_n_sample_d + '
+                    f'training_n_range_d + training_n_importance = {S} samples per ray; the '
+                    f'fused kernels take at most {limit}'
+                    + ('' if cfg.oneGrid else ' with a colour grid (oneGrid=False)'))
         if not cfg.tcnn_encoding:
             raise NotImplementedError('tcnn_encoding=True is the co-slam '
                                       'default (input_config.py:254)')
@@ -230,6 +253,10 @@ class JointEncoding(Model):
         self.register_buffer('_lin_full',
                              ls(cfg.cam_near, cfg.cam_far,
                                 cfg.training_n_samples), persistent=False)
+        # sample_pdf's det draw (utils.py:50-54), used when training_perturb == 0
+        N = cfg.training_n_importance
+        self.register_buffer('_lin_u', ls(0. + 0.5 / N, 1. - 0.5 / N, steps=N) if N else None,
+                             persistent=False)
         self._step_count = 0
         # set by the Algorithm around tracking (only pose params have optimizers
         # there, base_algorithm.py:168-181): the fused pass then produces d rays only
@@ -304,9 +331,13 @@ class JointEncoding(Model):
             m.grid_color = C.pointer(self._grid_struct(tc.detach(), self.embed_fn_color))
         return m
 
+    def _out_keys(self):
+        return OUT_KEYS + (IMPORTANCE_KEYS if self.config.training_n_importance else ())
+
     def _cfg_struct(self, S, seed=0, seed_dev=None, phase=0, n_rays_global=0,
-                    counts_global=None, counts_out=None):
-        """XrdCoslamCfg for S samples per ray; seed_dev and the counts are device tensors."""
+                    counts_global=None, counts_out=None, n_importance=0):
+        """XrdCoslamCfg for S samples per ray; seed_dev and the counts are device tensors.
+        n_importance: a fine pass (phase 2) over the z_vals of _importance_struct."""
         cfg = self.config
         return XrdCoslamCfg(
             n_samples=S, n_sample_d=cfg.training_n_sample_d, n_range_d=cfg.training_n_range_d,
@@ -318,15 +349,47 @@ class JointEncoding(Model):
             lin_nodepth=ptr(self._lin_nodepth), lin_full=ptr(self._lin_full),
             seed=seed, rays_per_tile=cfg.rays_per_tile, precision=cfg.precision, phase=phase,
             n_rays_global=n_rays_global, counts_global=ptr(counts_global),
-            counts_out=ptr(counts_out), seed_dev=ptr(seed_dev))
+            counts_out=ptr(counts_out), seed_dev=ptr(seed_dev), n_importance=n_importance)
 
-    def _outputs(self, R, S, dev):
-        """-> (buffers, XrdCoslamOut) of one pass over R rays of S samples."""
+    def _importance_struct(self, R, S, dev, z_vals, raw, target_d=None, u=None, seed=0,
+                           seed_dev=None, counts=None, bufs=None):
+        """-> (buffers z_vals [R,S+N], z_samples [R,N], z_std [R], XrdCoslamImportance) of the
+        hierarchical sampling after a coarse pass of S samples per ray (its z_vals, raw);
+        counts: DEVICE int32 [4] receiving the fine pass's loss-normaliser counts; bufs: the
+        buffers of an earlier call to write again."""
+        cfg = self.config
+        N = cfg.training_n_importance
+        f32 = dict(dtype=torch.float32, device=dev)
+        b = bufs or dict(z_vals=torch.empty(R, S + N, **f32), z_samples=torch.empty(R, N, **f32),
+                         z_std=torch.empty(R, **f32))
+        q = XrdCoslamImportance(
+            n_rays=R, n_samples=S, n_importance=N, det=int(cfg.training_perturb == 0),
+            trunc=cfg.training_trunc * cfg.data_sc_factor, depth_trunc=cfg.cam_depth_trunc,
+            z_vals=ptr(z_vals), raw=ptr(raw), target_d=ptr(target_d), u=ptr(u),
+            lin_u=ptr(self._lin_u), seed=seed, seed_dev=ptr(seed_dev), z_fine=ptr(b['z_vals']),
+            z_samples=ptr(b['z_samples']), z_std=ptr(b['z_std']), counts_out=ptr(counts))
+        return b, q
+
+    def _check_fine_samples(self, S):
+        """Raise ValueError naming the limit when the fine pass after a coarse pass of S samples
+        per ray is longer than the fused kernels take (a render without depth:
+        training_n_samples + N)."""
+        N = self.config.training_n_importance
+        if S + N > MAX_SAMPLES:
+            raise ValueError(
+                f'Co-SLAM importance sampling: the fine pass would march {S + N} samples per ray '
+                f'({S} + training_n_importance = {N}); the fused kernels take at most '
+                f'{MAX_SAMPLES} (a render without a depth target marches training_n_samples in '
+                f'its coarse pass)')
+
+    def _outputs(self, R, S, dev, z_vals=None):
+        """-> (buffers, XrdCoslamOut) of one pass over R rays of S samples (z_vals: a given
+        [R,S] buffer instead of a new one)."""
         f32 = dict(dtype=torch.float32, device=dev)
         o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f32),
                  disp_map=torch.empty(R, **f32), acc_map=torch.empty(R, **f32),
                  depth_var=torch.empty(R, **f32),
-                 z_vals=torch.empty(R, S, **f32),
+                 z_vals=torch.empty(R, S, **f32) if z_vals is None else z_vals,
                  raw=torch.empty(R, S, 4, **f32),
                  losses=torch.zeros(4, **f32))
         out = XrdCoslamOut(rgb=ptr(o['rgb']), depth=ptr(o['depth']), disp=ptr(o['disp_map']),
@@ -341,8 +404,13 @@ class JointEncoding(Model):
 
     def _launch(self, rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
                 target_d, noise, with_grads, need_ray_grads=True,
-                loss_scale=None, seed=None, map_grads=True, table_c=None):
-        """table_c: the colour grid's table (oneGrid=False; default embed_fn_color.params)."""
+                loss_scale=None, seed=None, map_grads=True, table_c=None, importance_u=None):
+        """table_c: the colour grid's table (oneGrid=False; default embed_fn_color.params).
+        With training_n_importance = N > 0 (joint_encoding.py:301-341): the coarse pass, whose
+        rgb and depth terms alone enter the losses and gradients, then xrd_coslam_importance
+        (importance_u [R,N]: its uniforms, else drawn from `seed`), then the fine pass over the
+        merged samples; the table and weight gradients of both passes add up in g, the ray
+        gradients are summed."""
         cfg = self.config
         if not cfg.oneGrid and table_c is None:
             table_c = self.embed_fn_color.params
@@ -363,6 +431,12 @@ class JointEncoding(Model):
         if noise is not None:
             noise = noise.detach().to(**f32).contiguous()
             assert noise.shape == (R, S)
+        N = cfg.training_n_importance
+        if N:
+            self._check_fine_samples(S)  # before any launch
+        if importance_u is not None:
+            importance_u = importance_u.detach().to(**f32).contiguous()
+            assert importance_u.shape == (R, N)
         o, out = self._outputs(R, S, dev)
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), ptr(ts), ptr(td))
         grid = self._grid_struct(table.detach())
@@ -388,15 +462,12 @@ class JointEncoding(Model):
                      d_rays_d=torch.empty(R, 3, **f32) if need_ray_grads else None,
                      d_table_color=z(table_c, **f32) if (map_grads and table_c is not None)
                      else None)
-            sc = loss_scale or [1.0, 1.0, 1.0, 1.0]
-            gs = XrdCoslamGrads(ptr(g['d_table']), ptr(g['d_w_sdf0']),
-                                ptr(g['d_w_sdf1']), ptr(g['d_w_col0']),
-                                ptr(g['d_w_col1']), ptr(g['d_rays_o']),
-                                ptr(g['d_rays_d']), (C.c_float * 4)(*sc),
-                                ptr(g['d_table_color']))
+            sc = list(loss_scale or [1.0, 1.0, 1.0, 1.0])
+            # with importance sampling the coarse pass adds its rgb and depth terms only
+            gs = self._grads_struct(g, sc[:2] + [0.0, 0.0] if N else sc)
         ws, ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
 
-        def step(grads):
+        def step(grads, c=c, out=out, ws=ws, ws_bytes=ws_bytes, noise=noise):
             _cabi.launch_on(dev, 'xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp),
                             C.byref(c), ptr(noise), C.byref(out), grads, ptr(ws), ws_bytes)
         if dp is not None:
@@ -410,7 +481,44 @@ class JointEncoding(Model):
             c.n_rays_global = R * dp.world  # equal shards
         step(C.byref(gs) if gs is not None else None)
         self._last_seed = seed
-        return o, g
+        if not N:
+            return o, g
+        # importance sampling -> the fine pass over S + N samples (phase 2, its own counts)
+        counts = torch.zeros(4, dtype=torch.int32, device=dev) if has_d else None
+        b, q = self._importance_struct(R, S, dev, o['z_vals'], o['raw'], td, importance_u,
+                                       seed=seed, counts=counts)
+        _cabi.launch_on(dev, 'xrd_coslam_importance', C.byref(q))
+        if dp is not None:
+            dp.all_reduce_sum(counts)
+        of, outf = self._outputs(R, S + N, dev, z_vals=b['z_vals'])
+        cf = self._cfg_struct(S + N, seed=seed, phase=2, counts_global=counts, n_importance=N,
+                              n_rays_global=R * dp.world if dp is not None else 0)
+        gsf = None
+        if g is not None:
+            gf = dict(g, d_rays_o=None, d_rays_d=None)
+            if need_ray_grads:
+                gf['d_rays_o'], gf['d_rays_d'] = torch.empty_like(g['d_rays_o']), torch.empty_like(
+                    g['d_rays_d'])
+            gsf = self._grads_struct(gf, sc)
+        wsf, wsf_bytes = _cabi.workspace(dev, 'coslam', R, S + N)
+        step(C.byref(gsf) if gsf is not None else None, c=cf, out=outf, ws=wsf,
+             ws_bytes=wsf_bytes, noise=None)
+        if g is not None:
+            of['losses'][:2] += o['losses'][:2]
+            if need_ray_grads:
+                g['d_rays_o'] += gf['d_rays_o']
+                g['d_rays_d'] += gf['d_rays_d']
+        of.update(rgb0=o['rgb'], disp0=o['disp_map'], acc0=o['acc_map'], depth0=o['depth'],
+                  depth_var0=o['depth_var'], z_std=b['z_std'])
+        return of, g
+
+    @staticmethod
+    def _grads_struct(g, scale):
+        """XrdCoslamGrads of the gradient buffers g with per-term loss scales `scale`."""
+        return XrdCoslamGrads(ptr(g['d_table']), ptr(g['d_w_sdf0']), ptr(g['d_w_sdf1']),
+                              ptr(g['d_w_col0']), ptr(g['d_w_col1']), ptr(g['d_rays_o']),
+                              ptr(g['d_rays_d']), (C.c_float * 4)(*scale),
+                              ptr(g['d_table_color']))
 
     def _launch_smooth(self, table, rand6, need_grad, weight=1.0):
         cfg = self.config
@@ -428,29 +536,32 @@ class JointEncoding(Model):
     # --------------------------------------------------------- Model API ---
     def get_outputs(self, input) -> Dict[str, Union[torch.Tensor, List]]:
         """joint_encoding.py:158-163.  Extra optional key ``noise`` [R,S]
-        replaces torch.rand(z_vals.shape) (:292) for parity runs."""
+        replaces torch.rand(z_vals.shape) (:292) for parity runs, and with
+        training_n_importance = N > 0 ``importance_u`` [R,N] replaces sample_pdf's
+        torch.rand (utils.py:56) / linspace."""
         return self.render_rays(input['rays_o'], input['rays_d'],
                                 target_d=input.get('target_d'),
                                 target_s=input.get('target_s'),
-                                noise=input.get('noise'))
+                                noise=input.get('noise'),
+                                importance_u=input.get('importance_u'))
 
     def render_rays(self, rays_o, rays_d, target_d=None, target_s=None,
-                    noise=None):
+                    noise=None, importance_u=None):
         table = self.embed_fn.params
         w0, w1, wc0, wc1 = self._weights()
         fused = (torch.is_grad_enabled() and target_d is not None
                  and target_s is not None)
         table_c = None if self.config.oneGrid else self.embed_fn_color.params
         if fused:
-            (losses, rgb, depth, disp, acc, var, z_vals,
-             raw) = _CoslamStep.apply(rays_o, rays_d, table, w0, w1, wc0, wc1,
-                                      self, target_s, target_d, noise, table_c)
-            ret = dict(rgb=rgb, depth=depth, disp_map=disp, acc_map=acc,
-                       depth_var=var, z_vals=z_vals, raw=raw)
+            losses, *outs = _CoslamStep.apply(rays_o, rays_d, table, w0, w1, wc0, wc1,
+                                              self, target_s, target_d, noise, table_c,
+                                              importance_u)
+            ret = dict(zip(self._out_keys(), outs))
             ret['_losses'] = losses
             return ret
         o, _ = self._launch(rays_o, rays_d, table, w0, w1, wc0, wc1, target_s,
-                            target_d, noise, with_grads=False, table_c=table_c)
+                            target_d, noise, with_grads=False, table_c=table_c,
+                            importance_u=importance_u)
         o.pop('losses')
         return o
 
