@@ -42,7 +42,11 @@ __global__ void __launch_bounds__(256) k_adam(const Args A) {
   const long long n4 = (vec && (!masked || (T.row_len & 3) == 0)) ? n / 4 : 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
        i += (long long)gridDim.x * blockDim.x) {
-    if (masked && !T.row_mask[(i * 4) / T.row_len]) continue;  // row_len % 4 == 0: one row per float4
+    if (masked && !T.row_mask[(i * 4) / T.row_len]) {  // row_len % 4 == 0: one row per float4
+      // a kept row holds its parameter and moments, but zero_grad still clears its gradient
+      if (A.zero_grad) reinterpret_cast<float4*>(T.grad)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
     float4 p = reinterpret_cast<float4*>(T.param)[i];
     float4 g = reinterpret_cast<float4*>(T.grad)[i];
     float4 m = reinterpret_cast<float4*>(T.exp_avg)[i];
@@ -58,7 +62,10 @@ __global__ void __launch_bounds__(256) k_adam(const Args A) {
   }
   for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x) {
-    if (masked && !T.row_mask[i / T.row_len]) continue;
+    if (masked && !T.row_mask[i / T.row_len]) {
+      if (A.zero_grad) T.grad[i] = 0.f;
+      continue;
+    }
     float p = T.param[i], g = T.grad[i], m = T.exp_avg[i], v = T.exp_avg_sq[i];
     upd(p, g, m, v, T, step_size, inv_sqrt_bc2);
     T.param[i] = p; T.exp_avg[i] = m; T.exp_avg_sq[i] = v;

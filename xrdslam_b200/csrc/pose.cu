@@ -34,7 +34,9 @@ __global__ void k_fwd(int n, const float* rot, const float* trans, float* c2w) {
     float K[9], K2[9];
     skew(k, K);
     mm3(K, K, K2);
-    const float s = sinf(th), c1 = 1.f - cosf(th);
+    // 1 - cos(th) as 2 sin^2(th / 2): 1.f - cosf(th) cancels to 0 for th < ~3e-4, which costs
+    // the backward's (dk - (dk . k) k) / th up to ~1e3 ulp of |G| there
+    const float s = sinf(th), h = sinf(0.5f * th), c1 = 2.f * h * h;
 #pragma unroll
     for (int q = 0; q < 9; ++q) R[q] = (q % 4 == 0 ? 1.f : 0.f) + K[q] * s + c1 * K2[q];
   }
@@ -78,7 +80,7 @@ __global__ void k_bwd(int n, const float* rot, const float* d_c2w, const unsigne
     for (int c = 0; c < 3; ++c) Kt[r * 3 + c] = K[c * 3 + r];
   mm3(G, Kt, GKt);
   mm3(Kt, G, KtG);
-  const float s = sinf(th), co = cosf(th), c1 = 1.f - co;
+  const float s = sinf(th), co = cosf(th), h = sinf(0.5f * th), c1 = 2.f * h * h;  // as in k_fwd
   float dK[9], gK = 0.f, gK2 = 0.f;
 #pragma unroll
   for (int q = 0; q < 9; ++q) {
