@@ -416,13 +416,33 @@ typedef struct {
                            * under data-parallel mapping (far clamp and zero-depth
                            * sampling are batch-global, SURVEY Q9); NULL -> computed
                            * from this call's rays                                  */
+  /* Sampling options of render_batch_ray (all zero: 32 + 16 samples, no jitter).
+   * n_importance > 0 runs two passes (conv_onet.py:498-520): pass 1 renders the S0 samples
+   * forward only, sample_pdf (slam/model_components/utils.py:31-76, called without the
+   * `device` keyword its signature lacks) draws n_importance more from pass 1's weights[1:-1],
+   * and pass 2 -- outputs, loss and gradients -- runs over the sorted merge of
+   * S0 + n_importance <= 128 samples.  XRD_E_SHAPE when n_importance < 0 or the total is
+   * over 128.  Pass 1 keeps the limit S0 <= 64. */
+  int n_importance;       /* rendering_n_importance                                   */
+  float perturb;          /* rendering_perturb: > 0 jitters the uniform samples within
+                           * their intervals (conv_onet.py:470-477); == 0 makes
+                           * sample_pdf deterministic (det = perturb == 0)             */
+  uint64_t seed;          /* Philox seed of the draws below that are not given        */
+  const float* perturb_u; /* DEVICE [R,n_samples] jitter uniforms, or NULL -> Philox(seed)
+                           * (the reference draws torch.rand on the CPU generator)     */
+  const float* importance_u; /* DEVICE [R,n_importance] sample_pdf uniforms, or NULL ->
+                           * t_importance when perturb == 0, else Philox(seed) on
+                           * counters disjoint from the jitter's                       */
+  const float* t_importance; /* DEVICE [n_importance] torch.linspace(0.5/N, 1-0.5/N, N),
+                           * sample_pdf's det draw; read when perturb == 0 and
+                           * importance_u is NULL                                      */
 } XrdNiceCfg;
 
 typedef struct {
   float* rgb;         /* [R,3]                                                     */
   double* depth;      /* [R]   float64 like the reference                          */
   double* uncertainty;/* [R]                                                       */
-  double* z_vals;     /* [R,S] optional                                            */
+  double* z_vals;     /* [R,S] optional; S = all samples of the last pass           */
   float* raw;         /* [R,S,4] optional (rgb, occupancy logit)                   */
   float* losses;      /* [2] depth_loss, rgb_loss (rgb 0 when the stage has none)  */
 } XrdNiceOut;
@@ -435,6 +455,7 @@ typedef struct {
   float* d_rays_d;             /* [R,3] or NULL                                     */
 } XrdNiceGrads;
 
+/* n_samples_total: n_samples + n_surface + n_importance */
 size_t xrd_nice_workspace_bytes(int n_rays, int n_samples_total, int with_grads);
 
 /* decoders[3] = middle, fine, color; grids[3] = middle, fine, color. */
@@ -442,6 +463,16 @@ int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
                   const XrdNiceDecoder decoders[3], const XrdNiceCfg* cfg,
                   XrdNiceOut* out, XrdNiceGrads* grads, void* workspace,
                   size_t workspace_bytes, void* stream);
+
+/* The sample_pdf stage of xrd_nice_step on given inputs (tests): pass 1's weights DEVICE
+ * [R,S0] fp32 and sorted samples [R,S0] fp64 -> the sorted merge z_out [R,S0+N] fp64 and,
+ * unless NULL, the samples in draw order z_samples [R,N] fp64.  u
+ * [R,N], else t_importance [N] when det, else Philox(seed), as in XrdNiceCfg.
+ * S0 <= 64, S0 + N <= 128. */
+int xrd_nice_sample_pdf(int n_rays, int n_samples, int n_importance, const float* weights,
+                        const double* z_vals, const float* u, const float* t_importance,
+                        int det, uint64_t seed, double* z_out, double* z_samples,
+                        void* stream);
 
 /* Mesher queries (slam/models/conv_onet.py:213-240 query_fn = NICE.forward(stage 'fine'),
  * color_func = stage 'color'; slam/common/mesher.py:138-167): raw [P,4] = (rgb or 0, occupancy
@@ -473,8 +504,23 @@ typedef struct {
   double coarse_bound_min[3];  /* scene bound * model_coarse_bound_enlarge                */
   double coarse_bound_max[3];
   const float* t_uniform;      /* DEVICE [n_samples] torch.linspace(0,1,n_samples)        */
+  /* as in XrdNiceCfg, with S0 = n_samples */
+  int n_importance;       /* rendering_n_importance                                   */
+  float perturb;          /* rendering_perturb: > 0 jitters the uniform samples within
+                           * their intervals (conv_onet.py:470-477); == 0 makes
+                           * sample_pdf deterministic (det = perturb == 0)             */
+  uint64_t seed;          /* Philox seed of the draws below that are not given        */
+  const float* perturb_u; /* DEVICE [R,n_samples] jitter uniforms, or NULL -> Philox(seed)
+                           * (the reference draws torch.rand on the CPU generator)     */
+  const float* importance_u; /* DEVICE [R,n_importance] sample_pdf uniforms, or NULL ->
+                           * t_importance when perturb == 0, else Philox(seed) on
+                           * counters disjoint from the jitter's                       */
+  const float* t_importance; /* DEVICE [n_importance] torch.linspace(0.5/N, 1-0.5/N, N),
+                           * sample_pdf's det draw; read when perturb == 0 and
+                           * importance_u is NULL                                      */
 } XrdNiceCoarseCfg;
 
+/* n_samples: n_samples + n_importance */
 size_t xrd_nice_coarse_workspace_bytes(int n_rays, int n_samples, int with_grads);
 /* out->losses[0] = depth loss (losses[1] = 0).  with_grads = 0: forward only. */
 int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid,

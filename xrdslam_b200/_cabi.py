@@ -108,12 +108,19 @@ class XrdNiceGrid(C.Structure):
     _fields_ = [('data', vp), ('nx', C.c_int), ('ny', C.c_int), ('nz', C.c_int)]
 
 
+# trailing sampling fields of XrdNiceCfg and XrdNiceCoarseCfg (rendering_n_importance,
+# rendering_perturb, the Philox seed and the optional uniforms)
+_NICE_SAMPLING = [('n_importance', C.c_int), ('perturb', C.c_float), ('seed', C.c_uint64),
+                  ('perturb_u', vp), ('importance_u', vp), ('t_importance', vp)]
+
+
 class XrdNiceCfg(C.Structure):
     _fields_ = [('stage', C.c_int), ('is_mapping', C.c_int), ('n_samples', C.c_int),
                 ('n_surface', C.c_int), ('bound_min', C.c_double * 3),
                 ('bound_max', C.c_double * 3), ('w_color', C.c_float),
                 ('handle_dynamic', C.c_int), ('use_color_in_tracking', C.c_int),
-                ('t_uniform', vp), ('t_surface', vp), ('max_depth_global', vp)]
+                ('t_uniform', vp), ('t_surface', vp), ('max_depth_global', vp)] + \
+        _NICE_SAMPLING
 
 
 class XrdNiceCoarseDecoder(C.Structure):
@@ -123,7 +130,7 @@ class XrdNiceCoarseDecoder(C.Structure):
 class XrdNiceCoarseCfg(C.Structure):
     _fields_ = [('n_samples', C.c_int), ('bound_min', C.c_double * 3),
                 ('bound_max', C.c_double * 3), ('coarse_bound_min', C.c_double * 3),
-                ('coarse_bound_max', C.c_double * 3), ('t_uniform', vp)]
+                ('coarse_bound_max', C.c_double * 3), ('t_uniform', vp)] + _NICE_SAMPLING
 
 
 class XrdNiceOut(C.Structure):
@@ -420,6 +427,8 @@ SYMBOLS = {
     'xrd_pointslam_knn_build': (C.c_int, [vp, C.c_int, C.c_float, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                           vp]),
     'xrd_nice_query_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'xrd_nice_sample_pdf': (C.c_int, [C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int,
+                                      C.c_uint64, vp, vp, vp]),
     'xrd_nice_query': (C.c_int, [vp, C.c_int, C.POINTER(XrdNiceGrid), C.POINTER(XrdNiceDecoder),
                                  C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, vp, vp,
                                  C.c_size_t, vp]),

@@ -27,6 +27,7 @@ from ._cabi import (XrdNiceCfg, XrdNiceCoarseCfg, XrdNiceCoarseDecoder, XrdNiceD
                     XrdNiceDecoderGrads, XrdNiceGrads, XrdNiceGrid, XrdNiceOut, XrdRays, ptr)
 from .base_model import FusedStep, Model, ModelConfig
 
+MAX_SAMPLES = 128  # samples per ray of the CUDA renderer (pass 2 with importance sampling)
 STAGES = {'middle': 0, 'fine': 1, 'color': 2}  # 'coarse' has its own entry (xrd_nice_coarse_step)
 GRIDS = ('grid_middle', 'grid_fine', 'grid_color')  # indexed by STAGES
 
@@ -53,6 +54,7 @@ class ConvOnetConfig(ModelConfig):
     rendering_n_importance: int = 0
     rendering_lindisp: bool = False
     rendering_perturb: float = 0.0
+    seed: int = 0  # Philox seed of the in-kernel draws when no noise / importance_u is passed
     points_batch_size: int = 500000
     tracking_w_color_loss: float = 0.5
     mapping_w_color_loss: float = 0.2
@@ -150,10 +152,22 @@ class ConvOnet(Model):
     def populate_modules(self):
         super().populate_modules()
         cfg = self.config
-        if cfg.rendering_n_importance or cfg.rendering_perturb or \
-                cfg.rendering_lindisp or not cfg.occupancy:
-            raise NotImplementedError('CUDA path covers the reference nice-slam config: '
-                                      'occupancy, no importance sampling / perturbation')
+        if cfg.rendering_lindisp:
+            # conv_onet.py:462-468: near = 0.01 * gt_depth is 0 on rays without depth, and
+            # 1 / near * (1 - t) at t = 1 is inf * 0 = NaN in their depth, uncertainty and rgb
+            raise NotImplementedError(
+                'rendering_lindisp: the reference samples in disparity from near = 0.01 * depth, '
+                'which is 0 on rays without depth and makes their depth, uncertainty and rgb NaN '
+                '(1 / near * (1 - t) = inf * 0 at t = 1)')
+        if not cfg.occupancy:
+            raise NotImplementedError('occupancy=False: the CUDA path composites occupancies')
+        if cfg.rendering_n_importance < 0:
+            raise ValueError(f'rendering_n_importance = {cfg.rendering_n_importance} < 0')
+        # pass 2 takes every sample; the coarse stage's n_samples + N is never more
+        total = cfg.rendering_n_samples + cfg.rendering_n_surface + cfg.rendering_n_importance
+        if total > MAX_SAMPLES:
+            raise ValueError(f'rendering_n_samples + rendering_n_surface + rendering_n_importance '
+                             f'= {total}: the renderer takes at most {MAX_SAMPLES} samples per ray')
         self.bounding_box = torch.as_tensor(np.asarray(self.bounding_box),
                                             dtype=torch.float64).clone()
         self.decoder = NICE(cfg.model_c_dim, coarse=cfg.coarse)
@@ -166,6 +180,10 @@ class ConvOnet(Model):
                              persistent=False)
         self.register_buffer('_t_surface', torch.linspace(0., 1., steps=cfg.rendering_n_surface),
                              persistent=False)
+        n = max(cfg.rendering_n_importance, 1)  # sample_pdf's det draw (utils.py:50-54)
+        self.register_buffer('_t_importance', torch.linspace(0. + 0.5 / n, 1. - 0.5 / n, steps=n),
+                             persistent=False)
+        self._step_count = 0
 
     def load_bound(self):
         """conv_onet.py:324-337 with its dtype chain (int32 * python float -> float32, Q2)."""
@@ -261,8 +279,39 @@ class ConvOnet(Model):
         return XrdNiceOut(ptr(o['rgb']), ptr(o['depth']), ptr(o['uncertainty']),
                           ptr(getattr(self, '_z_capture', None)), None, ptr(o['losses']))
 
+    def _sampling(self, c, R, S0, noise, importance_u, dev, keep):
+        """Fill the sampling fields of a step struct (rendering_perturb / rendering_n_importance,
+        conv_onet.py:470-506): explicit uniforms `noise` [R, n_samples] and `importance_u`
+        [R, N] when given, else draws from a seed that advances every launch (and differs per
+        rank under data-parallel mapping).  -> samples per ray of the last pass."""
+        cfg = self.config
+        N = cfg.rendering_n_importance
+        c.n_importance, c.perturb = N, float(cfg.rendering_perturb)
+        self._step_count += 1
+        rank = self.dp.rank if self.dp is not None else 0
+        c.seed = ((cfg.seed << 32) + self._step_count + (rank << 24)) & ((1 << 64) - 1)
+        f32 = dict(dtype=torch.float32, device=dev)
+        if noise is not None and cfg.rendering_perturb > 0:
+            noise = noise.detach().to(**f32).contiguous()
+            if tuple(noise.shape) != (R, cfg.rendering_n_samples):
+                raise ValueError(f'noise: shape {tuple(noise.shape)}, expected '
+                                 f'({R}, {cfg.rendering_n_samples})')
+            keep.append(noise)
+            c.perturb_u = ptr(noise)
+        if N > 0:
+            if importance_u is not None:
+                importance_u = importance_u.detach().to(**f32).contiguous()
+                if tuple(importance_u.shape) != (R, N):
+                    raise ValueError(f'importance_u: shape {tuple(importance_u.shape)}, '
+                                     f'expected ({R}, {N})')
+                keep.append(importance_u)
+                c.importance_u = ptr(importance_u)
+            c.t_importance = ptr(self._t_importance)
+        return S0 + max(N, 0)
+
     def _launch(self, stage, is_mapping, rays_o, rays_d, target_s, target_d, with_grads,
-                need_rays=False, need_grid=(False, False, False), need_col=False):
+                need_rays=False, need_grid=(False, False, False), need_col=False, noise=None,
+                importance_u=None):
         cfg = self.config
         dev = self.grids['grid_middle'].device
         _cabi.require_cuda(dev, 'model')
@@ -271,7 +320,6 @@ class ConvOnet(Model):
         rays_o = rays_o.detach().to(**f32).contiguous()
         rays_d = rays_d.detach().to(**f32).contiguous()
         R = rays_o.shape[0]
-        S = cfg.rendering_n_samples + cfg.rendering_n_surface
         td = target_d.detach().to(**f32).reshape(-1).contiguous()
         ts = target_s.detach().to(**f32).contiguous() if target_s is not None else None
         o = dict(rgb=torch.empty(R, 3, **f32), depth=torch.empty(R, **f64),
@@ -293,6 +341,8 @@ class ConvOnet(Model):
         if self.dp is not None and self.dp.world > 1 and is_mapping and with_grads:
             maxd = self.dp.all_reduce_max(td.max().reshape(1))  # batch-global (Q9), no host sync
         c.max_depth_global = ptr(maxd)
+        S = self._sampling(c, R, cfg.rendering_n_samples + cfg.rendering_n_surface, noise,
+                           importance_u, dev, keep)
         out = self._out_struct(o)
         g = None
         gs = None
@@ -321,7 +371,7 @@ class ConvOnet(Model):
         return o, g
 
     def _launch_coarse(self, rays_o, rays_d, target_d, with_grads, need_rays=False,
-                       need_grid=False):
+                       need_grid=False, noise=None, importance_u=None):
         """Stage 'coarse' through xrd_nice_coarse_step (csrc/nice.cu)."""
         cfg = self.config
         if not cfg.coarse:
@@ -356,6 +406,7 @@ class ConvOnet(Model):
             c.coarse_bound_min[k] = float(self.bounding_box[k, 0] * e)
             c.coarse_bound_max[k] = float(self.bounding_box[k, 1] * e)
         c.t_uniform = ptr(self._t_uniform)
+        S = self._sampling(c, R, S, noise, importance_u, dev, keep)
         out = self._out_struct(o)
         gr = None
         if with_grads:
@@ -377,12 +428,15 @@ class ConvOnet(Model):
         stage = input['stage']
         rays_o, rays_d = input['rays_o'], input['rays_d']
         target_d, target_s = input['target_d'], input.get('target_s')
+        # explicit uniforms of the jitter [R, n_samples] and of sample_pdf [R, N] (parity tests)
+        smp = dict(noise=input.get('noise'), importance_u=input.get('importance_u'))
         fused = torch.is_grad_enabled() and target_s is not None and 'is_mapping' in input
         if not fused:
             # conv_onet.py:137-138: the coarse level renders without depth guidance; the
             # target depth only enters the (mapping) loss
-            o, _ = self._launch_coarse(rays_o, rays_d, target_d, False) if stage == 'coarse' \
-                else self._launch(stage, True, rays_o, rays_d, target_s, target_d, False)
+            o, _ = self._launch_coarse(rays_o, rays_d, target_d, False, **smp) \
+                if stage == 'coarse' else \
+                self._launch(stage, True, rays_o, rays_d, target_s, target_d, False, **smp)
             o.pop('losses')
             return o
         if stage == 'coarse':
@@ -391,7 +445,7 @@ class ConvOnet(Model):
             def launch(needs):
                 need_rays, need_grid = needs[0] or needs[1], needs[2]
                 o, g = self._launch_coarse(rays_o, rays_d, target_d, need_rays or need_grid,
-                                           need_rays, need_grid)
+                                           need_rays, need_grid, **smp)
                 grads = None if g is None else [g['d_rays_o'], g['d_rays_d'], g['d_grid']]
                 return o['losses'], (o['rgb'], o['depth'], o['uncertainty']), grads
         else:
@@ -405,7 +459,7 @@ class ConvOnet(Model):
                 need_rays, need_grid, need_col = needs[0] or needs[1], needs[2:5], any(needs[5:])
                 o, g = self._launch(stage, is_mapping, rays_o, rays_d, target_s, target_d,
                                     need_rays or any(need_grid) or need_col, need_rays,
-                                    need_grid, need_col)
+                                    need_grid, need_col, **smp)
                 grads = None if g is None else \
                     [g['d_rays_o'], g['d_rays_d'], *g['d_grid'], *g['d_color']]
                 return o['losses'], (o['rgb'], o['depth'], o['uncertainty']), grads

@@ -9,14 +9,19 @@
 // Pipeline of one xrd_nice_step (all on the caller's stream):
 //   k_maxdepth      batch-global max(target_d) (far clamp / zero-depth sampling, Q9)
 //   k_sample        warp per ray: far from the bound (f64), 32 uniform + 16 surface samples
-//                   in f64, rank sort (== torch.sort values)
+//                   in f64, the uniform ones jittered when rendering_perturb > 0, rank sort
+//                   (== torch.sort values)
+//   [n_importance > 0: pass 1 = k_decoder_fwd and k_composite (weights only) over those
+//    samples, then k_sample_pdf: sample_pdf on pass 1's weights and the sorted merge; the
+//    pipeline below is pass 2, over the merged samples]
 //   k_decoder_fwd   x3 (middle [, fine [, color]]): thread per point, 8-lane cooperative
 //                   trilerp on the channel-last grid (one voxel = one 128 B line), decoder
 //                   weights transposed in shared memory, Fourier embedding + grid feature in
 //                   a per-thread shared-memory column, hidden state in registers; relu masks
 //                   (and, for the trainable colour decoder, layer inputs) go to an HBM
 //                   workspace in [feature][point] order
-//   k_composite_fwd warp per ray: occupancy compositing (f32 weights, f64 depth)
+//   k_composite_fwd warp per ray: occupancy compositing (f32 weights, f64 depth), S <= 64 in
+//                   two slots per lane, S <= 128 in four
 //   k_loss          per-ray loss coefficients; tracking: batch median of |d-D|/sqrt(var)
 //   k_composite_bwd d loss / d occupancy logit, d loss / d rgb per sample
 //   k_decoder_bwd   x3: transposed chain with the stored masks, grid scatter
@@ -94,8 +99,12 @@ struct SampleParams {
   const float *t_uniform, *t_surface;  // torch.linspace(0,1,n) tables
   const float* maxd;   // device scalar
   double* z;           // [R][ns+nsurf]
+  // PERTURB (rendering_perturb > 0): uniforms of the jitter, [R][ns] or NULL -> Philox(seed)
+  const float* noise;
+  uint64_t seed;
 };
 
+template <bool PERTURB>
 static __global__ void __launch_bounds__(128) k_sample(SampleParams p) {
   __shared__ double zs[4][64];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -136,6 +145,33 @@ static __global__ void __launch_bounds__(128) k_sample(SampleParams p) {
     z[k] = v;
   }
   __syncwarp();
+  if (PERTURB) {
+    // conv_onet.py:470-477: mids = .5 (z[1:] + z[:-1]), upper = [mids, z[-1]], lower = [z[0],
+    // mids], z = lower + (upper - lower) u over the ns uniform samples only, all in f64 with u
+    // promoted from f32; each product and sum rounded on its own (no fma contraction)
+    double zj[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int k = lane + 32 * i;
+      if (k >= p.ns) break;
+      const double lo = k == 0 ? z[0] : __dmul_rn(0.5, __dadd_rn(z[k], z[k - 1]));
+      const double hi = k == p.ns - 1 ? z[k] : __dmul_rn(0.5, __dadd_rn(z[k + 1], z[k]));
+      float u;
+      if (p.noise) {
+        u = p.noise[(size_t)r * p.ns + k];
+      } else {
+        float q[4];
+        philox4(p.seed, (uint64_t)r * p.ns + k, q);
+        u = q[0];
+      }
+      zj[i] = __dadd_rn(lo, __dmul_rn(__dsub_rn(hi, lo), (double)u));
+    }
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      if (lane + 32 * i < p.ns) z[lane + 32 * i] = zj[i];
+    __syncwarp();
+  }
   // rank sort (values equal torch.sort's)
   for (int k = lane; k < S; k += 32) {
     const double v = z[k];
@@ -659,6 +695,7 @@ struct CompParams {
   const float* gc;   // [R][3]
   float* d_occ;      // [P]
   float* d_rgb[3];   // [P]
+  float* o_w;        // [R][S] k_composite<false, .., true>: the weights alone
 };
 
 __device__ __forceinline__ bool in_bound(const CompParams& P, int r, double z) {
@@ -671,18 +708,20 @@ __device__ __forceinline__ bool in_bound(const CompParams& P, int r, double z) {
   return ok;
 }
 
-// warp per ray, S <= 64: lane handles samples lane and lane + 32
-template <bool BWD>
+// warp per ray, S <= 32 NS: lane handles samples lane + 32 s, s < NS (NS = 2: S <= 64, NS = 4:
+// S <= 128).  WEIGHTS (forward only): pass 1 of importance sampling, which needs the weights
+// [R][S] alone and writes nothing else.
+template <bool BWD, int NS, bool WEIGHTS>
 static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r = blockIdx.x * 4 + warp;
   if (r >= P.R) return;
   const int S = P.S;
-  float alpha[2], col[2][3], w[2], Tt[2];
-  double z[2];
-  bool inb[2], have[2];
+  float alpha[NS], col[NS][3], w[NS], Tt[NS];
+  double z[NS];
+  bool inb[NS], have[NS];
 #pragma unroll
-  for (int s = 0; s < 2; ++s) {
+  for (int s = 0; s < NS; ++s) {
     const int k = lane + 32 * s;
     have[s] = k < S;
     alpha[s] = 0.f; z[s] = 0.0; inb[s] = false;
@@ -696,7 +735,7 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
       alpha[s] = sigmoidf_acc(10.f * occ);
 #pragma unroll
       for (int c = 0; c < 3; ++c) col[s][c] = P.rgb[c] ? P.rgb[c][p] : 0.f;
-      if (!BWD && P.o_raw) {
+      if (!BWD && !WEIGHTS && P.o_raw) {
         float4 rw = make_float4(col[s][0], col[s][1], col[s][2], occ);
         *reinterpret_cast<float4*>(P.o_raw + p * 4) = rw;
       }
@@ -705,7 +744,7 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
   // exclusive product of (1 - alpha + 1e-10) in sample order (torch.cumprod, f32)
   float run = 1.f;
 #pragma unroll
-  for (int s = 0; s < 2; ++s) {
+  for (int s = 0; s < NS; ++s) {
     const float f = have[s] ? (1.f - alpha[s] + 1e-10f) : 1.f;
     float inc = f;
 #pragma unroll
@@ -719,10 +758,16 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
     run *= __shfl_sync(0xffffffffu, inc, 31);
     w[s] = alpha[s] * Tt[s];
   }
+  if (WEIGHTS) {
+#pragma unroll
+    for (int s = 0; s < NS; ++s)
+      if (have[s]) P.o_w[(size_t)r * S + lane + 32 * s] = w[s];
+    return;
+  }
   double depth = 0.0;
   float cr[3] = {0.f, 0.f, 0.f};
 #pragma unroll
-  for (int s = 0; s < 2; ++s)
+  for (int s = 0; s < NS; ++s)
     if (have[s]) {
       depth += (double)w[s] * z[s];
 #pragma unroll
@@ -737,7 +782,7 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
   if (!BWD) {
     double var = 0.0;
 #pragma unroll
-    for (int s = 0; s < 2; ++s)
+    for (int s = 0; s < NS; ++s)
       if (have[s]) { const double t = z[s] - depth; var += (double)w[s] * t * t; }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) var += __shfl_xor_sync(0xffffffffu, var, o);
@@ -750,19 +795,25 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
   // backward: q_k = gd z_k + <gc, c_k>;  dL/dalpha_k = q_k T_k - (sum_{j>k} q_j w_j)/(1-alpha_k+eps)
   const float gd = P.gd[r];
   const float gcx = P.gc[r * 3], gcy = P.gc[r * 3 + 1], gcz = P.gc[r * 3 + 2];
-  float qw[2], q[2];
+  float qw[NS], q[NS];
 #pragma unroll
-  for (int s = 0; s < 2; ++s) {
+  for (int s = 0; s < NS; ++s) {
     q[s] = have[s] ? (float)((double)gd * z[s]) + gcx * col[s][0] + gcy * col[s][1] + gcz * col[s][2] : 0.f;
     qw[s] = q[s] * w[s];
   }
-  // suffix sums (exclusive) over the 64 slots
-  float suf[2];
-  float tot1 = qw[1];
+  // suffix sums (exclusive) over the 32 NS slots: above[s] = the totals of the slots above s
+  float above[NS];
+  above[NS - 1] = 0.f;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) tot1 += __shfl_xor_sync(0xffffffffu, tot1, o);
+  for (int s = NS - 2; s >= 0; --s) {
+    float tot = qw[s + 1];
 #pragma unroll
-  for (int s = 0; s < 2; ++s) {
+    for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
+    above[s] = s == NS - 2 ? tot : tot + above[s + 1];
+  }
+  float suf[NS];
+#pragma unroll
+  for (int s = 0; s < NS; ++s) {
     float inc = qw[s];
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
@@ -771,10 +822,10 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
     }
     float exc = __shfl_down_sync(0xffffffffu, inc, 1);
     if (lane == 31) exc = 0.f;
-    suf[s] = exc + (s == 0 ? tot1 : 0.f);
+    suf[s] = exc + above[s];
   }
 #pragma unroll
-  for (int s = 0; s < 2; ++s)
+  for (int s = 0; s < NS; ++s)
     if (have[s]) {
       const size_t p = (size_t)r * S + lane + 32 * s;
       const float da = q[s] * Tt[s] - suf[s] / (1.f - alpha[s] + 1e-10f);
@@ -783,6 +834,128 @@ static __global__ void __launch_bounds__(128) k_composite(const CompParams P) {
         P.d_rgb[0][p] = gcx * w[s]; P.d_rgb[1][p] = gcy * w[s]; P.d_rgb[2][p] = gcz * w[s];
       }
     }
+}
+
+// the instantiation for S samples per ray (two or four slots per lane)
+template <bool BWD>
+static cudaError_t launch_composite(const CompParams& C, cudaStream_t stream) {
+  if (C.S <= 64) k_composite<BWD, 2, false><<<(C.R + 3) / 4, 128, 0, stream>>>(C);
+  else k_composite<BWD, 4, false><<<(C.R + 3) / 4, 128, 0, stream>>>(C);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------- sample_pdf ---
+// Importance samples of pass 2 (conv_onet.py:498-506 with sample_pdf,
+// slam/model_components/utils.py:31-76), one warp per ray:
+//   pdf = (w[1:-1] + 1e-5) / sum, w = pass 1's composite weights (k_composite<.., WEIGHTS>)
+//   cdf = [0, cumsum(pdf)]: the prefix sums in float64 and each rounded to float, as
+//         torch.cumsum does on float32
+//   bins = .5 (z[1:] + z[:-1]) in float64; searchsorted(cdf, u, right=True), the below / above
+//         clamps, denom < 1e-5 -> 1, z = bins[below] + t (bins[above] - bins[below]) in float64
+//   z_out = sort(z ++ samples), each value written at its rank.
+// The cdf and the inversion are the arithmetic of Co-SLAM's k_importance (coslam.cu) with
+// float64 bins.  That kernel keeps its own copy: moving its code into shared device functions
+// changed its SASS (the instruction schedule, same length) under CUDA 12.9.
+struct PdfParams {
+  int R, S, N;        // S: pass 1's samples per ray, N: importance samples per ray
+  const float* w;     // [R][S] pass 1's weights
+  const double* z;    // [R][S] pass 1's sorted samples
+  const float* u;     // [R][N] uniforms, or NULL
+  const float* lin_u; // [N] the det linspace (u NULL, det)
+  int det;
+  uint64_t seed;      // u NULL, !det: Philox at counters 2^63 + r N + j
+  double* z_out;      // [R][S + N]
+  double* z_samples;  // [R][N] the samples in draw order, or NULL
+};
+constexpr int kPdfS = 64, kPdfT = 128;  // limits of pass 1 and of the merge
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+static __global__ void __launch_bounds__(128) k_sample_pdf(const PdfParams p) {
+  __shared__ float s_pdf[4][kPdfS], s_cdf[4][kPdfS];
+  __shared__ double s_bins[4][kPdfS], s_z[4][kPdfT];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r = blockIdx.x * 4 + warp;
+  if (r >= p.R) return;  // warp-uniform
+  const int S = p.S, N = p.N, T = S + N, M = S - 2;  // M inner weights; bins and cdf: M + 1
+  float* pdf = s_pdf[warp];
+  float* cdf = s_cdf[warp];
+  double* bins = s_bins[warp];
+  double* zall = s_z[warp];
+  const float* wr = p.w + (size_t)r * S;
+  const double* zr = p.z + (size_t)r * S;
+  double part = 0.0;
+  for (int j = lane; j < M; j += 32) {
+    const float w = __fadd_rn(wr[j + 1], 1e-5f);
+    pdf[j] = w;
+    part += (double)w;
+  }
+  const float sum = (float)warp_sum_d(part);
+  for (int j = lane; j < S - 1; j += 32) bins[j] = __dmul_rn(0.5, __dadd_rn(zr[j + 1], zr[j]));
+  for (int k = lane; k < S; k += 32) zall[k] = zr[k];
+  __syncwarp();
+  // cdf: lane owns the contiguous run [j0, j1) of the pdf; exclusive scan of the run totals
+  const int C = (M + 31) / 32, j0 = min(M, lane * C), j1 = min(M, j0 + C);
+  double run = 0.0;
+  for (int j = j0; j < j1; ++j) {
+    const float q = __fdiv_rn(pdf[j], sum);
+    pdf[j] = q;
+    run += (double)q;
+  }
+  double pre = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double v = __shfl_up_sync(0xffffffffu, pre, o);
+    if (lane >= o) pre += v;
+  }
+  pre -= run;
+  for (int j = j0; j < j1; ++j) {
+    pre += (double)pdf[j];
+    cdf[j + 1] = (float)pre;
+  }
+  if (lane == 0) cdf[0] = 0.f;
+  __syncwarp();
+  for (int j = lane; j < N; j += 32) {
+    float u;
+    if (p.u) {
+      u = p.u[(size_t)r * N + j];
+    } else if (p.det) {
+      u = p.lin_u[j];
+    } else {
+      // counters above 2^63: disjoint from the jitter's stream (k_sample)
+      float q[4];
+      philox4(p.seed, (1ull << 63) | ((uint64_t)r * N + j), q);
+      u = q[0];
+    }
+    // searchsorted(cdf, u, right=True): the first index whose cdf exceeds u, in [0, M + 1]
+    int lo = 0, hi = M + 1;
+    while (lo < hi) {
+      const int m = (lo + hi) >> 1;
+      if (cdf[m] <= u) lo = m + 1; else hi = m;
+    }
+    const int below = max(lo - 1, 0), above = min(lo, M);
+    const float c0 = cdf[below];
+    float den = __fsub_rn(cdf[above], c0);
+    if (den < 1e-5f) den = 1.f;
+    const float t = __fdiv_rn(__fsub_rn(u, c0), den);
+    const double b0 = bins[below];
+    zall[S + j] = __dadd_rn(b0, __dmul_rn((double)t, __dsub_rn(bins[above], b0)));
+    if (p.z_samples) p.z_samples[(size_t)r * N + j] = zall[S + j];
+  }
+  __syncwarp();
+  for (int e = lane; e < T; e += 32) {
+    const double v = zall[e];
+    int rank = 0;
+    for (int q = 0; q < T; ++q) {
+      const double x = zall[q];
+      rank += (x < v) || (x == v && q < e);
+    }
+    p.z_out[(size_t)r * T + rank] = v;
+  }
 }
 
 // ------------------------------------------------------------------ loss ---
@@ -926,7 +1099,54 @@ struct Ws : Carver {
   float *gd = g ? take<float>(R) : nullptr, *gc = g ? take<float>(R * 3) : nullptr;
   double* tmp = g ? take<double>(R) : nullptr;
   float* acts = g ? take<float>((size_t)n_rows(32) * align_up(P, 64)) : nullptr;
+  // importance sampling, pass 1 (S0 < S samples per ray): its sorted samples z1 [R*S0] f64
+  // and weights w1 [R*S0] f32 live in the rgb rows [3P] f32, which pass 1 does not decode into
+  // and pass 2 writes only after k_sample_pdf has read them (2 R S0 + R S0 floats <= 3P)
+  double* z1 = reinterpret_cast<double*>(rgb);
+  float* w1 = rgb + 2 * P;
 };
+
+// rendering_perturb / rendering_n_importance of one call (the trailing fields of XrdNiceCfg and
+// XrdNiceCoarseCfg); -> XRD_OK or the status to return
+struct Sampling {
+  int S0, N, S;  // pass 1, importance, total samples per ray
+  bool perturb;
+  int check() const {
+    if (N < 0 || S0 > kPdfS || S > kPdfT) return XRD_E_SHAPE;
+    return XRD_OK;
+  }
+};
+
+template <class Cfg>
+static Sampling sampling(const Cfg* cfg, int S0) {
+  Sampling m;
+  m.S0 = S0; m.N = cfg->n_importance; m.S = S0 + (m.N > 0 ? m.N : 0);
+  m.perturb = cfg->perturb > 0.f;
+  return m;
+}
+
+static cudaError_t launch_sample(const SampleParams& sp, bool perturb, cudaStream_t stream) {
+  if (perturb) k_sample<true><<<(sp.R + 3) / 4, 128, 0, stream>>>(sp);
+  else k_sample<false><<<(sp.R + 3) / 4, 128, 0, stream>>>(sp);
+  return cudaGetLastError();
+}
+
+// pass 1's weights (k_composite over the S0 samples at z1, occupancies already decoded) and
+// sample_pdf -> the merged samples z [R][S0 + N]
+template <class Cfg>
+static cudaError_t importance(CompParams C, const Cfg* cfg, const Sampling& m, const Ws& L,
+                              double* z, cudaStream_t stream) {
+  C.z = L.z1; C.S = m.S0; C.o_w = L.w1;
+  k_composite<false, 2, true><<<(C.R + 3) / 4, 128, 0, stream>>>(C);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  PdfParams q;
+  q.R = C.R; q.S = m.S0; q.N = m.N; q.w = L.w1; q.z = L.z1;
+  q.u = cfg->importance_u; q.lin_u = cfg->t_importance; q.det = cfg->perturb == 0.f;
+  q.seed = cfg->seed; q.z_out = z; q.z_samples = nullptr;
+  k_sample_pdf<<<(C.R + 3) / 4, 128, 0, stream>>>(q);
+  return cudaGetLastError();
+}
 }  // namespace
 
 extern "C" size_t xrd_nice_workspace_bytes(int n_rays, int n_samples_total, int with_grads) {
@@ -940,9 +1160,12 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   if (!rays || !grids || !decoders || !cfg || !out || !workspace) return XRD_E_NULL;
   if (!rays->rays_o || !rays->rays_d || !rays->target_d) return XRD_E_NULL;
   if (!out->rgb || !out->depth || !out->uncertainty) return XRD_E_NULL;
-  const int R = rays->n_rays, S = cfg->n_samples + cfg->n_surface;
+  const Sampling m = sampling(cfg, cfg->n_samples + cfg->n_surface);
+  const int R = rays->n_rays, S = m.S;
   if (R <= 0) return XRD_OK;
-  if (S < 2 || S > 64 || cfg->n_samples < 2 || cfg->n_surface < 2) return XRD_E_SHAPE;
+  if (m.S0 < 2 || m.S0 > 64 || cfg->n_samples < 2 || cfg->n_surface < 2) return XRD_E_SHAPE;
+  if (int st = m.check()) return st;
+  if (m.N > 0 && !cfg->importance_u && !m.perturb && !cfg->t_importance) return XRD_E_NULL;
   if (cfg->stage < XRD_NICE_MIDDLE || cfg->stage > XRD_NICE_COLOR) return XRD_E_SHAPE;
   if (!cfg->t_uniform || !cfg->t_surface) return XRD_E_NULL;
   if (decoders[0].c_dim != 32 || decoders[1].c_dim != 64 || decoders[2].c_dim != 32) return XRD_E_SHAPE;
@@ -969,8 +1192,9 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   for (int d = 0; d < 3; ++d) { sp.bmin[d] = cfg->bound_min[d]; sp.bmax[d] = cfg->bound_max[d]; }
   sp.maxd = cfg->max_depth_global ? cfg->max_depth_global : L.maxd; sp.z = z;
   sp.t_uniform = cfg->t_uniform; sp.t_surface = cfg->t_surface;
-  k_sample<<<(R + 3) / 4, 128, 0, stream>>>(sp);
-  XRD_LAUNCH_CHECK();
+  sp.noise = cfg->perturb_u; sp.seed = cfg->seed;
+  if (m.N > 0) sp.z = L.z1;
+  XRD_CUDA_TRY(launch_sample(sp, m.perturb, stream));
 
   const bool train_color = grads && grads->d_color && stage == XRD_NICE_COLOR;
   auto dec_params = [&](int d) {
@@ -987,6 +1211,33 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
     return D;
   };
 
+  CompParams C;
+  C.R = R; C.S = S; C.z = z; C.rays_o = rays->rays_o; C.rays_d = rays->rays_d;
+  C.target_s = rays->target_s; C.target_d = rays->target_d;
+  for (int d = 0; d < 3; ++d) { C.bmin[d] = cfg->bound_min[d]; C.bmax[d] = cfg->bound_max[d]; }
+  C.occ_a = occ_mid; C.occ_b = stage >= XRD_NICE_FINE ? occ_fine : nullptr;
+  for (int c = 0; c < 3; ++c) C.rgb[c] = stage == XRD_NICE_COLOR ? rgb + (size_t)c * P : nullptr;
+  C.o_rgb = out->rgb; C.o_depth = out->depth; C.o_var = out->uncertainty; C.o_raw = out->raw;
+  C.gd = nullptr; C.gc = nullptr; C.d_occ = nullptr; C.d_rgb[0] = C.d_rgb[1] = C.d_rgb[2] = nullptr;
+  C.o_w = nullptr;
+
+  if (m.N > 0) {
+    // pass 1 (conv_onet.py:483-496): decoders and weights over the S0 samples at z1, no loss,
+    // no backward; its outputs are dropped
+    const int P1 = R * m.S0;
+    for (int d = 0; d <= (stage < XRD_NICE_FINE ? stage : XRD_NICE_FINE); ++d) {
+      DecParams D = dec_params(d);
+      D.P = P1; D.S = m.S0; D.z = L.z1; D.masks = nullptr; D.acts = nullptr; D.need_dp = 0;
+      if (d == 0) D.out[0] = occ_mid;
+      if (d == 1) D.out[0] = occ_fine;
+      XRD_CUDA_TRY(launch_decoder(D, false, stream));
+    }
+    CompParams C1 = C;
+    for (int c = 0; c < 3; ++c) C1.rgb[c] = nullptr;  // the weights need occupancies only: no
+                                                      // colour decoder in pass 1
+    XRD_CUDA_TRY(importance(C1, cfg, m, L, z, stream));
+  }
+
   for (int d = 0; d <= stage; ++d) {
     DecParams D = dec_params(d);
     if (d == 0) D.out[0] = occ_mid;
@@ -996,16 +1247,7 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
     XRD_CUDA_TRY(launch_decoder(D, false, stream));
   }
 
-  CompParams C;
-  C.R = R; C.S = S; C.z = z; C.rays_o = rays->rays_o; C.rays_d = rays->rays_d;
-  C.target_s = rays->target_s; C.target_d = rays->target_d;
-  for (int d = 0; d < 3; ++d) { C.bmin[d] = cfg->bound_min[d]; C.bmax[d] = cfg->bound_max[d]; }
-  C.occ_a = occ_mid; C.occ_b = stage >= XRD_NICE_FINE ? occ_fine : nullptr;
-  for (int c = 0; c < 3; ++c) C.rgb[c] = stage == XRD_NICE_COLOR ? rgb + (size_t)c * P : nullptr;
-  C.o_rgb = out->rgb; C.o_depth = out->depth; C.o_var = out->uncertainty; C.o_raw = out->raw;
-  C.gd = nullptr; C.gc = nullptr; C.d_occ = nullptr; C.d_rgb[0] = C.d_rgb[1] = C.d_rgb[2] = nullptr;
-  k_composite<false><<<(R + 3) / 4, 128, 0, stream>>>(C);
-  XRD_LAUNCH_CHECK();
+  XRD_CUDA_TRY(launch_composite<false>(C, stream));
   if (!grads) return XRD_OK;
 
   LossParams LP;
@@ -1022,8 +1264,7 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
   C.d_occ = L.d_occ;
   if (stage == XRD_NICE_COLOR)
     for (int c = 0; c < 3; ++c) C.d_rgb[c] = L.d_rgb + (size_t)c * P;
-  k_composite<true><<<(R + 3) / 4, 128, 0, stream>>>(C);
-  XRD_LAUNCH_CHECK();
+  XRD_CUDA_TRY(launch_composite<true>(C, stream));
 
   XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   for (int d = 0; d <= stage; ++d) {
@@ -1070,6 +1311,23 @@ extern "C" int xrd_nice_step(const XrdRays* rays, const XrdNiceGrid grids[3],
                                                  grads->d_rays_d);
     XRD_LAUNCH_CHECK();
   }
+  return XRD_OK;
+}
+
+extern "C" int xrd_nice_sample_pdf(int n_rays, int n_samples, int n_importance,
+                                   const float* weights, const double* z_vals, const float* u,
+                                   const float* t_importance, int det, uint64_t seed,
+                                   double* z_out, double* z_samples, void* stream_) {
+  if (!weights || !z_vals || !z_out) return XRD_E_NULL;
+  if (n_rays <= 0 || n_importance <= 0) return XRD_OK;
+  if (n_samples < 2 || n_samples > kPdfS || n_samples + n_importance > kPdfT) return XRD_E_SHAPE;
+  if (!u && det && !t_importance) return XRD_E_NULL;
+  PdfParams q;
+  q.R = n_rays; q.S = n_samples; q.N = n_importance; q.w = weights; q.z = z_vals;
+  q.u = u; q.lin_u = t_importance; q.det = det; q.seed = seed; q.z_out = z_out;
+  q.z_samples = z_samples;
+  k_sample_pdf<<<(n_rays + 3) / 4, 128, 0, (cudaStream_t)stream_>>>(q);
+  XRD_LAUNCH_CHECK();
   return XRD_OK;
 }
 
@@ -1144,9 +1402,12 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   if (!rays->rays_o || !rays->rays_d || !grid->data || !cfg->t_uniform) return XRD_E_NULL;
   if (!out->rgb || !out->depth || !out->uncertainty) return XRD_E_NULL;
   if (with_grads && (!rays->target_d || !out->losses)) return XRD_E_NULL;
-  const int R = rays->n_rays, S = cfg->n_samples;
+  const Sampling m = sampling(cfg, cfg->n_samples);
+  const int R = rays->n_rays, S = m.S;
   if (R <= 0) return XRD_OK;
-  if (S < 2 || S > 64) return XRD_E_SHAPE;
+  if (m.S0 < 2 || m.S0 > 64) return XRD_E_SHAPE;
+  if (int st = m.check()) return st;
+  if (m.N > 0 && !cfg->importance_u && !m.perturb && !cfg->t_importance) return XRD_E_NULL;
   const Ws L(workspace, R, S, with_grads);
   if (int st = L.check(workspace_bytes)) return st;
   cudaStream_t stream = (cudaStream_t)stream_;
@@ -1155,12 +1416,12 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   float* occ = L.occ_mid;
 
   SampleParams sp;
-  sp.R = R; sp.ns = S; sp.nsurf = 0; sp.no_depth = 1;
+  sp.R = R; sp.ns = m.S0; sp.nsurf = 0; sp.no_depth = 1;
   sp.rays_o = rays->rays_o; sp.rays_d = rays->rays_d; sp.target_d = nullptr;
   for (int d = 0; d < 3; ++d) { sp.bmin[d] = cfg->bound_min[d]; sp.bmax[d] = cfg->bound_max[d]; }
-  sp.maxd = nullptr; sp.z = z; sp.t_uniform = cfg->t_uniform; sp.t_surface = nullptr;
-  k_sample<<<(R + 3) / 4, 128, 0, stream>>>(sp);
-  XRD_LAUNCH_CHECK();
+  sp.maxd = nullptr; sp.z = m.N > 0 ? L.z1 : z; sp.t_uniform = cfg->t_uniform; sp.t_surface = nullptr;
+  sp.noise = cfg->perturb_u; sp.seed = cfg->seed;
+  XRD_CUDA_TRY(launch_sample(sp, m.perturb, stream));
 
   DecParams D;
   D.P = P; D.S = S; D.z = z; D.rays_o = rays->rays_o; D.rays_d = rays->rays_d;
@@ -1178,12 +1439,6 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   const int sms = num_sms();
   const int gridx = n_tiles < sms ? n_tiles : sms;
   XRD_CUDA_TRY(cudaFuncSetAttribute(k_coarse<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  {
-    KernelTimer kt(stream);
-    k_coarse<false><<<gridx, T, smem, stream>>>(D, W);
-  }
-  XRD_LAUNCH_CHECK();
-
   CompParams C;
   C.R = R; C.S = S; C.z = z; C.rays_o = rays->rays_o; C.rays_d = rays->rays_d;
   C.target_s = rays->target_s; C.target_d = rays->target_d;
@@ -1192,8 +1447,23 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   for (int c = 0; c < 3; ++c) C.rgb[c] = nullptr;
   C.o_rgb = out->rgb; C.o_depth = out->depth; C.o_var = out->uncertainty; C.o_raw = out->raw;
   C.gd = nullptr; C.gc = nullptr; C.d_occ = nullptr; C.d_rgb[0] = C.d_rgb[1] = C.d_rgb[2] = nullptr;
-  k_composite<false><<<(R + 3) / 4, 128, 0, stream>>>(C);
+  C.o_w = nullptr;
+  if (m.N > 0) {  // pass 1 over the S0 samples at z1, forward only
+    DecParams D1 = D;
+    D1.P = R * m.S0; D1.S = m.S0; D1.z = L.z1; D1.masks = nullptr; D1.need_dp = 0;
+    D1.ga.grad = nullptr;
+    const int t1 = (D1.P + T - 1) / T;
+    k_coarse<false><<<t1 < sms ? t1 : sms, T, smem, stream>>>(D1, W);
+    XRD_LAUNCH_CHECK();
+    XRD_CUDA_TRY(importance(C, cfg, m, L, z, stream));
+  }
+  {
+    KernelTimer kt(stream);
+    k_coarse<false><<<gridx, T, smem, stream>>>(D, W);
+  }
   XRD_LAUNCH_CHECK();
+
+  XRD_CUDA_TRY(launch_composite<false>(C, stream));
   if (!with_grads) return XRD_OK;
 
   LossParams LP;
@@ -1206,8 +1476,7 @@ extern "C" int xrd_nice_coarse_step(const XrdRays* rays, const XrdNiceGrid* grid
   XRD_LAUNCH_CHECK();
   C.gd = LP.gd; C.gc = LP.gc;
   C.d_occ = L.d_occ;
-  k_composite<true><<<(R + 3) / 4, 128, 0, stream>>>(C);
-  XRD_LAUNCH_CHECK();
+  XRD_CUDA_TRY(launch_composite<true>(C, stream));
   XRD_CUDA_TRY(cudaMemsetAsync(L.dp, 0, 3 * (size_t)P * 4, stream));
   D.dout[0] = C.d_occ;
   XRD_CUDA_TRY(cudaFuncSetAttribute(k_coarse<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
