@@ -24,6 +24,7 @@ import torch
 
 from . import _cabi
 from ._cabi import XrdAdamTensor, XrdCoslamGrads, XrdRays, launch, ptr
+from .joint_encoding import CoarseToFine
 from .optimizers import FusedAdam, adam_desc, init_adam_state
 
 
@@ -51,58 +52,25 @@ class _ScalarRing:
         self._ev[k].record(torch.cuda.current_stream(self.dev))
 
 
-def _fused_step(sess, stream, gs, fine=False, **cfg):
-    """xrd_coslam_step over a session's rays with the seed read from its `dyn` block; `cfg`
-    gives the sharded-mapping fields of XrdCoslamCfg.  With training_n_importance > 0 this is
-    the coarse pass into sess._out_c, or with `fine` the fine pass into sess._out over the
-    z_vals and counts of _importance_step."""
+def _structs(sess):
+    """(XrdRays, XrdHashGrid, XrdCoslamMlp) of a session's rays and the model's parameters."""
     model = sess.model
-    rays = XrdRays(sess.R, ptr(sess.rays_o), ptr(sess.rays_d), ptr(sess.ts), ptr(sess.td))
-    grid = model._grid_struct(model.embed_fn.params.detach())
-    mlp = model._mlp_struct(model._weights())
-    S = model._n_samples()
-    if fine:
-        N = model.config.training_n_importance
-        cfg = dict(phase=2, n_importance=N, counts_global=sess.counts_f,
-                   n_rays_global=sess.R * sess.world)
-        S += N
-    c = model._cfg_struct(S, seed_dev=sess.dyn, **cfg)
-    launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(c), None,
-           C.byref(sess._out if fine else sess._out_c), None if gs is None else C.byref(gs),
+    return (XrdRays(sess.R, ptr(sess.rays_o), ptr(sess.rays_d), ptr(sess.ts), ptr(sess.td)),
+            model._grid_struct(model.embed_fn.params.detach()), model._mlp_struct(model._weights()))
+
+
+def _cfg(sess, **cfg):
+    """XrdCoslamCfg of a session's pass, its seed read from `dyn`; cfg: sharded-mapping fields."""
+    return sess.model._cfg_struct(sess.model._n_samples(), seed_dev=sess.dyn, **cfg)
+
+
+def _fused_step(sess, stream, gs, **cfg):
+    """xrd_coslam_step into a session's outputs (with importance sampling the coarse pass's)."""
+    rays, grid, mlp = _structs(sess)
+    out = sess.c2f._coarse if sess.c2f else sess._out
+    launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp),
+           C.byref(_cfg(sess, **cfg)), None, C.byref(out), None if gs is None else C.byref(gs),
            ptr(sess.ws), sess.ws_bytes, stream=stream)
-
-
-def _importance_setup(sess, R, S, dev):
-    """training_n_importance = N > 0: the coarse pass's outputs (sess.out_c), the importance
-    step's buffers and counts, the fine pass's outputs (sess.out, over S + N samples) and the
-    coarse pass's ray gradients.  N == 0: sess.out_c is sess.out (allocated by the caller)."""
-    model = sess.model
-    N = model.config.training_n_importance
-    f32 = dict(dtype=torch.float32, device=dev)
-    if not N:
-        sess.out_c, sess._out_c = sess.out, sess._out
-        return
-    sess.out_c, sess._out_c = model._outputs(R, S, dev)
-    sess.imp, _ = model._importance_struct(R, S, dev, sess.out_c['z_vals'], sess.out_c['raw'])
-    sess.out, sess._out = model._outputs(R, S + N, dev, z_vals=sess.imp['z_vals'])
-    sess.counts_f = torch.zeros(4, dtype=torch.int32, device=dev)
-    sess.d_rays_o_c, sess.d_rays_d_c = torch.zeros(R, 3, **f32), torch.zeros(R, 3, **f32)
-
-
-def _importance_step(sess, stream):
-    """xrd_coslam_importance between the coarse and the fine pass, u drawn from the seed in
-    the session's `dyn` block (a fresh draw every replay)."""
-    model = sess.model
-    _, q = model._importance_struct(sess.R, model._n_samples(), sess.dev, sess.out_c['z_vals'],
-                                    sess.out_c['raw'], sess.td, seed_dev=sess.dyn,
-                                    counts=sess.counts_f, bufs=sess.imp)
-    launch('xrd_coslam_importance', C.byref(q), stream=stream)
-
-
-def _coarse_scale(sess):
-    """Per-term loss scales of the coarse pass: with importance sampling only its rgb and depth
-    terms count (joint_encoding.py:118-121)."""
-    return (1.0, 1.0, 0.0, 0.0) if sess.model.config.training_n_importance else (1.0,) * 4
 
 
 class MappingGraphSession:
@@ -127,13 +95,18 @@ class MappingGraphSession:
         # outputs before the workspaces and the gradient bucket: allocated after them, the
         # captured iteration measured ~0.4 % slower on an H100 80GB HBM3 at 700 W
         N = self.N = cfg.training_n_importance
+        self.c2f = None
         if not N:
             self.out, self._out = model._outputs(R, S, dev)
         # with importance sampling the coarse and the fine pass share the fine pass's workspace
         self.ws, self.ws_bytes = _cabi.workspace(dev, 'coslam', R, S + N)
         self.ws_s, self.ws_s_bytes = _cabi.workspace(dev, 'coslam_smoothness',
                                                      cfg.trainging_smooth_pts)
-        _importance_setup(self, R, S, dev)
+        if N:
+            ws = (self.ws, self.ws_bytes)
+            d_rays = (self.d_rays_o, self.d_rays_d) if bundle_adjust else (None, None)
+            self.c2f = CoarseToFine(model, R, S, dev, ws, ws, self._grads, d_rays)
+            self.out, self._out = self.c2f.fine, self.c2f._fine
         # per-iteration scalars: [seed u64 | smooth_rand f32 x6 | (lr, bc1, bc2) per group (<= 3)]
         self._scalars = _ScalarRing(128, dev)
         self.dyn = self._scalars.dyn
@@ -222,36 +195,24 @@ class MappingGraphSession:
                               ptr(d_rays_d) if self.ba else None, (C.c_float * 4)(*scale),
                               ptr(G[self.table_c]) if self.table_c is not None else None)
 
+    def _sharded(self):
+        """XrdCoslamCfg fields of a pass over a sharded batch"""
+        return {} if self.world == 1 else dict(phase=2, n_rays_global=self.R * self.world,
+                                               counts_global=self.counts)
+
     def _part_b(self, stream, smooth=True, pose=True):
         """fused forward / loss / backward (+ smoothness, pose-gradient reduction); with
-        importance sampling the coarse pass, the importance step, the counts all-reduce when
-        sharded, and the fine pass."""
-        self._part_b_coarse(stream)
+        importance sampling both passes of self.c2f, the fine counts all-reduced when sharded."""
         if self.N:
-            if self.world > 1:
-                self.dp.all_reduce_sum(self.counts_f)  # the fine pass's loss normalisers (Q9)
-            self._part_b_fine(stream)
+            self.c2f.run(stream, _structs(self), _cfg(self, **self._sharded()), self.td,
+                         reduce=self.dp.all_reduce_sum if self.world > 1 else None)
+        else:
+            _fused_step(self, stream, self._grads(self.d_rays_o, self.d_rays_d, (1.0,) * 4),
+                        **self._sharded())
         if smooth:
             self._part_smooth(stream)
         if pose:
             self._part_pose(stream)
-
-    def _part_b_coarse(self, stream):
-        sharded = dict(phase=2, n_rays_global=self.R * self.world, counts_global=self.counts)
-        d_rays = (self.d_rays_o_c, self.d_rays_d_c) if self.N else (self.d_rays_o, self.d_rays_d)
-        _fused_step(self, stream, self._grads(*d_rays, _coarse_scale(self)),
-                    **(sharded if self.world > 1 else {}))
-        if self.N:
-            _importance_step(self, stream)
-
-    def _part_b_fine(self, stream):
-        """the fine pass; its loss terms and ray gradients take the coarse pass's in"""
-        _fused_step(self, stream, self._grads(self.d_rays_o, self.d_rays_d, (1.0,) * 4),
-                    fine=True)
-        self.losses[:2] += self.out_c['losses'][:2]
-        if self.ba:
-            self.d_rays_o += self.d_rays_o_c
-            self.d_rays_d += self.d_rays_d_c
 
     def _part_smooth(self, stream):
         """Smoothness / TV term into the same table-gradient buffer (red.add, order-free).
@@ -366,10 +327,11 @@ class MappingGraphSession:
                 parts = [self._part_a, self._part_b, lambda st: self._part_c(st, with_adam=True)]
                 self._reduces = [self.counts, self.flat]  # all-reduced after graphs 0, 1
                 if self.N:  # the fine pass's counts: one more segment boundary
-                    parts[1:2] = [self._part_b_coarse,
-                                  lambda st: (self._part_b_fine(st), self._part_smooth(st),
-                                              self._part_pose(st))]
-                    self._reduces.insert(1, self.counts_f)
+                    parts[1:2] = [lambda st: self.c2f.coarse_pass(
+                                      st, _structs(self), _cfg(self, **self._sharded()), self.td),
+                                  lambda st: (self.c2f.fine_pass(st, _structs(self)),
+                                              self._part_smooth(st), self._part_pose(st))]
+                    self._reduces.insert(1, self.c2f.counts)
                 for part in parts:
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g, pool=pool, capture_error_mode='relaxed'):
@@ -383,8 +345,7 @@ class MappingGraphSession:
         """Drop the captured graphs and every device buffer of this session."""
         self.graphs = []
         for k in ('flat', 'grads', 'out', 'ws', 'ws_s', 'rows', 'ids', 'rays_o', 'rays_d',
-                  'd_rays_o', 'd_rays_d', 'dirs', 'ts', 'td', 'out_c', 'imp', 'd_rays_o_c',
-                  'd_rays_d_c'):
+                  'd_rays_o', 'd_rays_d', 'dirs', 'ts', 'td', 'c2f'):
             self.__dict__.pop(k, None)
 
     # ------------------------------------------------------------------ running ---
@@ -538,12 +499,16 @@ class TrackingGraphSession:
         self.best_rot, self.best_trans = z(1, 3), z(1, 3)
         self.rays_o, self.rays_d = z(R, 3), z(R, 3)
         self.d_rays_o, self.d_rays_d = z(R, 3), z(R, 3)
-        self.N, self.world = cfg.training_n_importance, 1
+        self.N, self.c2f = cfg.training_n_importance, None
         if not self.N:
             self.out, self._out = model._outputs(R, S, dev)
-        _importance_setup(self, R, S, dev)
-        self.losses = self.out['losses']
         self.ws, self.ws_bytes = _cabi.workspace(dev, 'coslam', R, S + self.N)
+        if self.N:
+            ws = (self.ws, self.ws_bytes)
+            self.c2f = CoarseToFine(model, R, S, dev, ws, ws, self._grads,
+                                    (self.d_rays_o, self.d_rays_d))
+            self.out, self._out = self.c2f.fine, self.c2f._fine
+        self.losses = self.out['losses']
         # per-iteration scalars: [seed u64 | pad | (lr, bc1, bc2) rot | (lr, bc1, bc2) trans]
         self._scalars = _ScalarRing(64, dev)
         self.dyn = self._scalars.dyn
@@ -574,20 +539,10 @@ class TrackingGraphSession:
                stream=stream)
         launch('xrd_rays_from_poses', R, ptr(self.dirs), None, ptr(self.poses), 1,
                ptr(self.rays_o), ptr(self.rays_d), stream=stream)
-        def pose_only(d_rays_o, d_rays_d, scale):
-            return XrdCoslamGrads(None, None, None, None, None, ptr(d_rays_o), ptr(d_rays_d),
-                                  (C.c_float * 4)(*scale))
-        if self.N:  # coarse pass, importance step, fine pass; the two passes' terms add up
-            _fused_step(self, stream, pose_only(self.d_rays_o_c, self.d_rays_d_c,
-                                                _coarse_scale(self)))
-            _importance_step(self, stream)
-            _fused_step(self, stream, pose_only(self.d_rays_o, self.d_rays_d, (1.0,) * 4),
-                        fine=True)
-            self.losses[:2] += self.out_c['losses'][:2]
-            self.d_rays_o += self.d_rays_o_c
-            self.d_rays_d += self.d_rays_d_c
+        if self.N:
+            self.c2f.run(stream, _structs(self), _cfg(self), self.td)
         else:
-            _fused_step(self, stream, pose_only(self.d_rays_o, self.d_rays_d, (1.0,) * 4))
+            _fused_step(self, stream, self._grads(self.d_rays_o, self.d_rays_d, (1.0,) * 4))
         launch('xrd_rays_pose_grads', R, ptr(self.dirs), None, 1, ptr(self.d_rays_o),
                ptr(self.d_rays_d), ptr(self.d_poses), stream=stream)
         self.d_rot.zero_()
@@ -610,6 +565,11 @@ class TrackingGraphSession:
                                    getattr(oo, 'weight_decay', 0),
                                    dyn=None if warm else self.dyn.data_ptr() + 16 + 12 * k))
         launch('xrd_adam_step', (XrdAdamTensor * 2)(*descs), 2, 0, stream=stream)
+
+    @staticmethod
+    def _grads(d_rays_o, d_rays_d, scale):  # pose only
+        return XrdCoslamGrads(None, None, None, None, None, ptr(d_rays_o), ptr(d_rays_d),
+                              (C.c_float * 4)(*scale))
 
     def begin(self, frame):
         self.depth_img.copy_(self.algo._frame_tensor(frame, 'depth'))

@@ -39,6 +39,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "sample_pdf.cuh"
 
 namespace xrd {
 namespace coslam {
@@ -2019,14 +2020,10 @@ static int fill_grid(GridDev& g, const XrdHashGrid* h) {
 }
 
 // -------------------------------------------------------------- importance ---
-// Hierarchical sampling between the coarse and the fine pass (joint_encoding.py:301-315 and
-// sample_pdf, slam/model_components/utils.py:31-76), one warp per ray:
-//   the coarse pass's weights (composite_weights on its raw sdf and z_vals)
-//   -> pdf of weights[1:-1] + 1e-5 -> cdf = [0, cumsum(pdf)], the prefix sums in float64 and each
-//      rounded to float, as torch.cumsum does on float32
-//   -> inverse-cdf samples at u over the S0-1 bin midpoints
-//   -> z_fine = sort(z_vals ++ z_samples), each value written at its rank
-//   -> the fine pass's counts n_fs, n_sdf, n_valid over z_fine.
+// Hierarchical sampling between the coarse and the fine pass (joint_encoding.py:301-315), one
+// warp per ray: sample_pdf (sample_pdf.cuh) on the coarse pass's weights (composite_weights on
+// its raw sdf and z_vals, divided by their sum), z_fine = sort(z_vals ++ z_samples), the spread
+// z_std of the samples and the fine pass's counts n_fs, n_sdf, n_valid over z_fine.
 struct ImportanceParams {
   int R, S, N, det;
   float trunc, depth_trunc;
@@ -2040,17 +2037,11 @@ constexpr int kImpWarps = 4;
 // shared floats per warp: sigma / pdf, weights, cdf, bin midpoints (S each), merged values (S + N)
 __host__ __device__ constexpr int imp_floats(int S, int N) { return 4 * S + S + N; }
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 __global__ void __launch_bounds__(kImpWarps * 32) k_importance(ImportanceParams p) {
   extern __shared__ float ism[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r = blockIdx.x * kImpWarps + warp;
-  const int S = p.S, N = p.N, T = S + N, M = S - 2;  // M inner weights; bins and cdf: M + 1
+  const int S = p.S, N = p.N, T = S + N;
   float* pdf = ism + (size_t)warp * imp_floats(S, N);
   float* wu = pdf + S;
   float* cdf = wu + S;
@@ -2063,70 +2054,19 @@ __global__ void __launch_bounds__(kImpWarps * 32) k_importance(ImportanceParams 
     const float W = composite_weights<4, 0, false>(const_cast<float*>(p.raw) + (size_t)r * S * 4,
                                                    zr, S, p.trunc, pdf, wu, lane);
     __syncwarp();  // the weights other lanes wrote in composite_weights are read below
-    double part = 0.0;
-    for (int j = lane; j < M; j += 32) {
-      const float w = __fadd_rn(wu[j + 1] / W, 1e-5f);
-      pdf[j] = w;
-      part += (double)w;
+    pdf_cdf([&](int j) { return wu[j] / W; }, zr, S, pdf, cdf, mid, zall, lane);
+    const PdfDraw draw{p.u, p.lin_u, p.det, p.seed_dev ? *p.seed_dev : p.seed};
+    invert_cdf(draw, r, S, N, cdf, mid, zall, p.z_samples ? p.z_samples + (size_t)r * N : nullptr,
+               lane);
+    rank_merge(zall, T, p.z_fine + (size_t)r * T, lane);
+    if (p.counts) {
+      const float d = p.target_d[r];
+      for (int e = lane; e < T; e += 32) count_sample(zall[e], d, p.trunc, c_fs, c_sdf);
+      if (lane == 0) c_valid = (d > 0.f && d < p.depth_trunc);
     }
-    const float sum = (float)warp_sum_d(part);
-    for (int j = lane; j < S - 1; j += 32) mid[j] = __fmul_rn(0.5f, __fadd_rn(zr[j + 1], zr[j]));
-    for (int k = lane; k < S; k += 32) zall[k] = zr[k];
-    __syncwarp();
-    // cdf: lane owns the contiguous run [j0, j1) of the pdf; exclusive scan of the run totals
-    const int C = (M + 31) / 32, j0 = min(M, lane * C), j1 = min(M, j0 + C);
-    double run = 0.0;
-    for (int j = j0; j < j1; ++j) {
-      const float q = __fdiv_rn(pdf[j], sum);
-      pdf[j] = q;
-      run += (double)q;
-    }
-    double pre = run;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const double v = __shfl_up_sync(0xffffffffu, pre, o);
-      if (lane >= o) pre += v;
-    }
-    pre -= run;
-    for (int j = j0; j < j1; ++j) {
-      pre += (double)pdf[j];
-      cdf[j + 1] = (float)pre;
-    }
-    if (lane == 0) cdf[0] = 0.f;
-    __syncwarp();
-    const uint64_t seed = p.seed_dev ? *p.seed_dev : p.seed;
-    double zsum = 0.0;
-    for (int j = lane; j < N; j += 32) {
-      float u;
-      if (p.u) {
-        u = p.u[(size_t)r * N + j];
-      } else if (p.det) {
-        u = p.lin_u[j];
-      } else {
-        // counters above 2^63: disjoint from the coarse pass's jitter stream (k_sample)
-        float q[4];
-        philox4(seed, (1ull << 63) | ((uint64_t)r * N + j), q);
-        u = q[0];
-      }
-      // searchsorted(cdf, u, right=True): the first index whose cdf exceeds u, in [0, M + 1]
-      int lo = 0, hi = M + 1;
-      while (lo < hi) {
-        const int m = (lo + hi) >> 1;
-        if (cdf[m] <= u) lo = m + 1; else hi = m;
-      }
-      const int below = max(lo - 1, 0), above = min(lo, M);
-      const float c0 = cdf[below];
-      float den = __fsub_rn(cdf[above], c0);
-      if (den < 1e-5f) den = 1.f;
-      const float t = __fdiv_rn(__fsub_rn(u, c0), den);
-      const float b0 = mid[below];
-      const float z = __fadd_rn(b0, __fmul_rn(t, __fsub_rn(mid[above], b0)));
-      zall[S + j] = z;
-      zsum += (double)z;
-      if (p.z_samples) p.z_samples[(size_t)r * N + j] = z;
-    }
-    __syncwarp();
     if (p.z_std) {  // std(z_samples, unbiased=False), two passes in float64
+      double zsum = 0.0;
+      for (int j = lane; j < N; j += 32) zsum += (double)zall[S + j];
       const double mean = warp_sum_d(zsum) / N;
       double v = 0.0;
       for (int j = lane; j < N; j += 32) {
@@ -2136,18 +2076,6 @@ __global__ void __launch_bounds__(kImpWarps * 32) k_importance(ImportanceParams 
       v = warp_sum_d(v);
       if (lane == 0) p.z_std[r] = (float)sqrt(v / N);
     }
-    const float d = p.counts ? p.target_d[r] : 0.f;
-    for (int e = lane; e < T; e += 32) {
-      const float v = zall[e];
-      int rank = 0;
-      for (int q = 0; q < T; ++q) {
-        const float w = zall[q];
-        rank += (w < v) || (w == v && q < e);
-      }
-      p.z_fine[(size_t)r * T + rank] = v;
-      if (p.counts) count_sample(v, d, p.trunc, c_fs, c_sdf);
-    }
-    if (p.counts && lane == 0) c_valid = (d > 0.f && d < p.depth_trunc);
   }
   if (p.counts) add_counts(p.counts, c_fs, c_sdf, c_valid, lane);
 }

@@ -33,6 +33,7 @@
 
 #include "mlp.cuh"
 #include "nice.cuh"
+#include "sample_pdf.cuh"
 
 namespace xrd {
 namespace nice {
@@ -845,17 +846,9 @@ static cudaError_t launch_composite(const CompParams& C, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------- sample_pdf ---
-// Importance samples of pass 2 (conv_onet.py:498-506 with sample_pdf,
-// slam/model_components/utils.py:31-76), one warp per ray:
-//   pdf = (w[1:-1] + 1e-5) / sum, w = pass 1's composite weights (k_composite<.., WEIGHTS>)
-//   cdf = [0, cumsum(pdf)]: the prefix sums in float64 and each rounded to float, as
-//         torch.cumsum does on float32
-//   bins = .5 (z[1:] + z[:-1]) in float64; searchsorted(cdf, u, right=True), the below / above
-//         clamps, denom < 1e-5 -> 1, z = bins[below] + t (bins[above] - bins[below]) in float64
-//   z_out = sort(z ++ samples), each value written at its rank.
-// The cdf and the inversion are the arithmetic of Co-SLAM's k_importance (coslam.cu) with
-// float64 bins.  That kernel keeps its own copy: moving its code into shared device functions
-// changed its SASS (the instruction schedule, same length) under CUDA 12.9.
+// Importance samples of pass 2 (conv_onet.py:498-506), one warp per ray: sample_pdf
+// (sample_pdf.cuh, shared with Co-SLAM's k_importance) with float64 bins and samples on pass 1's
+// composite weights (k_composite<.., WEIGHTS>), z_out = sort(z ++ samples).
 struct PdfParams {
   int R, S, N;        // S: pass 1's samples per ray, N: importance samples per ray
   const float* w;     // [R][S] pass 1's weights
@@ -869,93 +862,19 @@ struct PdfParams {
 };
 constexpr int kPdfS = 64, kPdfT = 128;  // limits of pass 1 and of the merge
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 static __global__ void __launch_bounds__(128) k_sample_pdf(const PdfParams p) {
   __shared__ float s_pdf[4][kPdfS], s_cdf[4][kPdfS];
   __shared__ double s_bins[4][kPdfS], s_z[4][kPdfT];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r = blockIdx.x * 4 + warp;
   if (r >= p.R) return;  // warp-uniform
-  const int S = p.S, N = p.N, T = S + N, M = S - 2;  // M inner weights; bins and cdf: M + 1
-  float* pdf = s_pdf[warp];
-  float* cdf = s_cdf[warp];
-  double* bins = s_bins[warp];
-  double* zall = s_z[warp];
+  const int S = p.S, N = p.N;
   const float* wr = p.w + (size_t)r * S;
-  const double* zr = p.z + (size_t)r * S;
-  double part = 0.0;
-  for (int j = lane; j < M; j += 32) {
-    const float w = __fadd_rn(wr[j + 1], 1e-5f);
-    pdf[j] = w;
-    part += (double)w;
-  }
-  const float sum = (float)warp_sum_d(part);
-  for (int j = lane; j < S - 1; j += 32) bins[j] = __dmul_rn(0.5, __dadd_rn(zr[j + 1], zr[j]));
-  for (int k = lane; k < S; k += 32) zall[k] = zr[k];
-  __syncwarp();
-  // cdf: lane owns the contiguous run [j0, j1) of the pdf; exclusive scan of the run totals
-  const int C = (M + 31) / 32, j0 = min(M, lane * C), j1 = min(M, j0 + C);
-  double run = 0.0;
-  for (int j = j0; j < j1; ++j) {
-    const float q = __fdiv_rn(pdf[j], sum);
-    pdf[j] = q;
-    run += (double)q;
-  }
-  double pre = run;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const double v = __shfl_up_sync(0xffffffffu, pre, o);
-    if (lane >= o) pre += v;
-  }
-  pre -= run;
-  for (int j = j0; j < j1; ++j) {
-    pre += (double)pdf[j];
-    cdf[j + 1] = (float)pre;
-  }
-  if (lane == 0) cdf[0] = 0.f;
-  __syncwarp();
-  for (int j = lane; j < N; j += 32) {
-    float u;
-    if (p.u) {
-      u = p.u[(size_t)r * N + j];
-    } else if (p.det) {
-      u = p.lin_u[j];
-    } else {
-      // counters above 2^63: disjoint from the jitter's stream (k_sample)
-      float q[4];
-      philox4(p.seed, (1ull << 63) | ((uint64_t)r * N + j), q);
-      u = q[0];
-    }
-    // searchsorted(cdf, u, right=True): the first index whose cdf exceeds u, in [0, M + 1]
-    int lo = 0, hi = M + 1;
-    while (lo < hi) {
-      const int m = (lo + hi) >> 1;
-      if (cdf[m] <= u) lo = m + 1; else hi = m;
-    }
-    const int below = max(lo - 1, 0), above = min(lo, M);
-    const float c0 = cdf[below];
-    float den = __fsub_rn(cdf[above], c0);
-    if (den < 1e-5f) den = 1.f;
-    const float t = __fdiv_rn(__fsub_rn(u, c0), den);
-    const double b0 = bins[below];
-    zall[S + j] = __dadd_rn(b0, __dmul_rn((double)t, __dsub_rn(bins[above], b0)));
-    if (p.z_samples) p.z_samples[(size_t)r * N + j] = zall[S + j];
-  }
-  __syncwarp();
-  for (int e = lane; e < T; e += 32) {
-    const double v = zall[e];
-    int rank = 0;
-    for (int q = 0; q < T; ++q) {
-      const double x = zall[q];
-      rank += (x < v) || (x == v && q < e);
-    }
-    p.z_out[(size_t)r * T + rank] = v;
-  }
+  pdf_cdf([&](int j) { return wr[j]; }, p.z + (size_t)r * S, S, s_pdf[warp], s_cdf[warp],
+          s_bins[warp], s_z[warp], lane);
+  invert_cdf(PdfDraw{p.u, p.lin_u, p.det, p.seed}, r, S, N, s_cdf[warp], s_bins[warp], s_z[warp],
+             p.z_samples ? p.z_samples + (size_t)r * N : nullptr, lane);
+  rank_merge(s_z[warp], S + N, p.z_out + (size_t)r * (S + N), lane);
 }
 
 // ------------------------------------------------------------------ loss ---

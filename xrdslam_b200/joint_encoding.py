@@ -195,6 +195,65 @@ class _CoslamStep(torch.autograd.Function):
                 grads['d_w_col1'], None, None, None, None, grads['d_table_color'], None)
 
 
+class CoarseToFine:
+    """A step with training_n_importance = N > 0 (joint_encoding.py:301-341): the coarse pass
+    over S samples per ray (its rgb and depth terms alone count), xrd_coslam_importance, the fine
+    pass over the S + N merged samples, which takes the coarse pass's terms and ray gradients in.
+    Owns both passes' outputs, the importance buffers, the fine counts and the coarse ray
+    gradients.  ws, ws_fine: (buffer, bytes); grads(d_rays_o, d_rays_d, loss_scale) -> the
+    caller's XrdCoslamGrads (None: forward only); d_rays: the caller's ray-gradient buffers;
+    structs: the step's (XrdRays, XrdHashGrid, XrdCoslamMlp)."""
+
+    def __init__(self, model, R, S, dev, ws, ws_fine, grads=None, d_rays=(None, None),
+                 loss_scale=(1.0,) * 4):
+        self.model, self.R, self.S, self.N = model, R, S, model.config.training_n_importance
+        self.dev, self.ws, self.ws_fine, self.grads, self.d_rays = dev, ws, ws_fine, grads, d_rays
+        self.loss_scale = list(loss_scale)
+        self.coarse, self._coarse = model._outputs(R, S, dev)
+        self.imp, _ = model._importance_struct(R, S, dev, self.coarse['z_vals'], self.coarse['raw'])
+        self.fine, self._fine = model._outputs(R, S + self.N, dev, z_vals=self.imp['z_vals'])
+        self.counts = torch.zeros(4, dtype=torch.int32, device=dev)
+        self.d_rays_c = [d if d is None else torch.zeros_like(d) for d in d_rays]
+
+    def run(self, stream, structs, cfg, td, noise=None, u=None, reduce=None):
+        """coarse_pass(), reduce(counts) (the all-reduce of a sharded batch), fine_pass()."""
+        self.coarse_pass(stream, structs, cfg, td, noise, u)
+        if reduce is not None:
+            reduce(self.counts)
+        self.fine_pass(stream, structs)
+
+    def coarse_pass(self, stream, structs, cfg, td, noise=None, u=None):
+        """The coarse pass (XrdCoslamCfg `cfg`), then the importance step: uniforms u [R,N], else
+        drawn from cfg's seed; with the depth targets td it counts the fine pass's normalisers."""
+        self._cfg, self._counts = cfg, self.counts if td is not None else None
+        self._step(stream, structs, cfg, noise, self._coarse, self.loss_scale[:2] + [0.0, 0.0],
+                   self.d_rays_c, self.ws)
+        _, q = self.model._importance_struct(self.R, self.S, self.dev, self.coarse['z_vals'],
+                                             self.coarse['raw'], td, u, seed=cfg.seed,
+                                             counts=self._counts, bufs=self.imp)
+        q.seed_dev = cfg.seed_dev
+        _cabi.launch('xrd_coslam_importance', C.byref(q), stream=stream)
+
+    def fine_pass(self, stream, structs):
+        """The fine pass, then the coarse pass's rgb and depth terms and ray gradients added in."""
+        c = XrdCoslamCfg.from_buffer_copy(self._cfg)
+        c.n_samples, c.phase, c.n_importance = self.S + self.N, 2, self.N
+        c.counts_out, c.counts_global = None, ptr(self._counts)
+        self._step(stream, structs, c, None, self._fine, self.loss_scale, self.d_rays, self.ws_fine)
+        if self.grads is not None:
+            self.fine['losses'][:2] += self.coarse['losses'][:2]
+        for d, d_c in zip(self.d_rays, self.d_rays_c):
+            if d is not None:
+                d += d_c
+
+    def _step(self, stream, structs, cfg, noise, out, loss_scale, d_rays, ws):
+        gs = self.grads(*d_rays, loss_scale) if self.grads else None
+        rays, grid, mlp = structs
+        _cabi.launch('xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp), C.byref(cfg),
+                     ptr(noise), C.byref(out), None if gs is None else C.byref(gs), ptr(ws[0]),
+                     ws[1], stream=stream)
+
+
 class JointEncoding(Model):
     """Model class (slam/models/joint_encoding.py:69-531)."""
 
@@ -437,7 +496,6 @@ class JointEncoding(Model):
         if importance_u is not None:
             importance_u = importance_u.detach().to(**f32).contiguous()
             assert importance_u.shape == (R, N)
-        o, out = self._outputs(R, S, dev)
         rays = XrdRays(R, ptr(rays_o), ptr(rays_d), ptr(ts), ptr(td))
         grid = self._grid_struct(table.detach())
         mlp = self._mlp_struct((w0, w1, wc0, wc1), table_c)
@@ -447,8 +505,7 @@ class JointEncoding(Model):
         dp = self.dp if (self.dp is not None and self.dp.world > 1 and with_grads
                          and map_grads) else None
         c = self._cfg_struct(S, seed=seed)
-        g = None
-        gs = None
+        g = grads = None
         if with_grads:
             if not has_d or ts is None:
                 raise RuntimeError('gradients need target_s and target_d')
@@ -462,14 +519,16 @@ class JointEncoding(Model):
                      d_rays_d=torch.empty(R, 3, **f32) if need_ray_grads else None,
                      d_table_color=z(table_c, **f32) if (map_grads and table_c is not None)
                      else None)
-            sc = list(loss_scale or [1.0, 1.0, 1.0, 1.0])
-            # with importance sampling the coarse pass adds its rgb and depth terms only
-            gs = self._grads_struct(g, sc[:2] + [0.0, 0.0] if N else sc)
-        ws, ws_bytes = _cabi.workspace(dev, 'coslam', R, S)
+            grads = lambda d_o, d_d, sc: self._grads_struct(dict(g, d_rays_o=d_o, d_rays_d=d_d), sc)
+        sc = list(loss_scale or [1.0, 1.0, 1.0, 1.0])
+        ws = _cabi.workspace(dev, 'coslam', R, S)
+        c2f = CoarseToFine(self, R, S, dev, ws, _cabi.workspace(dev, 'coslam', R, S + N), grads,
+                           (g['d_rays_o'], g['d_rays_d']) if g else (None, None), sc) if N else None
+        o, out = (c2f.coarse, c2f._coarse) if N else self._outputs(R, S, dev)
 
-        def step(grads, c=c, out=out, ws=ws, ws_bytes=ws_bytes, noise=noise):
+        def step(gs):
             _cabi.launch_on(dev, 'xrd_coslam_step', C.byref(rays), C.byref(grid), C.byref(mlp),
-                            C.byref(c), ptr(noise), C.byref(out), grads, ptr(ws), ws_bytes)
+                            C.byref(c), ptr(noise), C.byref(out), gs, ptr(ws[0]), ws[1])
         if dp is not None:
             # sharded mapping: the loss normalisers are batch-global (SURVEY Q9):
             # sample -> all-reduce the three counters -> render with the global counts
@@ -479,38 +538,16 @@ class JointEncoding(Model):
             dp.all_reduce_sum(counts)
             c.phase, c.counts_global = 2, ptr(counts)
             c.n_rays_global = R * dp.world  # equal shards
-        step(C.byref(gs) if gs is not None else None)
         self._last_seed = seed
         if not N:
+            step(C.byref(self._grads_struct(g, sc)) if g is not None else None)
             return o, g
         # importance sampling -> the fine pass over S + N samples (phase 2, its own counts)
-        counts = torch.zeros(4, dtype=torch.int32, device=dev) if has_d else None
-        b, q = self._importance_struct(R, S, dev, o['z_vals'], o['raw'], td, importance_u,
-                                       seed=seed, counts=counts)
-        _cabi.launch_on(dev, 'xrd_coslam_importance', C.byref(q))
-        if dp is not None:
-            dp.all_reduce_sum(counts)
-        of, outf = self._outputs(R, S + N, dev, z_vals=b['z_vals'])
-        cf = self._cfg_struct(S + N, seed=seed, phase=2, counts_global=counts, n_importance=N,
-                              n_rays_global=R * dp.world if dp is not None else 0)
-        gsf = None
-        if g is not None:
-            gf = dict(g, d_rays_o=None, d_rays_d=None)
-            if need_ray_grads:
-                gf['d_rays_o'], gf['d_rays_d'] = torch.empty_like(g['d_rays_o']), torch.empty_like(
-                    g['d_rays_d'])
-            gsf = self._grads_struct(gf, sc)
-        wsf, wsf_bytes = _cabi.workspace(dev, 'coslam', R, S + N)
-        step(C.byref(gsf) if gsf is not None else None, c=cf, out=outf, ws=wsf,
-             ws_bytes=wsf_bytes, noise=None)
-        if g is not None:
-            of['losses'][:2] += o['losses'][:2]
-            if need_ray_grads:
-                g['d_rays_o'] += gf['d_rays_o']
-                g['d_rays_d'] += gf['d_rays_d']
-        of.update(rgb0=o['rgb'], disp0=o['disp_map'], acc0=o['acc_map'], depth0=o['depth'],
-                  depth_var0=o['depth_var'], z_std=b['z_std'])
-        return of, g
+        with torch.cuda.device(dev):
+            c2f.run(torch.cuda.current_stream(dev).cuda_stream, (rays, grid, mlp), c, td, noise,
+                    importance_u, dp.all_reduce_sum if dp is not None else None)
+        return dict(c2f.fine, rgb0=o['rgb'], disp0=o['disp_map'], acc0=o['acc_map'],
+                    depth0=o['depth'], depth_var0=o['depth_var'], z_std=c2f.imp['z_std']), g
 
     @staticmethod
     def _grads_struct(g, scale):
